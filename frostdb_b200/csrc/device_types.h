@@ -205,7 +205,7 @@ struct SeedJob {
   uint32_t n_runs, total, n_chunks, is_def;
 };
 
-// ---- sorted-run scan (k_runs): the plan shape of compacted parts ---------------------------------------
+// ---- sorted-run scan (k_runs_tma): the plan shape of compacted parts -----------------------------------
 // Row groups whose filter columns and aggregate inputs are PLAIN non-null int64 and whose group-key
 // columns are run-length only (sorted parts) are scanned by a dedicated kernel that walks the key run
 // directories with warp-uniform cursors.  The host lists those row groups here; the rest of the table
@@ -216,11 +216,19 @@ constexpr int kRtConsumerWarps = 8;                         // k_runs_tma: consu
 constexpr int kRtMaxThreads = (kRtConsumerWarps + 1) * 32;  // + one producer warp
 constexpr int kRtDirMax = 128;                              // most directory entries staged per cursor column and tile
 
+// Staged column c of a row group: uint{8,16,32,64}(value - base) per row, 1 << lg bytes each (a frame-of-reference
+// image, or the 8-byte PLAIN values with base 0), at byte soff of the stage's column region.  A decided leaf's column
+// in a row group that is not all_pass is not staged (RunsRg::col[c] null): it takes a staged column's entry (stand-in).
+struct alignas(16) RunsCol {
+  uint32_t soff, lg;
+  long long base;
+};
+
 struct RunsRg {
   uint32_t n_rows;
   uint32_t all_pass;  // 1: the chunk statistics decided every leaf (all rows pass); the leaf columns are not staged
   long long lo[kRunsLeaves], hi[kRunsLeaves];  // inclusive bounds of the (fused) range leaves for this row group
-  const uint8_t* col[kRunsCols];               // the staged PLAIN columns (distinct leaf and aggregate inputs)
+  const uint8_t* col[kRunsCols];               // the staged columns (distinct leaf and aggregate inputs): image or values
   const Run* runs[kRunsKeys];                  // run directory of every group-key column (dictionary ids premapped)
   const Seed* seeds[kRunsKeys];                // cursor seeds, one per kIndexRows rows
   // dictionary leaves (== / != / contains / regex on a run-length column): row-space directory + seeds of the
@@ -230,10 +238,10 @@ struct RunsRg {
   const uint8_t* pred_lut[kRunsPreds];
   uint32_t n_runs[kRunsKeys];                  // entries of every key directory (the sentinel not counted)
   uint32_t pred_n_runs[kRunsPreds];
-  uint32_t tile_rows;                          // k_runs_tma: rows per tile in this row group (fewer when more columns are staged)
-  uint8_t col_pos[8];                          // k_runs_tma: place of col[c] among the row group's staged (non-null) columns
+  uint32_t tile_rows;                          // rows per tile in this row group (about 32 KB of staged column data)
+  RunsCol cl[kRunsCols];                       // layout of every staged column (copied into each stage header)
 };
-static_assert(kRunsCols <= 8 && (kRunsKeys + kRunsPreds + 1) % 2 == 0, "RunsRg layout");
+static_assert(sizeof(RunsRg) % 16 == 0, "RunsRg::cl is copied with TMA");
 
 struct RunsDesc {
   uint32_t n_rg, n_spans;
@@ -347,6 +355,17 @@ struct FlatJob {
   uint32_t first_block;  // prefix over the jobs of one launch: 128-row blocks before this job
   uint32_t _pad;
 };
+
+// One PLAIN non-null int64 column chunk to restage as a frame-of-reference image (k_chunk_minmax, then k_narrow).
+struct NarrowJob {
+  const long long* src;  // resident values
+  uint8_t* out;          // k_narrow: uint{8,16,32}(v - base) per row, 128-byte aligned, padded
+  long long base;        // k_narrow: the chunk minimum
+  uint32_t n_rows, w;    // rows; k_narrow: bytes per row
+  uint32_t first_block;  // prefix over the jobs of one launch: kNarrowRows-row blocks before this job
+  uint32_t _pad;
+};
+constexpr uint32_t kNarrowRows = 4096;
 
 constexpr int kMaxRanks = 16;  // GPUs of one node exchanging partial tables (comm.cu)
 

@@ -242,8 +242,7 @@ extern "C" char** environ;
 const std::string& env_switches() {
   static const char* const kNames[] = {"FROSTGPU_NO_TILE", "FROSTGPU_NO_RUNS", "FROSTGPU_NO_PRUNE", "FROSTGPU_NO_FAST", "FROSTGPU_NO_FUSE",
                                        "FROSTGPU_NO_TAKE", "FROSTGPU_TA_TILE", "FROSTGPU_TA_STAGES", "FROSTGPU_TA_GLOBAL", "FROSTGPU_TA_CHUNK", "FROSTGPU_TA_CARRY",
-                                       "FROSTGPU_VL", "FROSTGPU_RING", "FROSTGPU_RUNS_BR", "FROSTGPU_RUNS_RING", "FROSTGPU_RUNS_SPAN",
-                                       "FROSTGPU_RUNS_V1", "FROSTGPU_RT_TILE", "FROSTGPU_RT_STAGES", "FROSTGPU_RT_SPAN", "FROSTGPU_RT_WARPS",
+                                       "FROSTGPU_VL", "FROSTGPU_RING", "FROSTGPU_RT_TILE", "FROSTGPU_RT_STAGES", "FROSTGPU_RT_SPAN", "FROSTGPU_RT_WARPS",
                                        "FROSTGPU_NO_EXEC_CACHE", "FROSTGPU_NO_PLAN_CACHE", "FROSTGPU_PROFILE"};
   static std::mutex mu;
   static std::string cached;
@@ -537,6 +536,106 @@ int32_t ensure_flat(fgpu_ctx* ctx, Part* part, const std::string& column) {
   return FGPU_OK;
 }
 
+// Frame-of-reference images of PLAIN non-null INT64 columns for the sorted-run kernel: for every resident chunk of every
+// listed (part, column) whose range max - min fits 32 bits, one image of uint{8,16,32}(value - min) per row, the
+// narrowest of the three (one allocation per (part, column), kept until the part goes).  The sorted-run kernel then
+// stages 1, 2 or 4 bytes per row instead of 8.  Minimum and maximum come from the values on the device, not from the
+// footer statistics, so that a chunk without statistics narrows as well and wrong statistics cannot change a result.
+// The whole list costs one min / max launch, one synchronisation and one narrowing launch.
+int32_t ensure_narrow(fgpu_ctx* ctx, const std::vector<std::pair<Part*, std::string>>& want) {
+  struct Job {
+    ColumnImage* img;
+    ChunkHost* ch;
+  };
+  std::vector<Job> host;
+  std::vector<NarrowJob> jobs;
+  std::vector<ColumnImage*> imgs;
+  uint32_t blocks = 0;
+  for (const auto& pc : want) {
+    ColumnImage& img = pc.first->images[pc.second];
+    if (img.narrowed) continue;
+    if (!img.resident) return fail(FGPU_ERR_INVALID, "narrow image requested for a column that is not resident: " + pc.second);
+    img.narrowed = true;
+    imgs.push_back(&img);
+    for (RowGroupHost& rg : pc.first->rgs) {
+      auto it = rg.cols.find(pc.second);
+      if (it == rg.cols.end()) continue;
+      ChunkHost& ch = it->second;
+      if (!ch.error.empty() || ch.desc.kind != CK_PLAIN64 || ch.desc.has_nulls || ch.phys != PT_INT64 || rg.n_rows == 0) continue;
+      NarrowJob j{};
+      j.src = reinterpret_cast<const long long*>(ch.desc.values);
+      j.n_rows = rg.n_rows;
+      j.first_block = blocks;
+      blocks += (rg.n_rows + kNarrowRows - 1) / kNarrowRows;
+      jobs.push_back(j);
+      host.push_back({&img, &ch});
+    }
+  }
+  if (jobs.empty()) return FGPU_OK;
+  const size_t jb = jobs.size() * sizeof(NarrowJob), mmb = jobs.size() * 16;
+  std::vector<long long> mm(2 * jobs.size());
+  for (size_t i = 0; i < jobs.size(); i++) {
+    mm[2 * i] = std::numeric_limits<long long>::max();
+    mm[2 * i + 1] = std::numeric_limits<long long>::min();
+  }
+  void* tmp = nullptr;  // [jobs][min, max per job]
+  CUDA_TRY(cudaMallocAsync(&tmp, jb + mmb, ctx->stream));
+  NarrowJob* d_jobs = static_cast<NarrowJob*>(tmp);
+  long long* d_mm = reinterpret_cast<long long*>(static_cast<uint8_t*>(tmp) + jb);
+  auto upload = [&](const void* src, void* dst, size_t n) {
+    if (void* pin = ctx->arena_take(n)) {
+      std::memcpy(pin, src, n);
+      src = pin;
+    }
+    return cudaMemcpyAsync(dst, src, n, cudaMemcpyHostToDevice, ctx->stream);
+  };
+  cudaError_t e = upload(jobs.data(), d_jobs, jb);
+  if (e == cudaSuccess) e = upload(mm.data(), d_mm, mmb);
+  if (e == cudaSuccess) e = launch_chunk_minmax(d_jobs, uint32_t(jobs.size()), blocks, d_mm, ctx->stream);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(mm.data(), d_mm, mmb, cudaMemcpyDeviceToHost, ctx->stream);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+  // widths, then one image allocation per (part, column) and the narrowing pass over the chunks that fit 32 bits
+  std::map<ColumnImage*, uint64_t> bytes;
+  std::vector<uint64_t> offs(jobs.size());
+  std::vector<NarrowJob> pass2;
+  uint32_t blocks2 = 0;
+  for (size_t i = 0; i < jobs.size() && e == cudaSuccess; i++) {
+    const uint64_t range = uint64_t(mm[2 * i + 1]) - uint64_t(mm[2 * i]);
+    jobs[i].w = range <= 0xffu ? 1u : (range <= 0xffffu ? 2u : (range <= 0xffffffffu ? 4u : 0u));
+    if (!jobs[i].w) continue;  // needs 64 bits: read from the extent as before
+    jobs[i].base = mm[2 * i];
+    uint64_t& b = bytes[host[i].img];
+    offs[i] = b;
+    b += (uint64_t(jobs[i].n_rows) * jobs[i].w + 16 + 127) & ~uint64_t(127);  // 128-byte aligned, >= 16 readable pad bytes (tile copies round up to 16)
+  }
+  for (ColumnImage* img : imgs) {
+    auto it = bytes.find(img);
+    if (it == bytes.end() || e != cudaSuccess) continue;
+    e = cudaMallocAsync(&img->narrow_dev, it->second, ctx->stream);
+  }
+  for (size_t i = 0; i < jobs.size() && e == cudaSuccess; i++) {
+    if (!jobs[i].w) continue;
+    jobs[i].out = static_cast<uint8_t*>(host[i].img->narrow_dev) + offs[i];
+    jobs[i].first_block = blocks2;
+    blocks2 += (jobs[i].n_rows + kNarrowRows - 1) / kNarrowRows;
+    pass2.push_back(jobs[i]);
+  }
+  if (e == cudaSuccess && !pass2.empty()) e = upload(pass2.data(), d_jobs, pass2.size() * sizeof(NarrowJob));
+  if (e == cudaSuccess) e = launch_narrow(d_jobs, uint32_t(pass2.size()), blocks2, ctx->stream);
+  cudaFreeAsync(tmp, ctx->stream);
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    return fail(FGPU_ERR_CUDA, std::string("narrow images: ") + cudaGetErrorString(e));
+  }
+  for (size_t i = 0; i < jobs.size(); i++) {
+    if (!jobs[i].w) continue;
+    host[i].ch->narrow = jobs[i].out;
+    host[i].ch->narrow_w = uint8_t(jobs[i].w);
+    host[i].ch->narrow_base = jobs[i].base;
+  }
+  return FGPU_OK;
+}
+
 // After the stream has been synchronised the host staging of uploaded columns can go.
 void release_staging(fgpu_ctx* ctx) {
   ctx->arena_used = 0;
@@ -551,6 +650,7 @@ void free_part(fgpu_ctx* ctx, Part* p) {
   for (auto& kv : p->images) {
     if (kv.second.dev) cudaFreeAsync(kv.second.dev, ctx->stream);
     if (kv.second.flat_dev) cudaFreeAsync(kv.second.flat_dev, ctx->stream);
+    if (kv.second.narrow_dev) cudaFreeAsync(kv.second.narrow_dev, ctx->stream);
   }
 }
 
@@ -671,7 +771,7 @@ struct ExecCache {
   bool ready = false;
   QueryDesc qd{};
   const QueryDesc* qdesc_dev = nullptr;
-  bool has_runs = false, has_ta = false, runs_v1 = false;
+  bool has_runs = false, has_ta = false;
   RunsDesc rd{};
   int runs_nl = 0, runs_nk = 0, runs_na = 0;
   TileAggDesc td{};
@@ -1643,8 +1743,7 @@ int32_t run_cached(fgpu_ctx* ctx, ExecCache& x, fgpu_result* res, int collective
   CUDA_TRY(launch_table_init(x.qd, s));
   CUDA_TRY(cudaEventRecord(ctx->ev[1], s));
   if (x.has_runs) {
-    if (x.runs_v1) CUDA_TRY(launch_runs(x.rd, x.runs_nl, x.runs_nk, x.runs_na, ctx->sm_count, s));
-    else CUDA_TRY(launch_runs_tma(x.rd, x.runs_nl, x.runs_nk, x.runs_na, ctx->sm_count, s));
+    CUDA_TRY(launch_runs_tma(x.rd, x.runs_nl, x.runs_nk, x.runs_na, ctx->sm_count, s));
   }
   if (x.has_ta) CUDA_TRY(launch_tile_agg(x.td, ctx->sm_count, s));
   CUDA_TRY(launch_scan(x.qdesc_dev, x.qd, ctx->sm_count, s));
@@ -1732,14 +1831,19 @@ int32_t run_scan(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, fgpu_result* re
   std::vector<std::pair<size_t, size_t>> lut_fix;  // (index into lrt, offset into lutbytes)
   uint32_t tiles = 0;
   const uint32_t tile_len = q.kind == FGPU_PLAN_FILTER ? uint32_t(kTileRows) : uint32_t(qd.vl);  // rows plan: CTA tiles; scan: warp vectors
-  // ---- sorted-run scan: query-level eligibility (see runs_scan.cu) --------------------------------
+  // ---- sorted-run scan: query-level eligibility (see runs_tma.cu) --------------------------------
   // One launch over the qualifying row groups; a row group whose statistics already decided every
   // leaf is flagged all_pass (its leaf columns are neither uploaded nor staged).
+  struct RunsRgCols {  // the chunks behind RunsRg::col (null: not staged)
+    Part* part = nullptr;
+    ChunkHost* ch[kRunsCols] = {nullptr};
+  };
   struct RunsBatch {
     RunsDesc rd{};
     int nl = 0;
     int col_slot[kRunsCols] = {0};
     std::vector<RunsRg> rgs;
+    std::vector<RunsRgCols> cols;
     std::vector<uint32_t> rows, first_span;
     size_t o_rg = 0, o_span = 0;
   };
@@ -1749,7 +1853,6 @@ int32_t run_scan(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, fgpu_result* re
   int runs_leaf_slot[kRunsLeaves] = {0}, runs_agg_slot[kRunsAggs] = {0}, runs_agg_index[kRunsAggs] = {0};
   uint32_t runs_agg_func[kRunsAggs] = {0};
   bool runs_q = q.kind != FGPU_PLAN_FILTER && c.runs_shape && !getenv("FROSTGPU_NO_RUNS");
-  const bool runs_v1 = getenv("FROSTGPU_RUNS_V1") != nullptr;  // the warp-private cp.async kernel (runs_scan.cu), kept for A/B measurements
   if (runs_q) {
     for (int l = 0; l < n_leaves && runs_q; l++) {
       const LeafDesc& ld = qd.leaves[l];
@@ -1919,6 +2022,7 @@ int32_t run_scan(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, fgpu_result* re
       all_pass = all_all;
     }
     RunsRg rr{};
+    RunsRgCols rcols{};
     if (runs_ok) {
       RunsBatch& B = batches[bi];
       rr.n_rows = rg.n_rows;
@@ -1945,22 +2049,21 @@ int32_t run_scan(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, fgpu_result* re
         B.rd.pred_null[i] = rt.null_result;
       }
       rr.all_pass = all_pass ? 1 : 0;
-      const uint8_t* any_col = nullptr;
+      bool any_col = false;
+      rcols.part = c.rgs[size_t(g0)].part;
       for (uint32_t i = 0; i < B.rd.n_cols && runs_ok; i++) {
         const ChunkDesc& d = chunks[size_t(g) * n_slots + B.col_slot[i]];
         rr.col[i] = nullptr;
         if ((c.rgs[size_t(g0)].skip_slots >> B.col_slot[i]) & 1) continue;  // a decided leaf's own column
         if (d.kind != CK_PLAIN64 || d.has_nulls) runs_ok = false;
         rr.col[i] = d.values;
-        any_col = d.values;
+        rcols.ch[i] = &rg.cols.at(c.slot_names[size_t(B.col_slot[i])]);
+        any_col = true;
       }
       // all_pass: the leaf columns stay null (not staged).  Otherwise a decided leaf still runs its
-      // (widened) range test: any staged column stands in for the one that was not uploaded.
-      for (uint32_t i = 0; i < B.rd.n_cols && runs_ok && !all_pass; i++) {
-        if (rr.col[i]) continue;
-        if (!any_col) runs_ok = false;
-        rr.col[i] = any_col;
-      }
+      // (widened) range test: a staged column stands in for the one that was not uploaded (see the tile plan).
+      for (uint32_t i = 0; i < B.rd.n_cols && runs_ok && !all_pass; i++)
+        if (!rr.col[i] && !any_col) runs_ok = false;
       if (all_pass)  // aggregate inputs must be there
         for (int a = 0; a < runs_na && runs_ok; a++)
           if (!rr.col[B.rd.agg_col[a]]) runs_ok = false;
@@ -1976,6 +2079,7 @@ int32_t run_scan(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, fgpu_result* re
     }
     if (runs_ok) {
       batches[bi].rgs.push_back(rr);
+      batches[bi].cols.push_back(rcols);
       batches[bi].rows.push_back(rg.n_rows);
       lut_fix.erase(std::remove_if(lut_fix.begin(), lut_fix.end(), [&](const std::pair<size_t, size_t>& f) { return f.first >= size_t(g) * n_leaves; }), lut_fix.end());
       continue;  // slot g of the general tables is reused by the next row group
@@ -2053,66 +2157,69 @@ int32_t run_scan(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, fgpu_result* re
   first_tile[size_t(gi)] = tiles;
   qd.n_rg = gi;
   qd.n_tiles = tiles;
-  // spans of the sorted-run kernel: sized so that every warp of the grid gets several
+  // ---- sorted-run kernel: frame-of-reference images, tile rows, stage layout ------------------------
   for (RunsBatch& B : batches) {
     if (B.rgs.empty()) continue;
     RunsDesc& rd = B.rd;
     auto envi = [](const char* n, int d) { const char* e = getenv(n); return e ? atoi(e) : d; };
     rd.n_rg = uint32_t(B.rgs.size());
+    {  // every staged int64 column of every part, narrowed in one batch
+      std::set<std::pair<Part*, std::string>> seen;
+      std::vector<std::pair<Part*, std::string>> want;
+      for (const RunsRgCols& rc2 : B.cols)
+        for (uint32_t i = 0; i < rd.n_cols; i++)
+          if (rc2.ch[i] && rc2.ch[i]->phys == PT_INT64 && seen.emplace(rc2.part, c.slot_names[size_t(B.col_slot[i])]).second)
+            want.emplace_back(rc2.part, c.slot_names[size_t(B.col_slot[i])]);
+      if (int32_t rcn = ensure_narrow(ctx, want)) return rcn;
+    }
+    // every row group is cut into tiles of about tile_bytes of staged column data; the launch's tile table {row group,
+    // first row} is dealt to the CTAs in chunks of consecutive entries
+    uint32_t tile_bytes = 4096 * 8;
+    { const int f = envi("FROSTGPU_RT_TILE", 0); if (f == 1024 || f == 2048 || f == 4096 || f == 8192) tile_bytes = uint32_t(f) * 8u; }  // (rows of 8 bytes)
+    uint32_t tiles_rt = 0, gidx = 0, col_region = 0, max_tile = 1024;
     uint64_t total = 0;
     for (uint32_t r : B.rows) total += r;
-    int br = 0;
-    uint64_t span_blocks = 0;
-    if (!runs_v1) {
-      // CTA-cooperative kernel (runs_tma.cu): tiles of br rows, spans of span_blocks tiles dealt to the CTAs in turn
-      // CTA-cooperative kernel (runs_tma.cu): every row group is cut into tiles of about 32 KB of column data; the
-      // launch's tile table {row group, first row} is dealt to the CTAs in chunks of consecutive entries
-      uint32_t base_tile = 4096;
-      { const int f = envi("FROSTGPU_RT_TILE", 0); if (f == 1024 || f == 2048 || f == 4096 || f == 8192) base_tile = uint32_t(f); }
-      uint32_t tiles_rt = 0, gidx = 0, col_region = 0;
-      for (RunsRg& r : B.rgs) {
-        uint32_t nc = 0;
-        for (uint32_t i = 0; i < rd.n_cols; i++) {
-          r.col_pos[i] = uint8_t(nc);
-          if (r.col[i]) nc++;
+    // small launches: at least one tile per resident CTA (three per SM), or the grid is not filled
+    const uint32_t fill_rows = uint32_t(std::min<uint64_t>(1u << 20, std::max<uint64_t>(1024, (total / (uint64_t(ctx->sm_count) * 3)) & ~uint64_t(1023))));
+    for (size_t k = 0; k < B.rgs.size(); k++) {
+      RunsRg& r = B.rgs[k];
+      uint32_t row_bytes = 0, max_runs = 0;
+      for (uint32_t i = 0; i < rd.n_cols; i++) {
+        const ChunkHost* ch = B.cols[k].ch[i];
+        r.cl[i] = RunsCol{0, 3, 0};
+        if (ch && ch->narrow) {
+          r.col[i] = ch->narrow;
+          r.cl[i].lg = ch->narrow_w == 1 ? 0 : (ch->narrow_w == 2 ? 1 : 2);
+          r.cl[i].base = ch->narrow_base;
+          st.algorithmic_bytes = st.algorithmic_bytes - ch->stored_bytes + uint64_t(r.n_rows) * ch->narrow_w;
         }
-        r.tile_rows = runs_tma_tile_rows(base_tile, nc);
-        col_region = std::max(col_region, nc * r.tile_rows * 8u);
-        for (uint32_t r0 = 0; r0 < r.n_rows; r0 += r.tile_rows) {
-          B.first_span.push_back(gidx);
-          B.first_span.push_back(r0);
-          tiles_rt++;
-        }
-        gidx++;
+        if (r.col[i]) row_bytes += 1u << r.cl[i].lg;
       }
-      runs_tma_plan(rd, runs_nk + runs_np, base_tile, col_region, envi("FROSTGPU_RT_STAGES", 0), envi("FROSTGPU_RT_WARPS", 0), envi("FROSTGPU_RT_SPAN", 0));
-      rd.n_spans = tiles_rt;
-      (void)br; (void)span_blocks;
-      continue;
-    } else {
-      br = envi("FROSTGPU_RUNS_BR", 256);
-      if (br != 128 && br != 256 && br != 512) br = 256;
-      int ring = envi("FROSTGPU_RUNS_RING", 2);
-      ring = std::min(4, std::max(2, ring));
-      if (rd.n_cols == 0) { br = 128; ring = 2; }  // nothing is staged (count per group): the ring is idle
-      rd.block_rows = uint32_t(br);
-      rd.n_ring = uint32_t(ring);
-      int per_sm = 1;
-      CUDA_TRY(runs_blocks_per_sm(rd, B.nl, runs_nk, runs_na, &per_sm));
-      const uint64_t warps = uint64_t(ctx->sm_count) * uint64_t(std::max(per_sm, 1)) * (kRunsThreads / 32);
-      span_blocks = total / (warps * 8 * uint64_t(br));
-      span_blocks = std::min<uint64_t>(64, std::max<uint64_t>(4, span_blocks));
-      if (const char* e = getenv("FROSTGPU_RUNS_SPAN")) span_blocks = uint64_t(std::max(1, atoi(e)));
+      for (int q = 0; q < runs_nk; q++) max_runs = std::max(max_runs, r.n_runs[q]);
+      for (int q = 0; q < runs_np; q++)
+        if (r.pred_runs[q]) max_runs = std::max(max_runs, r.pred_n_runs[q]);
+      r.tile_rows = std::min(runs_tma_tile_rows(tile_bytes, row_bytes, r.n_rows, max_runs), fill_rows);
+      int first = -1;
+      uint32_t off = 0;
+      for (uint32_t i = 0; i < rd.n_cols; i++) {
+        if (!r.col[i]) continue;
+        if (first < 0) first = int(i);
+        r.cl[i].soff = off;
+        off += ((r.tile_rows << r.cl[i].lg) + 127u) & ~127u;
+      }
+      for (uint32_t i = 0; i < rd.n_cols && first >= 0; i++)  // a column that is not staged reads a staged one
+        if (!r.col[i]) r.cl[i] = r.cl[first];
+      col_region = std::max(col_region, off);
+      max_tile = std::max(max_tile, r.tile_rows);
+      for (uint32_t r0 = 0; r0 < r.n_rows; r0 += r.tile_rows) {
+        B.first_span.push_back(gidx);
+        B.first_span.push_back(r0);
+        tiles_rt++;
+      }
+      gidx++;
     }
-    rd.span_blocks = uint32_t(span_blocks);
-    const uint64_t span_rows = span_blocks * uint64_t(br);
-    uint32_t spans = 0;
-    for (uint32_t r : B.rows) {
-      B.first_span.push_back(spans);
-      spans += uint32_t((uint64_t(r) + span_rows - 1) / span_rows);
-    }
-    B.first_span.push_back(spans);
-    rd.n_spans = spans;
+    runs_tma_plan(rd, runs_nk + runs_np, max_tile, col_region, envi("FROSTGPU_RT_STAGES", 0), envi("FROSTGPU_RT_WARPS", 0), envi("FROSTGPU_RT_SPAN", 0));
+    rd.n_spans = tiles_rt;
   }
 
   // ---- tile aggregate: tile size, ring depth and the shared-memory table -------------------------------
@@ -2422,8 +2529,7 @@ int32_t run_scan(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, fgpu_result* re
       rd.t_rows = qd.t_rows;
       for (int a = 0; a < runs_na; a++) rd.t_agg[a] = qd.t_agg[runs_agg_index[a]];
       rd.counters = qd.counters;
-      if (runs_v1) CUDA_TRY(launch_runs(rd, B.nl, runs_nk, runs_na, ctx->sm_count, s));
-      else CUDA_TRY(launch_runs_tma(rd, B.nl, runs_nk, runs_na, ctx->sm_count, s));
+      CUDA_TRY(launch_runs_tma(rd, B.nl, runs_nk, runs_na, ctx->sm_count, s));
       st.kernel_launches++;
       st.row_groups_runs += uint32_t(B.rgs.size());
     }
@@ -2509,7 +2615,6 @@ int32_t run_scan(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, fgpu_result* re
     x.qd = qd;
     x.qdesc_dev = qdesc_dev;
     x.has_runs = !batches[0].rgs.empty();
-    x.runs_v1 = runs_v1;
     x.rd = batches[0].rd;
     x.runs_nl = batches[0].nl;
     x.runs_nk = runs_nk;

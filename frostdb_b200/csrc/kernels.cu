@@ -27,6 +27,7 @@
 // per-warp vectors; see DESIGN.md.)
 #include <cuda_runtime.h>
 
+#include <climits>
 #include <cstdint>
 
 #include "device_types.h"
@@ -2164,6 +2165,76 @@ cudaError_t launch_flatten(const FlatJob* d_jobs, uint32_t n_jobs, uint32_t tota
   uint32_t grid = (total_blocks + NWARP - 1) / NWARP;
   if (grid > uint32_t(sm_count) * 8) grid = uint32_t(sm_count) * 8;
   k_flatten<<<grid, NT, 0, st>>>(d_jobs, n_jobs, total_blocks);
+  return cudaGetLastError();
+}
+
+// ======================================================================================================
+// Frame-of-reference images of PLAIN int64 chunks for the sorted-run kernel (runs_tma.cu).
+//   k_chunk_minmax: min / max of every job's chunk into mm[2 j], mm[2 j + 1] (preset to INT64_MAX / INT64_MIN).
+//   k_narrow:       out[r] = uint{8,16,32}(src[r] - base) for the jobs whose range fits 32 bits.
+// One CTA per kNarrowRows-row block of one job.
+// ======================================================================================================
+__device__ __forceinline__ uint32_t narrow_job(const NarrowJob* jobs, uint32_t n_jobs, uint32_t blk) {
+  uint32_t lo = 0, hi = n_jobs;  // last job with first_block <= blk
+  while (hi - lo > 1) {
+    const uint32_t mid = (lo + hi) >> 1;
+    if (__ldg(&jobs[mid].first_block) <= blk) lo = mid; else hi = mid;
+  }
+  return lo;
+}
+
+__global__ void __launch_bounds__(NT) k_chunk_minmax(const NarrowJob* __restrict__ jobs, uint32_t n_jobs, long long* mm) {
+  __shared__ long long s_lo[NWARP], s_hi[NWARP];
+  const uint32_t j = narrow_job(jobs, n_jobs, blockIdx.x);
+  const NarrowJob& J = jobs[j];
+  const uint32_t r0 = (blockIdx.x - J.first_block) * kNarrowRows, r1 = min(J.n_rows, r0 + kNarrowRows);
+  long long lo = LLONG_MAX, hi = LLONG_MIN;
+  for (uint32_t r = r0 + threadIdx.x; r < r1; r += NT) {
+    const long long v = __ldg(J.src + r);
+    lo = min(lo, v);
+    hi = max(hi, v);
+  }
+  for (int o = 16; o; o >>= 1) {
+    lo = min(lo, __shfl_xor_sync(0xffffffffu, lo, o));
+    hi = max(hi, __shfl_xor_sync(0xffffffffu, hi, o));
+  }
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  if (lane == 0) {
+    s_lo[warp] = lo;
+    s_hi[warp] = hi;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int w = 1; w < NWARP; w++) {
+      lo = min(lo, s_lo[w]);
+      hi = max(hi, s_hi[w]);
+    }
+    atomicMin(mm + 2 * j, lo);
+    atomicMax(mm + 2 * j + 1, hi);
+  }
+}
+
+__global__ void __launch_bounds__(NT) k_narrow(const NarrowJob* __restrict__ jobs, uint32_t n_jobs) {
+  const NarrowJob& J = jobs[narrow_job(jobs, n_jobs, blockIdx.x)];
+  const uint32_t r0 = (blockIdx.x - J.first_block) * kNarrowRows, r1 = min(J.n_rows, r0 + kNarrowRows), w = J.w;
+  const unsigned long long base = (unsigned long long)J.base;
+  for (uint32_t r = r0 + threadIdx.x; r < r1; r += NT) {
+    const unsigned long long d = (unsigned long long)__ldg(J.src + r) - base;  // < 2^(8 w): the host chose w from the range
+    if (w == 1) J.out[r] = uint8_t(d);
+    else if (w == 2) reinterpret_cast<uint16_t*>(J.out)[r] = uint16_t(d);
+    else reinterpret_cast<uint32_t*>(J.out)[r] = uint32_t(d);
+  }
+}
+
+cudaError_t launch_chunk_minmax(const NarrowJob* d_jobs, uint32_t n_jobs, uint32_t total_blocks, long long* d_mm, cudaStream_t st) {
+  if (n_jobs == 0 || total_blocks == 0) return cudaSuccess;
+  k_chunk_minmax<<<total_blocks, NT, 0, st>>>(d_jobs, n_jobs, d_mm);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_narrow(const NarrowJob* d_jobs, uint32_t n_jobs, uint32_t total_blocks, cudaStream_t st) {
+  if (n_jobs == 0 || total_blocks == 0) return cudaSuccess;
+  k_narrow<<<total_blocks, NT, 0, st>>>(d_jobs, n_jobs);
   return cudaGetLastError();
 }
 

@@ -18,13 +18,10 @@ constexpr int kIndexRows = 128;  // chunk index granularity (one warp): fixed wh
 
 cudaError_t launch_table_init(const QueryDesc& q, cudaStream_t st, bool zero_counters = true);
 cudaError_t launch_scan(const QueryDesc* d_q, const QueryDesc& q, int sm_count, cudaStream_t st);
-// sorted-run scan (runs_scan.cu): nl range leaves, nk run-length keys, na Sum(int64) aggregates
-constexpr int kRunsThreads = 128;
-cudaError_t launch_runs(const RunsDesc& d, int nl, int nk, int na, int sm_count, cudaStream_t st);
-cudaError_t runs_blocks_per_sm(const RunsDesc& d, int nl, int nk, int na, int* per_sm);  // resident CTAs per SM for this shape
-// sorted-run scan, CTA-cooperative with TMA-staged column tiles (runs_tma.cu): same descriptors as launch_runs
-uint32_t runs_tma_tile_rows(uint32_t base, uint32_t nc);  // rows per tile of a row group that stages nc columns
-void runs_tma_plan(RunsDesc& d, int nq, uint32_t base_tile, uint32_t col_region, int force_stages, int force_warps, int force_chunk);  // tile rows, ring depth, stage layout
+// sorted-run scan, CTA-cooperative with TMA-staged column tiles (runs_tma.cu): nl range leaves, nk run-length keys,
+// na Sum / Min / Max aggregates
+uint32_t runs_tma_tile_rows(uint32_t tile_bytes, uint32_t row_bytes, uint32_t n_rows, uint32_t max_runs);  // rows per tile of one row group
+void runs_tma_plan(RunsDesc& d, int nq, uint32_t max_tile, uint32_t col_region, int force_stages, int force_warps, int force_chunk);  // ring depth, stage layout
 size_t runs_tma_smem_bytes(const RunsDesc& d);
 int runs_tma_ctas_per_sm(const RunsDesc& d);
 cudaError_t launch_runs_tma(const RunsDesc& d, int nl, int nk, int na, int sm_count, cudaStream_t st);
@@ -36,6 +33,9 @@ cudaError_t launch_tile_agg(const TileAggDesc& d, int sm_count, cudaStream_t st)
 size_t tile_agg_smem_bytes(const TileAggDesc& d);
 // dictionary column chunks -> flat code arrays (kernels.cu)
 cudaError_t launch_flatten(const FlatJob* d_jobs, uint32_t n_jobs, uint32_t total_blocks, int sm_count, cudaStream_t st);
+// PLAIN int64 column chunks -> frame-of-reference images (kernels.cu): min / max per job, then the narrowing pass
+cudaError_t launch_chunk_minmax(const NarrowJob* d_jobs, uint32_t n_jobs, uint32_t total_blocks, long long* d_mm, cudaStream_t st);
+cudaError_t launch_narrow(const NarrowJob* d_jobs, uint32_t n_jobs, uint32_t total_blocks, cudaStream_t st);
 // partial-table exchange over peer-mapped mailboxes (comm.cu)
 cudaError_t launch_comm_push(const CommPush& p, int sm_count, cudaStream_t st);
 cudaError_t launch_comm_wait(const CommWait& w, cudaStream_t st);

@@ -55,6 +55,11 @@ struct ChunkHost {
   // flat code array of a CK_DICT_STR chunk (device pointer; derived on first use by k_flatten, see tile_agg.cu)
   const uint8_t* flat = nullptr;
   uint8_t flat_w = 0, flat_bias = 0;
+  // frame-of-reference image of a PLAIN non-null INT64 chunk whose range fits 32 bits (device pointer; derived on first
+  // use by the sorted-run kernel, see ensure_narrow): narrow_w bytes per row holding value - narrow_base
+  const uint8_t* narrow = nullptr;
+  uint8_t narrow_w = 0;
+  int64_t narrow_base = 0;
 };
 
 struct RowGroupHost {
@@ -82,6 +87,8 @@ struct ColumnImage {
   uint32_t n_seed_jobs = 0, max_seed_chunks = 0;
   std::string error;             // whole-column error (a chunk the engine cannot read)
   void* flat_dev = nullptr;      // flat code arrays of every row group of this column (one allocation) + the job table
+  bool narrowed = false;         // ensure_narrow ran (narrow_dev stays null when no chunk fits 32 bits)
+  void* narrow_dev = nullptr;    // frame-of-reference images of every narrowed chunk of this column (one allocation)
 };
 
 struct Part {

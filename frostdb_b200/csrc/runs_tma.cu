@@ -1,5 +1,5 @@
 // k_runs_tma: scan + range filter + group-by aggregate for row groups of SORTED parts, CTA-cooperative
-// with TMA-staged column tiles (sm_90a).  Same plan shape and the same descriptors as k_runs (runs_scan.cu):
+// with TMA-staged column tiles (sm_90a).  The plan shape:
 //   * the filter is a conjunction of <= 2 int64 range leaves on PLAIN non-null columns and <= 2 dictionary-column
 //     leaves on run-length columns (physicalplan/filter.go:276-323, binaryscalarexpr.go:41-311),
 //   * every group key is a dictionary-string column that is run-length only in the row group (what compaction
@@ -8,8 +8,9 @@
 //
 // Structure: kRtConsumerWarps consumer warps + ONE producer warp per CTA, two CTAs per SM.
 //   producer  walks the CTA's tiles (block_rows consecutive rows of one row group).  For every tile it waits until
-//             the consumers released the ring stage, issues ONE TMA bulk copy per staged PLAIN column
-//             (cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes, 8 - 32 KB each) and then stages the
+//             the consumers released the ring stage, issues ONE TMA bulk copy per staged column
+//             (cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes, rows x 1, 2, 4 or 8 bytes: the chunk's
+//             frame-of-reference image when its range fits 32 bits, see ensure_narrow) and then stages the
 //             piece of every key column's run directory that covers the tile: dir_entries entries from the run
 //             that holds the tile's first row (found through the 128-row seed), each reduced to
 //             {end row of the run, dense-table contribution (id + 1) * stride} — for a dictionary LEAF column
@@ -19,14 +20,15 @@
 //             of the tile: it finds its first run in the staged directory with one ballot per 32 entries, then walks
 //             SEGMENTS — stretches of rows up to the nearest run end of any cursor column, i.e. rows of ONE group.
 //             A segment is read with steps aligned to ITS first row (lane i reads row a + 32 s + i: conflict-free
-//             8-byte shared loads at any alignment), so only its last step is masked, and in row groups whose filter
+//             1-, 2-, 4- or 8-byte shared loads at any alignment, widened to base + v in 64 bits before the range test
+//             and the aggregate), so only its last step is masked, and in row groups whose filter
 //             was decided by the chunk statistics the row count of a segment is its length.  Partial sums stay in
 //             registers per lane while the group does not change; a change costs three REDUX (22-bit pieces of the
 //             64-bit lane sums), and one atomic per aggregate into the dense table in L2.
 //             Cursor moves read the staged directory (shared memory), never global memory, except in tiles that
 //             hold more runs than dir_entries (global fallback, same result).
 //
-// Algorithmic bytes per row: 8 per distinct staged column (the run directories are O(groups)).
+// Algorithmic bytes per row: the staged width of every distinct staged column (the run directories are O(groups)).
 #include <cuda_runtime.h>
 #include <cstdio>
 
@@ -87,6 +89,34 @@ __device__ __forceinline__ uint32_t lds32(uint32_t a) {
   asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(a));
   return v;
 }
+__device__ __forceinline__ uint32_t lds16(uint32_t a) {
+  uint32_t v;
+  asm volatile("ld.shared.u16 %0, [%1];" : "=r"(v) : "r"(a));
+  return v;
+}
+__device__ __forceinline__ uint32_t lds8(uint32_t a) {
+  uint32_t v;
+  asm volatile("ld.shared.u8 %0, [%1];" : "=r"(v) : "r"(a));
+  return v;
+}
+// one staged value of 1 << LG bytes, zero-extended
+template <uint32_t LG>
+__device__ __forceinline__ unsigned long long ldsw(uint32_t a) {
+  if constexpr (LG == 3) return lds64(a);
+  else if constexpr (LG == 2) return lds32(a);
+  else if constexpr (LG == 1) return lds16(a);
+  else return lds8(a);
+}
+__device__ __forceinline__ unsigned long long ldsw(uint32_t a, uint32_t lg) {  // lg warp-uniform
+  if (lg == 3) return lds64(a);
+  if (lg == 2) return lds32(a);
+  if (lg == 1) return lds16(a);
+  return lds8(a);
+}
+template <uint32_t V>
+struct Lg {
+  static constexpr uint32_t value = V;
+};
 __device__ __forceinline__ void sts_v2(uint32_t a, uint32_t x, uint32_t y) {
   asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(a), "r"(x), "r"(y) : "memory");
 }
@@ -144,9 +174,22 @@ __device__ __noinline__ uint3 cursor_global(const RunsRg* R, int q, int nk, uint
   return make_uint3(e.x, e.y, idx - k0);
 }
 
-// stage header (64 bytes): k0 of every cursor column, then the tile itself
+// stage header (144 bytes): k0 of every cursor column, then the tile itself, then the staged columns' layout
 constexpr uint32_t kHdrCnt = 20;                           // directory entries staged for every cursor column (0: a decided leaf)
 constexpr uint32_t kHdrR0 = 40, kHdrN = 44, kHdrRg = 48, kHdrT = 52;  // first row inside the row group; rows (0: no more tiles); row group; its tile rows
+constexpr uint32_t kHdrCol = 64;  // staged column c: {byte offset in the column region, log2 bytes per row, base (8 bytes)} at kHdrCol + 16 c
+constexpr uint32_t kHdrBytes = kHdrCol + 16u * kRunsCols;
+__device__ __forceinline__ uint4 lds_v4(uint32_t a) {
+  uint4 v;
+  asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(a));
+  return v;
+}
+// base + the staged value of column c in row r (col: the lane's address of row 0); the layout is read from the stage
+// header per use, so that neither the width nor the base of any column occupies registers across the loops
+__device__ __forceinline__ unsigned long long col_value(uint32_t stage_s, uint32_t c, uint32_t col, uint32_t r) {
+  const uint4 m = lds_v4(stage_s + kHdrCol + 16u * c);
+  return ((unsigned long long)m.z | ((unsigned long long)m.w << 32)) + ldsw(col + (r << m.y), m.y);
+}
 
 // GEN = false: every stored aggregate is Sum(int64).  GEN = true: Sum / Min / Max over int64 or float64 (agg_ops.cuh).
 // HP: the launch has dictionary leaves (cursor columns behind the keys).
@@ -160,7 +203,7 @@ __global__ void __launch_bounds__(kRtMaxThreads, 3) k_runs_tma(const __grid_cons
   const uint32_t kW = d.n_consumers;
   const uint32_t dir_bytes = E * 16u;
   const uint32_t bars = smem_u32(dyn);
-  const uint32_t stage0 = bars + 128u;  // stage: [header 64][directories kNQ x E x 8][columns n_cols x T x 8]
+  const uint32_t stage0 = bars + 128u;  // stage: [header 64][directories kNQ x E x 16][columns at RunsRg::col_soff]
 
   if (tid == 0) {
     for (uint32_t s = 0; s < S; s++) {
@@ -203,7 +246,7 @@ __global__ void __launch_bounds__(kRtMaxThreads, 3) k_runs_tma(const __grid_cons
       const Run* runs;    // link 2: this lane's cursor column (lane < nq), null: decided leaf
       const Seed* seeds;
       const uint8_t* col;  // this lane's staged column (lane < n_cols), null: not staged in this row group
-      uint32_t col_pos;    // its place among the row group's staged columns
+      uint32_t col_sl;     // its RunsCol: soff | lg << 24
       uint32_t n_runs, n_rows, T;
       uint32_t k0, k1;    // link 3: runs that hold the tile's first row and the first row behind the tile
     };
@@ -219,7 +262,7 @@ __global__ void __launch_bounds__(kRtMaxThreads, 3) k_runs_tma(const __grid_cons
       c.runs = nullptr;
       c.seeds = nullptr;
       c.col = nullptr;
-      c.col_pos = 0;
+      c.col_sl = 0;
       c.n_runs = 0;
       c.n_rows = 0;
       c.T = 0;
@@ -235,7 +278,8 @@ __global__ void __launch_bounds__(kRtMaxThreads, 3) k_runs_tma(const __grid_cons
         }
         if (uint32_t(lane) < n_cols) {
           c.col = ldg_ptr(&R->col[lane]);
-          c.col_pos = __ldg(&R->col_pos[lane]);
+          const uint2 sl = __ldg(reinterpret_cast<const uint2*>(&R->cl[lane]));
+          c.col_sl = sl.x | (sl.y << 24);
         }
       }
     };
@@ -270,13 +314,17 @@ __global__ void __launch_bounds__(kRtMaxThreads, 3) k_runs_tma(const __grid_cons
       for (int c = 0; c < kRunsCols; c++) {
         if (uint32_t(c) < n_cols) {
           const unsigned long long colc = __shfl_sync(FULL, reinterpret_cast<unsigned long long>(c0.col), c);
-          const uint32_t posc = __shfl_sync(FULL, c0.col_pos, c);
+          const uint32_t sl = __shfl_sync(FULL, c0.col_sl, c), lg = sl >> 24;
           if (lane == 0 && colc != 0ull) {
-            const uint32_t cb = (n * 8u + 15u) & ~15u;
-            bulk_g2s(stage_s + d.col_off + posc * c0.T * 8u, reinterpret_cast<const uint8_t*>(colc) + size_t(c0.r0) * 8u, cb, full);
+            const uint32_t cb = ((n << lg) + 15u) & ~15u;  // (images and extents keep >= 16 readable bytes behind the last row)
+            bulk_g2s(stage_s + d.col_off + (sl & 0xffffffu), reinterpret_cast<const uint8_t*>(colc) + (size_t(c0.r0) << lg), cb, full);
             bytes += cb;
           }
         }
+      }
+      if (lane == 0 && n_cols) {  // the columns' layout {soff, lg, base} for the consumers: RunsRg::cl
+        bulk_g2s(stage_s + kHdrCol, d.rgs[c0.rg].cl, n_cols * 16u, full);
+        bytes += n_cols * 16u;
       }
       // directory slices: entries k0 .. k1 + 1 of every cursor column (the entry behind the last run carries its end)
 #pragma unroll
@@ -287,7 +335,7 @@ __global__ void __launch_bounds__(kRtMaxThreads, 3) k_runs_tma(const __grid_cons
           if (lane == 0) {
             const uint32_t cnt = rq ? min(E, k1 - k0 + 2u) : 0u;
             if (cnt) {
-              bulk_g2s(stage_s + 64u + uint32_t(q) * dir_bytes, reinterpret_cast<const Run*>(rq) + k0, cnt * 16u, full);
+              bulk_g2s(stage_s + kHdrBytes + uint32_t(q) * dir_bytes, reinterpret_cast<const Run*>(rq) + k0, cnt * 16u, full);
               bytes += cnt * 16u;
             }
             sts32(stage_s + uint32_t(q) * 4u, k0);
@@ -384,12 +432,6 @@ __global__ void __launch_bounds__(kRtMaxThreads, 3) k_runs_tma(const __grid_cons
     uint32_t stride[NK > 0 ? NK : 1];
 #pragma unroll
     for (int k = 0; k < NK; k++) stride[k] = d.stride[k];
-    const RunsRg* R = d.rgs;
-    uint32_t lpos[NL > 0 ? NL : 1], apos[NA > 0 ? NA : 1];  // place of every leaf / aggregate column among the row group's staged columns
-#pragma unroll
-    for (int l = 0; l < NL; l++) lpos[l] = d.leaf_col[l];
-#pragma unroll
-    for (int a = 0; a < NA; a++) apos[a] = d.agg_col[a];
     const uint8_t* plut[kRunsPreds] = {nullptr, nullptr};  // result byte per GLOBAL dictionary id of every dictionary leaf
 
     uint32_t st = 0, ph = 0;
@@ -398,31 +440,24 @@ __global__ void __launch_bounds__(kRtMaxThreads, 3) k_runs_tma(const __grid_cons
       const uint32_t stage_s = stage0 + st * d.stage_bytes;
       const uint32_t n = lds32(stage_s + kHdrN);
       if (n == 0) break;  // the producer's end marker
-      const uint32_t r0 = lds32(stage_s + kHdrR0);
+      const uint32_t r0 = lds32(stage_s + kHdrR0), rg = lds32(stage_s + kHdrRg);
+      const RunsRg* const R = d.rgs + rg;
       if (NL > 0 || HP) {
-        const uint32_t rg = lds32(stage_s + kHdrRg);
         if (rg != rg_cached) {
           rg_cached = rg;
-          R = d.rgs + rg;
 #pragma unroll
           for (int l = 0; l < NL; l++) {
             lo[l] = __ldg(&R->lo[l]);
             hi[l] = __ldg(&R->hi[l]);
           }
-          if (NL > 0) {
-            all_pass = __ldg(&R->all_pass) != 0;  // warp-uniform: statistics decided the filter
-#pragma unroll
-            for (int l = 0; l < NL; l++) lpos[l] = __ldg(&R->col_pos[d.leaf_col[l]]);
-#pragma unroll
-            for (int a = 0; a < NA; a++) apos[a] = __ldg(&R->col_pos[d.agg_col[a]]);
-          }
+          if (NL > 0) all_pass = __ldg(&R->all_pass) != 0;  // warp-uniform: statistics decided the filter
           if constexpr (HP) {
 #pragma unroll
             for (int p = 0; p < kRunsPreds; p++) plut[p] = uint32_t(p) < n_pred ? ldg_ptr(&R->pred_lut[p]) : nullptr;
           }
         }
       }
-      const uint32_t T = lds32(stage_s + kHdrT), SUB = T >> d.consumers_log2, col_bytes = T * 8u;
+      const uint32_t T = lds32(stage_s + kHdrT), SUB = T >> d.consumers_log2;
       const uint32_t s0 = r0 + uint32_t(warp) * SUB, s1 = min(r0 + n, s0 + SUB);
       if (s0 < s1) {
         const uint32_t cols_s = stage_s + d.col_off;
@@ -430,14 +465,13 @@ __global__ void __launch_bounds__(kRtMaxThreads, 3) k_runs_tma(const __grid_cons
         // {first row, -, dictionary id or NULL, -}; the end of a run is the first row of the next entry)
         uint32_t ci[NQ > 0 ? NQ : 1], cend[NQ > 0 ? NQ : 1], ccon[NQ > 0 ? NQ : 1], ccnt[NQ > 0 ? NQ : 1];
         auto entry = [&](int q) {  // loads cend / ccon of cursor q at ci[q]
-          const uint32_t dq = stage_s + 64u + uint32_t(q) * dir_bytes + ci[q] * 16u;
+          const uint32_t dq = stage_s + kHdrBytes + uint32_t(q) * dir_bytes + ci[q] * 16u;
           if (ci[q] + 1u < ccnt[q]) {
             const uint32_t val = lds32(dq + 8u);
             cend[q] = lds32(dq + 16u);
             if (q < NK) ccon[q] = (val + 1u) * stride[q < NK ? q : 0];  // NULL (0xffffffff) contributes 0
             else ccon[q] = val == 0xffffffffu ? d.pred_null[q >= NK ? q - NK : 0] : uint32_t(__ldg(plut[q >= NK ? q - NK : 0] + val));
           } else {  // the tile holds more runs than the staged window
-            if (!(NL > 0 || HP)) R = d.rgs + lds32(stage_s + kHdrRg);
             const uint3 g = cursor_global(R, q, NK, q < NK ? stride[q < NK ? q : 0] : 0u, q < NK ? 0u : d.pred_null[q >= NK ? q - NK : 0],
                                           lds32(stage_s + uint32_t(q) * 4u), ci[q], 0u);
             cend[q] = g.x;
@@ -453,7 +487,7 @@ __global__ void __launch_bounds__(kRtMaxThreads, 3) k_runs_tma(const __grid_cons
           if (q < NK || uint32_t(q - NK) < n_pred) {
             ccnt[q] = lds32(stage_s + kHdrCnt + uint32_t(q) * 4u);
             if (ccnt[q]) {
-              const uint32_t dq = stage_s + 64u + uint32_t(q) * dir_bytes;
+              const uint32_t dq = stage_s + kHdrBytes + uint32_t(q) * dir_bytes;
               uint32_t idx = 0;
               for (uint32_t b = 0; b < ccnt[q]; b += 32u) {
                 const uint32_t j = b + uint32_t(lane);
@@ -465,7 +499,6 @@ __global__ void __launch_bounds__(kRtMaxThreads, 3) k_runs_tma(const __grid_cons
                 ci[q] = idx - 1u;  // entry 0 starts at or before the tile's first row
                 entry(q);
               } else {  // the run of s0 lies behind the staged window: found through the seed
-                if (!(NL > 0 || HP)) R = d.rgs + lds32(stage_s + kHdrRg);
                 const uint3 g = cursor_global(R, q, NK, q < NK ? stride[q < NK ? q : 0] : 0u, q < NK ? 0u : d.pred_null[q >= NK ? q - NK : 0],
                                               lds32(stage_s + uint32_t(q) * 4u), 0xffffffffu, s0);
                 cend[q] = g.x;
@@ -479,11 +512,42 @@ __global__ void __launch_bounds__(kRtMaxThreads, 3) k_runs_tma(const __grid_cons
           ci[q]++;
           entry(q);
         };
+        // staged leaf / aggregate columns: address of row r in lane i = col + (r + i) << lg; value = base + staged
         uint32_t lcol[NL > 0 ? NL : 1], acol[NA > 0 ? NA : 1];
+        auto col_addr = [&](uint32_t c) {
+          const uint2 m = lds_v2(stage_s + kHdrCol + 16u * c);
+          return cols_s + m.x + ((uint32_t(lane) - r0) << m.y);
+        };
 #pragma unroll
-        for (int l = 0; l < NL; l++) lcol[l] = cols_s + lpos[l] * col_bytes + uint32_t(lane) * 8u - r0 * 8u;
+        for (int l = 0; l < NL; l++) lcol[l] = col_addr(d.leaf_col[l]);
 #pragma unroll
-        for (int a = 0; a < NA; a++) acol[a] = cols_s + apos[a] * col_bytes + uint32_t(lane) * 8u - r0 * 8u;
+        for (int a = 0; a < NA; a++) acol[a] = col_addr(d.agg_col[a]);
+        // all_pass segment of aggregate q at row `row`: every step unmasked but the last, LG bytes per staged value
+        auto fold_seg = [&](int q, uint32_t row, uint32_t whole, uint32_t rem, auto L) {
+          constexpr uint32_t LG = decltype(L)::value, stp = 32u << LG;
+          const uint2 bw = lds_v2(stage_s + kHdrCol + 16u * d.agg_col[q] + 8u);
+          const unsigned long long b = (unsigned long long)bw.x | ((unsigned long long)bw.y << 32);
+          uint32_t a0 = acol[q] + (row << LG);
+#pragma unroll 1
+          for (uint32_t s = whole >> 2; s; s--, a0 += 4u * stp) {
+            const unsigned long long v0 = ldsw<LG>(a0), v1 = ldsw<LG>(a0 + stp), v2 = ldsw<LG>(a0 + 2u * stp), v3 = ldsw<LG>(a0 + 3u * stp);
+            fold(q, true, b + v0);
+            fold(q, true, b + v1);
+            fold(q, true, b + v2);
+            fold(q, true, b + v3);
+          }
+          if (whole & 2u) {
+            const unsigned long long v0 = ldsw<LG>(a0), v1 = ldsw<LG>(a0 + stp);
+            fold(q, true, b + v0);
+            fold(q, true, b + v1);
+            a0 += 2u * stp;
+          }
+          if (whole & 1u) {
+            fold(q, true, b + ldsw<LG>(a0));
+            a0 += stp;
+          }
+          if (uint32_t(lane) < rem) fold(q, true, b + ldsw<LG>(a0));
+        };
 
         uint32_t row = s0;
         while (row < s1) {
@@ -508,63 +572,48 @@ __global__ void __launch_bounds__(kRtMaxThreads, 3) k_runs_tma(const __grid_cons
               cs = us;
             }
             const uint32_t len = seg_end - row, whole = len >> 5, rem = len & 31u;
-            const uint32_t off = row * 8u;
             if (all_pass) {
               ucnt += len;
 #pragma unroll
               for (int q = 0; q < NA; q++) {
-                uint32_t a0 = acol[q] + off;
-#pragma unroll 1
-                for (uint32_t s = whole >> 2; s; s--, a0 += 1024u) {
-                  const unsigned long long v0 = lds64(a0), v1 = lds64(a0 + 256u), v2 = lds64(a0 + 512u), v3 = lds64(a0 + 768u);
-                  fold(q, true, v0);
-                  fold(q, true, v1);
-                  fold(q, true, v2);
-                  fold(q, true, v3);
+                switch (lds32(stage_s + kHdrCol + 16u * d.agg_col[q] + 4u)) {  // log2 bytes per row (warp-uniform)
+                  case 0: fold_seg(q, row, whole, rem, Lg<0>{}); break;
+                  case 1: fold_seg(q, row, whole, rem, Lg<1>{}); break;
+                  case 2: fold_seg(q, row, whole, rem, Lg<2>{}); break;
+                  default: fold_seg(q, row, whole, rem, Lg<3>{}); break;
                 }
-                if (whole & 2u) {
-                  const unsigned long long v0 = lds64(a0), v1 = lds64(a0 + 256u);
-                  fold(q, true, v0);
-                  fold(q, true, v1);
-                  a0 += 512u;
-                }
-                if (whole & 1u) {
-                  fold(q, true, lds64(a0));
-                  a0 += 256u;
-                }
-                if (uint32_t(lane) < rem) fold(q, true, lds64(a0));
               }
             } else if (NL > 0) {
               counted = true;
               // whole steps: no row mask; the tail step re-reads the segment's first row in the lanes behind its end
-              uint32_t so = off;
+              uint32_t r = row;
 #pragma unroll 2
-              for (uint32_t s = 0; s < whole; s++, so += 256u) {
+              for (uint32_t s = 0; s < whole; s++, r += 32u) {
                 bool in = true;
 #pragma unroll
                 for (int l = 0; l < NL; l++) {
-                  const long long x = (long long)lds64(lcol[l] + so);
+                  const long long x = (long long)col_value(stage_s, d.leaf_col[l], lcol[l], r);
                   in = in && x >= lo[l] && x <= hi[l];
                 }
                 if (in) cnt++;
 #pragma unroll
                 for (int q = 0; q < NA; q++) {
-                  const unsigned long long v = lds64(acol[q] + so);
+                  const unsigned long long v = col_value(stage_s, d.agg_col[q], acol[q], r);
                   if constexpr (GEN) fold(q, in, v);
                   else if (in) part[q] += v;
                 }
               }
               if (rem) {
                 bool in = uint32_t(lane) < rem;
-                if (!in) so = off - uint32_t(lane) * 8u;
+                if (!in) r = row - uint32_t(lane);
 #pragma unroll
                 for (int l = 0; l < NL; l++) {
-                  const long long x = (long long)lds64(lcol[l] + so);
+                  const long long x = (long long)col_value(stage_s, d.leaf_col[l], lcol[l], r);
                   in = in && x >= lo[l] && x <= hi[l];
                 }
                 if (in) cnt++;
 #pragma unroll
-                for (int q = 0; q < NA; q++) fold(q, in, lds64(acol[q] + so));
+                for (int q = 0; q < NA; q++) fold(q, in, col_value(stage_s, d.agg_col[q], acol[q], r));
               }
             }
           }
@@ -623,29 +672,35 @@ RtKern pick(const RunsDesc& d, int nl, int nk, int na) {
 
 }  // namespace
 
-// Rows per tile of a row group that stages nc columns: about 32 KB of column data per stage.
-uint32_t runs_tma_tile_rows(uint32_t base, uint32_t nc) {
-  uint32_t t = base;
-  for (uint32_t c = 1; c < nc && t > 1024u; c <<= 1) t >>= 1;
-  return t;
+// Rows per tile of a row group whose staged columns take row_bytes per row: tile_bytes of column data, a multiple of
+// 1024 rows, but not much more than the row group (the stage is sized for the largest tile of the launch) and, where
+// runs are short, few enough rows that the tile rarely holds more runs of a cursor column (max_runs in the row group)
+// than the staged directory window.
+uint32_t runs_tma_tile_rows(uint32_t tile_bytes, uint32_t row_bytes, uint32_t n_rows, uint32_t max_runs) {
+  uint64_t t = tile_bytes / std::max<uint32_t>(row_bytes, 1u);
+  t = std::min<uint64_t>(t, (uint64_t(n_rows) + 1023u) & ~uint64_t(1023));
+  if (max_runs) t = std::min<uint64_t>(t, uint64_t(kRtDirMax) * n_rows / max_runs);
+  return uint32_t(std::max<uint64_t>(t & ~uint64_t(1023), 1024u));
 }
 
-// Ring depth, consumer warps and stage layout for a launch with nq cursor columns whose largest tile holds
-// col_region bytes of column data (fills the descriptor; block_rows = the tile rows of a one-column row group).
-void runs_tma_plan(RunsDesc& d, int nq, uint32_t base_tile, uint32_t col_region, int force_stages, int force_warps, int force_chunk) {
+// Ring depth, consumer warps and stage layout for a launch with nq cursor columns whose largest tile has max_tile rows
+// and holds col_region bytes of column data (fills the descriptor).
+void runs_tma_plan(RunsDesc& d, int nq, uint32_t max_tile, uint32_t col_region, int force_stages, int force_warps, int force_chunk) {
   uint32_t S = 2;  // two stages of 32 KB leave room for three CTAs per SM: measured faster than deeper rings under two
   if (force_stages >= 2 && force_stages <= 8) S = uint32_t(force_stages);
   uint32_t W = uint32_t(kRtConsumerWarps);
   if (force_warps == 4 || force_warps == 8) W = uint32_t(force_warps);
-  d.block_rows = base_tile;
-  d.span_blocks = force_chunk >= 1 && force_chunk <= 64 ? uint32_t(force_chunk) : 4u;
+  d.block_rows = max_tile;
+  // one tile per ticket: with 1-2 bytes per staged row a launch has only a few tiles per CTA, and single tiles balance
+  // the tail best (DESIGN §7)
+  d.span_blocks = force_chunk >= 1 && force_chunk <= 64 ? uint32_t(force_chunk) : 1u;
   d.n_ring = S;
   d.n_consumers = W;
   d.consumers_log2 = W == 4 ? 2u : (W == 8 ? 3u : 4u);
-  // staged directory window: base_tile / 32 entries cover a tile whose runs average 32 rows; halved while two CTAs do not fit an SM
-  d.dir_entries = std::min<uint32_t>(base_tile / 32u, uint32_t(kRtDirMax));
+  // staged directory window: max_tile / 32 entries cover a tile whose runs average 32 rows; halved while two CTAs do not fit an SM
+  d.dir_entries = std::min<uint32_t>(max_tile / 32u, uint32_t(kRtDirMax));
   for (;;) {
-    d.col_off = (64u + uint32_t(nq) * d.dir_entries * 16u + 127u) & ~127u;
+    d.col_off = (kHdrBytes + uint32_t(nq) * d.dir_entries * 16u + 127u) & ~127u;
     d.stage_bytes = d.col_off + ((col_region + 127u) & ~127u);
     if (d.dir_entries <= 32u || 2 * (runs_tma_smem_bytes(d) + 1024) <= 228u * 1024u) break;
     d.dir_entries >>= 1;

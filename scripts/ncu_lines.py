@@ -1,7 +1,7 @@
 """Per-source-line instruction / stall profile of one kernel from an ncu report.
 
   python scripts/ncu_lines.py gpurun_out/prof.ncu-rep [kernel-symbol-substring] [rows]
-  (NCU_LINES_UNIT=runs_scan picks frostdb_b200/csrc/runs_scan.cu / build/runs_scan.o instead of kernels)
+  (NCU_LINES_UNIT=runs_tma picks frostdb_b200/csrc/runs_tma.cu / build/runs_tma.o instead of kernels)
 
 Joins `ncu --page source --csv` (per-SASS-instruction counters, in program order) with
 `nvdisasm -g` of the cubin inside frostdb_b200/csrc/build/kernels.o (line markers, same order)."""

@@ -1,6 +1,6 @@
-"""A/B probe of the sorted-run kernels on 32 Mi sorted rows (runs on the GPU box): k_runs_tma (TMA-staged tiles,
-CTA-cooperative) against k_runs (warp-private cp.async rings, FROSTGPU_RUNS_V1=1), tile / ring shapes, and a
-row-by-row comparison of the two kernels' results."""
+"""Probe of the sorted-run kernel k_runs_tma on PROBE_ROWS (default 32 Mi) sorted rows (runs on a GPU): kernel time of
+a set of plan shapes, then a sweep of tile bytes / ring stages / consumer warps / chunk tiles (FROSTGPU_RT_*), every
+result compared row by row with the default shape's."""
 import ctypes as C, os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
@@ -70,7 +70,6 @@ def run(table, name, kind, f, groups, aggs, env=None):
 ts, val, fval = lp.Col("timestamp"), lp.Col("value"), lp.Col("floatvalue")
 K01 = [lp.Col("labels.l00"), lp.Col("labels.l01")]
 AGG = _lib.PLAN_AGGREGATE
-V1 = {"FROSTGPU_RUNS_V1": "1"}
 load("s", True)
 F50 = lp.And(ts.GtEq(lp.Literal(bd.T0 + rows // 4)), ts.Lt(lp.Literal(bd.T0 + 3 * rows // 4)))
 VF = val.Lt(lp.Literal(500))
@@ -88,21 +87,18 @@ cases = [
     ("sorted: l01 != v000003, sum by l00,l01", lp.Col("labels.l01").NotEq(lp.Literal("v000003")), K01, [lp.Sum(val)]),
 ]
 for name, f, g, a in cases:
-    run("s", name, AGG, f, g, a, V1)
     run("s", name, AGG, f, g, a)
 if os.environ.get("PROBE_NOSWEEP"):
     sys.exit(0)
 def sweep(ci, combos):
-    for t, st, w in combos:
+    for t, st, w, sp in combos:
         env = {}
-        if t: env["FROSTGPU_RT_TILE"] = str(t)
+        if t: env["FROSTGPU_RT_TILE"] = str(t)  # tile bytes / 8
         if st: env["FROSTGPU_RT_STAGES"] = str(st)
         if w: env["FROSTGPU_RT_WARPS"] = str(w)
+        if sp: env["FROSTGPU_RT_SPAN"] = str(sp)
         run("s", cases[ci][0], AGG, cases[ci][1], cases[ci][2], cases[ci][3], env)
 
 
-for ci in (0, 1, 2, 4, 6):
-    sweep(ci, ((4096, 2, 8), (4096, 3, 8), (2048, 3, 8), (2048, 4, 4), (4096, 2, 4)))
-for ci in (0, 6):
-    for sp in (1, 2, 8, 16):
-        run("s", cases[ci][0], AGG, cases[ci][1], cases[ci][2], cases[ci][3], {"FROSTGPU_RT_SPAN": str(sp)})
+for ci in (1, 0, 2):
+    sweep(ci, [(t, st, 0, sp) for t in (2048, 4096, 8192) for st in (2, 3, 4) for sp in (1, 2, 4, 8)] + [(4096, 2, 4, 4), (2048, 3, 4, 2)])
