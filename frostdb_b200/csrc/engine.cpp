@@ -2276,15 +2276,17 @@ int32_t run_scan(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, fgpu_result* re
     TA.first_tile.push_back(t);
     td.n_tiles = t;
     td.chunk_tiles = std::max<uint32_t>(1, t / (uint32_t(ctx->sm_count) * 4));  // ~4 turns per CTA: a CTA stays inside one row group for a whole chunk
+    // (the override comes first: the 32-bit Sum bound below depends on the chunk length the launch uses)
+    if (const char* e = getenv("FROSTGPU_TA_CHUNK")) td.chunk_tiles = uint32_t(std::max(1, atoi(e)));
     td.keys8 = 1;
     for (uint32_t i = 0; i < td.nk; i++)
       if (TA.code_wmax[td.key_code[i]] > 8) td.keys8 = 0;
     {  // can a Sum leave 32 bits inside one CTA?  rows per CTA <= its share of the tiles (+ one chunk), all in one slot
       const uint64_t grid = uint64_t(std::max(1, ctx->sm_count));
-      const uint64_t rows_per_cta = (uint64_t(t) / grid + 2 * uint64_t(td.chunk_tiles) + 1) * td.tile_rows;
-      td.sums_fit32 = (TA.agg_bounded && !getenv("FROSTGPU_TA_CARRY") && TA.agg_max * rows_per_cta < (1ull << 32)) ? 1u : 0u;
+      const uint64_t rows_per_cta = std::min<uint64_t>(uint64_t(t), uint64_t(t) / grid + 2 * uint64_t(td.chunk_tiles) + 1) * td.tile_rows;
+      // agg_max * rows_per_cta <= 2^32 - 1, without the product (a large chunk override would overflow it)
+      td.sums_fit32 = (TA.agg_bounded && !getenv("FROSTGPU_TA_CARRY") && (TA.agg_max == 0 || rows_per_cta <= 0xffffffffull / TA.agg_max)) ? 1u : 0u;
     }
-    if (const char* e = getenv("FROSTGPU_TA_CHUNK")) td.chunk_tiles = uint32_t(std::max(1, atoi(e)));
   }
 
   // ---- filter-only plans over PLAIN columns: ordered take (take_rows.cu) instead of k_rows ------------
