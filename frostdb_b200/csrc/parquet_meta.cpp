@@ -597,7 +597,11 @@ bool walk_hybrid(const uint8_t* data, uint32_t len, int w, uint32_t count, uint3
         nbytes = avail;
       }
       uint32_t take = uint32_t(nvals < uint64_t(count - produced) ? nvals : uint64_t(count - produced));
-      if (take > 0 && take <= kShortLiteral) {
+      if (take > 0 && w == 0) {
+        // a width-0 literal (one-entry dictionary) is a run of index 0 of any length: recorded as one, it keeps
+        // such a column run-length only
+        push_rle(start0 + produced, 0);
+      } else if (take > 0 && take <= kShortLiteral) {
         // Writers close a repeated run on a multiple of 8 values and spill the boundary into one or two
         // literal groups ("aaaaabbb").  Such short literal runs are unpacked here into run-length
         // entries, so the directory of a sorted column holds no bit-packed run at all and the scan
