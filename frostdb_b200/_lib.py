@@ -80,7 +80,7 @@ class Stats(C.Structure):
                 ("scan_kernel_ms", C.c_float), ("total_device_ms", C.c_float), ("h2d_ms", C.c_float),
                 ("h2d_bytes", C.c_uint64), ("d2h_bytes", C.c_uint64),
                 ("row_groups_pruned", C.c_uint32), ("row_groups_runs", C.c_uint32),
-                ("row_groups_tiles", C.c_uint32), ("_reserved", C.c_uint32), ("rows_touched", C.c_uint64)]
+                ("row_groups_tiles", C.c_uint32), ("row_groups_prefix", C.c_uint32), ("rows_touched", C.c_uint64)]
 
     def asdict(self):
         return {k: getattr(self, k) for k, _ in self._fields_}

@@ -265,6 +265,34 @@ struct RunsDesc {
   unsigned long long* counters;
 };
 
+// ---- all-pass sorted row groups from prefix sums (k_runs_prefix, runs_prefix.cu) ----------------------------
+// A sorted-run row group whose filter the chunk statistics decided (every row passes) and whose stored aggregates are
+// all Sum(int64) is answered from the run directories of its key columns and the exclusive prefix sums of its Sum inputs
+// (ensure_narrow): the rows [b, e) of one group add P[e] - P[b] and e - b.  The host cuts the row groups into windows.
+struct PrefixRg {
+  uint32_t n_rows;
+  uint32_t _pad;
+  const long long* pre[kRunsAggs];  // P[0 .. n_rows] of every Sum input, P[i] = v[0] + ... + v[i-1] modulo 2^64
+  const Run* runs[kRunsKeys];       // row-space run directory of every key column (+ sentinel)
+  const Seed* seeds[kRunsKeys];     // its cursor seeds, one per kIndexRows rows
+  uint32_t n_runs[kRunsKeys];
+  uint32_t _pad2;
+};
+
+struct alignas(16) PrefixWin {
+  uint32_t rg, r0, rows, _pad;  // rows [r0, r0 + rows) of row group rg
+};
+
+struct PrefixDesc {
+  uint32_t n_win, nk, na;
+  uint32_t stride[kRunsKeys];  // dense-table stride of every key
+  const PrefixRg* rgs;
+  const PrefixWin* wins;
+  unsigned long long* t_rows;
+  long long* t_agg[kRunsAggs];
+  unsigned long long* counters;
+};
+
 // ---- filter-only plans over PLAIN columns (k_take_*, take_rows.cu) -----------------------------------
 constexpr int kTakeLeaves = 2, kTakeOut = 4;
 constexpr int kTakePreds = 2;  // dictionary-column leaves (==, !=, contains, regex, == NULL) evaluated from flat codes
@@ -356,14 +384,16 @@ struct FlatJob {
   uint32_t _pad;
 };
 
-// One PLAIN non-null int64 column chunk to restage as a frame-of-reference image (k_chunk_minmax, then k_narrow).
+// One PLAIN non-null int64 column chunk to restage as a frame-of-reference image and / or an exclusive prefix-sum image
+// (k_chunk_minmax, then k_narrow).
 struct NarrowJob {
   const long long* src;  // resident values
-  uint8_t* out;          // k_narrow: uint{8,16,32}(v - base) per row, 128-byte aligned, padded
+  uint8_t* out;          // k_narrow: uint{8,16,32}(v - base) per row, 128-byte aligned, padded (w == 0: none)
+  long long* pre;        // k_narrow: P[0 .. n_rows], P[i] = v[0] + ... + v[i-1] modulo 2^64 (null: none)
   long long base;        // k_narrow: the chunk minimum
   uint32_t n_rows, w;    // rows; k_narrow: bytes per row
   uint32_t first_block;  // prefix over the jobs of one launch: kNarrowRows-row blocks before this job
-  uint32_t _pad;
+  uint32_t sum_block;    // k_narrow: this job's first block in k_chunk_minmax's numbering (its block sums)
 };
 constexpr uint32_t kNarrowRows = 4096;
 

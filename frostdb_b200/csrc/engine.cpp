@@ -7,6 +7,7 @@
 #include <unistd.h>
 
 #include <algorithm>
+#include <array>
 #include <atomic>
 #include <chrono>
 #include <cmath>
@@ -241,7 +242,7 @@ extern "C" char** environ;
 // while the environment block looks unchanged (same array, same entry pointers: setenv / putenv replace an entry).
 const std::string& env_switches() {
   static const char* const kNames[] = {"FROSTGPU_NO_TILE", "FROSTGPU_NO_RUNS", "FROSTGPU_NO_PRUNE", "FROSTGPU_NO_FAST", "FROSTGPU_NO_FUSE",
-                                       "FROSTGPU_NO_TAKE", "FROSTGPU_TA_TILE", "FROSTGPU_TA_STAGES", "FROSTGPU_TA_GLOBAL", "FROSTGPU_TA_CHUNK", "FROSTGPU_TA_CARRY",
+                                       "FROSTGPU_NO_TAKE", "FROSTGPU_NO_PREFIX", "FROSTGPU_TA_TILE", "FROSTGPU_TA_STAGES", "FROSTGPU_TA_GLOBAL", "FROSTGPU_TA_CHUNK", "FROSTGPU_TA_CARRY",
                                        "FROSTGPU_VL", "FROSTGPU_RING", "FROSTGPU_RT_TILE", "FROSTGPU_RT_STAGES", "FROSTGPU_RT_SPAN", "FROSTGPU_RT_WARPS",
                                        "FROSTGPU_NO_EXEC_CACHE", "FROSTGPU_NO_PLAN_CACHE", "FROSTGPU_PROFILE"};
   static std::mutex mu;
@@ -542,23 +543,41 @@ int32_t ensure_flat(fgpu_ctx* ctx, Part* part, const std::string& column) {
 // stages 1, 2 or 4 bytes per row instead of 8.  Minimum and maximum come from the values on the device, not from the
 // footer statistics, so that a chunk without statistics narrows as well and wrong statistics cannot change a result.
 // The whole list costs one min / max launch, one synchronisation and one narrowing launch.
-int32_t ensure_narrow(fgpu_ctx* ctx, const std::vector<std::pair<Part*, std::string>>& want) {
+// want_prefix: (part, column) pairs that also get exclusive prefix-sum images for the prefix path of the sorted-run scan
+// (k_runs_prefix): every PLAIN non-null INT64 chunk, whatever its range, n_rows + 1 wrapping int64 sums (one allocation
+// per (part, column), kept until the part goes).  They are written by the same two launches: the min / max pass also
+// leaves every block's sum, the narrowing pass turns the values into the prefix, so the values are read no more often.
+int32_t ensure_narrow(fgpu_ctx* ctx, const std::vector<std::pair<Part*, std::string>>& want,
+                      const std::vector<std::pair<Part*, std::string>>& want_prefix) {
   struct Job {
     ColumnImage* img;
     ChunkHost* ch;
+    bool narrow, prefix;
   };
   std::vector<Job> host;
   std::vector<NarrowJob> jobs;
-  std::vector<ColumnImage*> imgs;
+  std::vector<ColumnImage*> imgs, pimgs;
   uint32_t blocks = 0;
-  for (const auto& pc : want) {
-    ColumnImage& img = pc.first->images[pc.second];
-    if (img.narrowed) continue;
-    if (!img.resident) return fail(FGPU_ERR_INVALID, "narrow image requested for a column that is not resident: " + pc.second);
-    img.narrowed = true;
-    imgs.push_back(&img);
-    for (RowGroupHost& rg : pc.first->rgs) {
-      auto it = rg.cols.find(pc.second);
+  std::map<std::pair<Part*, std::string>, std::pair<bool, bool>> todo;  // (narrow, prefix), in a fixed order
+  for (const auto& pc : want) todo[pc].first = true;
+  for (const auto& pc : want_prefix) todo[pc].second = true;
+  for (const auto& kv : todo) {
+    Part* part = kv.first.first;
+    const std::string& col = kv.first.second;
+    ColumnImage& img = part->images[col];
+    const bool nar = kv.second.first && !img.narrowed, pre = kv.second.second && !img.prefixed;
+    if (!nar && !pre) continue;
+    if (!img.resident) return fail(FGPU_ERR_INVALID, "narrow image requested for a column that is not resident: " + col);
+    if (nar) {
+      img.narrowed = true;
+      imgs.push_back(&img);
+    }
+    if (pre) {
+      img.prefixed = true;
+      pimgs.push_back(&img);
+    }
+    for (RowGroupHost& rg : part->rgs) {
+      auto it = rg.cols.find(col);
       if (it == rg.cols.end()) continue;
       ChunkHost& ch = it->second;
       if (!ch.error.empty() || ch.desc.kind != CK_PLAIN64 || ch.desc.has_nulls || ch.phys != PT_INT64 || rg.n_rows == 0) continue;
@@ -566,9 +585,10 @@ int32_t ensure_narrow(fgpu_ctx* ctx, const std::vector<std::pair<Part*, std::str
       j.src = reinterpret_cast<const long long*>(ch.desc.values);
       j.n_rows = rg.n_rows;
       j.first_block = blocks;
+      j.sum_block = blocks;
       blocks += (rg.n_rows + kNarrowRows - 1) / kNarrowRows;
       jobs.push_back(j);
-      host.push_back({&img, &ch});
+      host.push_back({&img, &ch, nar, pre});
     }
   }
   if (jobs.empty()) return FGPU_OK;
@@ -578,10 +598,11 @@ int32_t ensure_narrow(fgpu_ctx* ctx, const std::vector<std::pair<Part*, std::str
     mm[2 * i] = std::numeric_limits<long long>::max();
     mm[2 * i + 1] = std::numeric_limits<long long>::min();
   }
-  void* tmp = nullptr;  // [jobs][min, max per job]
-  CUDA_TRY(cudaMallocAsync(&tmp, jb + mmb, ctx->stream));
+  void* tmp = nullptr;  // [jobs][min, max per job][sum per block]
+  CUDA_TRY(cudaMallocAsync(&tmp, jb + mmb + size_t(blocks) * 8, ctx->stream));
   NarrowJob* d_jobs = static_cast<NarrowJob*>(tmp);
   long long* d_mm = reinterpret_cast<long long*>(static_cast<uint8_t*>(tmp) + jb);
+  unsigned long long* d_bsum = reinterpret_cast<unsigned long long*>(static_cast<uint8_t*>(tmp) + jb + mmb);
   auto upload = [&](const void* src, void* dst, size_t n) {
     if (void* pin = ctx->arena_take(n)) {
       std::memcpy(pin, src, n);
@@ -591,17 +612,23 @@ int32_t ensure_narrow(fgpu_ctx* ctx, const std::vector<std::pair<Part*, std::str
   };
   cudaError_t e = upload(jobs.data(), d_jobs, jb);
   if (e == cudaSuccess) e = upload(mm.data(), d_mm, mmb);
-  if (e == cudaSuccess) e = launch_chunk_minmax(d_jobs, uint32_t(jobs.size()), blocks, d_mm, ctx->stream);
+  if (e == cudaSuccess) e = launch_chunk_minmax(d_jobs, uint32_t(jobs.size()), blocks, d_mm, d_bsum, ctx->stream);
   if (e == cudaSuccess) e = cudaMemcpyAsync(mm.data(), d_mm, mmb, cudaMemcpyDeviceToHost, ctx->stream);
   if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-  // widths, then one image allocation per (part, column) and the narrowing pass over the chunks that fit 32 bits
-  std::map<ColumnImage*, uint64_t> bytes;
-  std::vector<uint64_t> offs(jobs.size());
+  // widths, then one image allocation per (part, column) and the narrowing pass over the chunks that fit 32 bits or want
+  // a prefix image
+  std::map<ColumnImage*, uint64_t> bytes, pbytes;
+  std::vector<uint64_t> offs(jobs.size()), poffs(jobs.size());
   std::vector<NarrowJob> pass2;
   uint32_t blocks2 = 0;
   for (size_t i = 0; i < jobs.size() && e == cudaSuccess; i++) {
+    if (host[i].prefix) {
+      uint64_t& b = pbytes[host[i].img];
+      poffs[i] = b;
+      b += (uint64_t(jobs[i].n_rows + 1) * 8 + 127) & ~uint64_t(127);
+    }
     const uint64_t range = uint64_t(mm[2 * i + 1]) - uint64_t(mm[2 * i]);
-    jobs[i].w = range <= 0xffu ? 1u : (range <= 0xffffu ? 2u : (range <= 0xffffffffu ? 4u : 0u));
+    jobs[i].w = !host[i].narrow ? 0u : range <= 0xffu ? 1u : (range <= 0xffffu ? 2u : (range <= 0xffffffffu ? 4u : 0u));
     if (!jobs[i].w) continue;  // needs 64 bits: read from the extent as before
     jobs[i].base = mm[2 * i];
     uint64_t& b = bytes[host[i].img];
@@ -613,21 +640,28 @@ int32_t ensure_narrow(fgpu_ctx* ctx, const std::vector<std::pair<Part*, std::str
     if (it == bytes.end() || e != cudaSuccess) continue;
     e = cudaMallocAsync(&img->narrow_dev, it->second, ctx->stream);
   }
+  for (ColumnImage* img : pimgs) {
+    auto it = pbytes.find(img);
+    if (it == pbytes.end() || e != cudaSuccess) continue;
+    e = cudaMallocAsync(&img->prefix_dev, it->second, ctx->stream);
+  }
   for (size_t i = 0; i < jobs.size() && e == cudaSuccess; i++) {
-    if (!jobs[i].w) continue;
-    jobs[i].out = static_cast<uint8_t*>(host[i].img->narrow_dev) + offs[i];
+    if (jobs[i].w) jobs[i].out = static_cast<uint8_t*>(host[i].img->narrow_dev) + offs[i];
+    if (host[i].prefix) jobs[i].pre = reinterpret_cast<long long*>(static_cast<uint8_t*>(host[i].img->prefix_dev) + poffs[i]);
+    if (!jobs[i].w && !jobs[i].pre) continue;
     jobs[i].first_block = blocks2;
     blocks2 += (jobs[i].n_rows + kNarrowRows - 1) / kNarrowRows;
     pass2.push_back(jobs[i]);
   }
   if (e == cudaSuccess && !pass2.empty()) e = upload(pass2.data(), d_jobs, pass2.size() * sizeof(NarrowJob));
-  if (e == cudaSuccess) e = launch_narrow(d_jobs, uint32_t(pass2.size()), blocks2, ctx->stream);
+  if (e == cudaSuccess) e = launch_narrow(d_jobs, uint32_t(pass2.size()), blocks2, d_bsum, ctx->stream);
   cudaFreeAsync(tmp, ctx->stream);
   if (e != cudaSuccess) {
     cudaGetLastError();
     return fail(FGPU_ERR_CUDA, std::string("narrow images: ") + cudaGetErrorString(e));
   }
   for (size_t i = 0; i < jobs.size(); i++) {
+    if (jobs[i].pre) host[i].ch->prefix = jobs[i].pre;
     if (!jobs[i].w) continue;
     host[i].ch->narrow = jobs[i].out;
     host[i].ch->narrow_w = uint8_t(jobs[i].w);
@@ -651,6 +685,7 @@ void free_part(fgpu_ctx* ctx, Part* p) {
     if (kv.second.dev) cudaFreeAsync(kv.second.dev, ctx->stream);
     if (kv.second.flat_dev) cudaFreeAsync(kv.second.flat_dev, ctx->stream);
     if (kv.second.narrow_dev) cudaFreeAsync(kv.second.narrow_dev, ctx->stream);
+    if (kv.second.prefix_dev) cudaFreeAsync(kv.second.prefix_dev, ctx->stream);
   }
 }
 
@@ -774,6 +809,8 @@ struct ExecCache {
   bool has_runs = false, has_ta = false;
   RunsDesc rd{};
   int runs_nl = 0, runs_nk = 0, runs_na = 0;
+  bool has_prefix = false;
+  PrefixDesc pd{};
   TileAggDesc td{};
   fgpu_stats stats{};             // everything about the scan that does not change between Executes
   std::vector<KeyOut> keys;       // with the dictionary snapshots
@@ -1745,6 +1782,7 @@ int32_t run_cached(fgpu_ctx* ctx, ExecCache& x, fgpu_result* res, int collective
   if (x.has_runs) {
     CUDA_TRY(launch_runs_tma(x.rd, x.runs_nl, x.runs_nk, x.runs_na, ctx->sm_count, s));
   }
+  if (x.has_prefix) CUDA_TRY(launch_runs_prefix(x.pd, ctx->sm_count, s));
   if (x.has_ta) CUDA_TRY(launch_tile_agg(x.td, ctx->sm_count, s));
   CUDA_TRY(launch_scan(x.qdesc_dev, x.qd, ctx->sm_count, s));
   CUDA_TRY(cudaEventRecord(ctx->ev[2], s));
@@ -1848,6 +1886,18 @@ int32_t run_scan(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, fgpu_result* re
     size_t o_rg = 0, o_span = 0;
   };
   RunsBatch batches[1];
+  // Row groups of the sorted-run shape whose filter the statistics decided, without undecided dictionary leaves and with
+  // Sum(int64) as the only stored aggregates, are answered from prefix sums instead (k_runs_prefix, runs_prefix.cu) when
+  // their runs average at least kPrefixRunRows rows: then a step per group run is cheaper than reading its rows.
+  constexpr uint64_t kPrefixRunRows = 64;
+  struct PrefixBatch {
+    PrefixDesc pd{};
+    std::vector<PrefixRg> rgs;
+    std::vector<std::array<ChunkHost*, kRunsAggs>> sums;  // per row group: the chunk of every Sum input
+    std::vector<Part*> parts;
+    std::vector<PrefixWin> wins;
+    size_t o_rg = 0, o_win = 0;
+  } PB;
   int runs_nl = 0, runs_nk = 0, runs_na = 0, runs_np = 0;
   int runs_leaf_index[kRunsLeaves] = {0}, runs_pred_leaf[kRunsPreds] = {0};  // query leaf behind every range / dictionary leaf
   int runs_leaf_slot[kRunsLeaves] = {0}, runs_agg_slot[kRunsAggs] = {0}, runs_agg_index[kRunsAggs] = {0};
@@ -1879,6 +1929,9 @@ int32_t run_scan(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, fgpu_result* re
     if (qd.n_keys > kRunsKeys) runs_q = false;
     runs_nk = qd.n_keys;
   }
+  bool prefix_q = runs_q && !getenv("FROSTGPU_NO_PREFIX");
+  for (int a = 0; a < runs_na && prefix_q; a++)
+    if (runs_agg_func[a] != uint32_t(FGPU_AGG_SUM)) prefix_q = false;  // Min / Max / float64 Sum stay with k_runs_tma
   if (runs_q) {  // distinct staged columns of each batch
     for (int bi = 0; bi < 1; bi++) {
       RunsBatch& B = batches[bi];
@@ -2077,6 +2130,44 @@ int32_t run_scan(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, fgpu_result* re
         rr.n_runs[k] = d.n_row_runs;
       }
     }
+    if (runs_ok && prefix_q && (runs_nl == 0 || all_pass)) {  // (the kernel treats a launch without range leaves as all-pass)
+      bool ok = true;
+      uint64_t sum_runs = 0;
+      for (int i = 0; i < runs_np; i++)
+        if (rr.pred_runs[i]) ok = false;  // an undecided dictionary leaf
+      for (int k = 0; k < runs_nk; k++) sum_runs += rr.n_runs[k];
+      std::array<ChunkHost*, kRunsAggs> sums{};
+      for (int a = 0; a < runs_na && ok; a++) {
+        sums[size_t(a)] = rcols.ch[batches[bi].rd.agg_col[a]];
+        if (!sums[size_t(a)] || sums[size_t(a)]->phys != PT_INT64) ok = false;
+      }
+      if (ok && uint64_t(rg.n_rows) >= kPrefixRunRows * sum_runs) {
+        PrefixRg pr{};
+        pr.n_rows = rg.n_rows;
+        for (int k = 0; k < runs_nk; k++) {
+          pr.runs[k] = rr.runs[k];
+          pr.seeds[k] = rr.seeds[k];
+          pr.n_runs[k] = rr.n_runs[k];
+          st.algorithmic_bytes += uint64_t(rr.n_runs[k]) * sizeof(Run);  // the directories, read whole
+        }
+        const uint32_t win = runs_prefix_window_rows(rg.n_rows, uint32_t(sum_runs));
+        uint32_t n_win = 0;
+        for (uint32_t r0 = 0; r0 < rg.n_rows; r0 += win, n_win++)
+          PB.wins.push_back(PrefixWin{uint32_t(PB.rgs.size()), r0, std::min(win, rg.n_rows - r0), 0u});
+        // a Sum input is read at the segment boundaries (at most every run start, every window start and the end), not
+        // row by row
+        for (int a = 0; a < runs_na; a++) {
+          bool first = true;
+          for (int a2 = 0; a2 < a; a2++) first = first && sums[size_t(a2)] != sums[size_t(a)];
+          if (first) st.algorithmic_bytes = st.algorithmic_bytes - sums[size_t(a)]->stored_bytes + (sum_runs + n_win + 1) * 8;
+        }
+        PB.rgs.push_back(pr);
+        PB.sums.push_back(sums);
+        PB.parts.push_back(rcols.part);
+        lut_fix.erase(std::remove_if(lut_fix.begin(), lut_fix.end(), [&](const std::pair<size_t, size_t>& f) { return f.first >= size_t(g) * n_leaves; }), lut_fix.end());
+        continue;  // slot g of the general tables is reused by the next row group
+      }
+    }
     if (runs_ok) {
       batches[bi].rgs.push_back(rr);
       batches[bi].cols.push_back(rcols);
@@ -2157,21 +2248,31 @@ int32_t run_scan(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, fgpu_result* re
   first_tile[size_t(gi)] = tiles;
   qd.n_rg = gi;
   qd.n_tiles = tiles;
-  // ---- sorted-run kernel: frame-of-reference images, tile rows, stage layout ------------------------
+  // ---- sorted-run kernels: frame-of-reference and prefix-sum images, tile rows, stage layout ------------------------
+  {  // every staged int64 column and every Sum input of the prefix path of every part, in one batch
+    std::set<std::pair<Part*, std::string>> seen, pseen;
+    std::vector<std::pair<Part*, std::string>> want, want_prefix;
+    for (const RunsBatch& B : batches)
+      for (const RunsRgCols& rc2 : B.cols)
+        for (uint32_t i = 0; i < B.rd.n_cols; i++)
+          if (rc2.ch[i] && rc2.ch[i]->phys == PT_INT64 && seen.emplace(rc2.part, c.slot_names[size_t(B.col_slot[i])]).second)
+            want.emplace_back(rc2.part, c.slot_names[size_t(B.col_slot[i])]);
+    for (size_t k = 0; k < PB.rgs.size(); k++)
+      for (int a = 0; a < runs_na; a++)
+        if (pseen.emplace(PB.parts[k], c.slot_names[size_t(runs_agg_slot[a])]).second) want_prefix.emplace_back(PB.parts[k], c.slot_names[size_t(runs_agg_slot[a])]);
+    if (!want.empty() || !want_prefix.empty())
+      if (int32_t rcn = ensure_narrow(ctx, want, want_prefix)) return rcn;
+    for (size_t k = 0; k < PB.rgs.size(); k++)
+      for (int a = 0; a < runs_na; a++) {
+        PB.rgs[k].pre[a] = PB.sums[k][size_t(a)]->prefix;
+        if (!PB.rgs[k].pre[a]) return fail(FGPU_ERR_INVALID, "prefix-sum image missing for column " + c.slot_names[size_t(runs_agg_slot[a])]);
+      }
+  }
   for (RunsBatch& B : batches) {
     if (B.rgs.empty()) continue;
     RunsDesc& rd = B.rd;
     auto envi = [](const char* n, int d) { const char* e = getenv(n); return e ? atoi(e) : d; };
     rd.n_rg = uint32_t(B.rgs.size());
-    {  // every staged int64 column of every part, narrowed in one batch
-      std::set<std::pair<Part*, std::string>> seen;
-      std::vector<std::pair<Part*, std::string>> want;
-      for (const RunsRgCols& rc2 : B.cols)
-        for (uint32_t i = 0; i < rd.n_cols; i++)
-          if (rc2.ch[i] && rc2.ch[i]->phys == PT_INT64 && seen.emplace(rc2.part, c.slot_names[size_t(B.col_slot[i])]).second)
-            want.emplace_back(rc2.part, c.slot_names[size_t(B.col_slot[i])]);
-      if (int32_t rcn = ensure_narrow(ctx, want)) return rcn;
-    }
     // every row group is cut into tiles of about tile_bytes of staged column data; the launch's tile table {row group,
     // first row} is dealt to the CTAs in chunks of consecutive entries
     uint32_t tile_bytes = 4096 * 8;
@@ -2427,6 +2528,11 @@ int32_t run_scan(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, fgpu_result* re
     B.o_span = align16(B.o_rg + B.rgs.size() * sizeof(RunsRg));
     o_cnt = align16(B.o_span + B.first_span.size() * 4);
   }
+  if (!PB.rgs.empty()) {
+    PB.o_rg = o_cnt;
+    PB.o_win = align16(PB.o_rg + PB.rgs.size() * sizeof(PrefixRg));
+    o_cnt = align16(PB.o_win + PB.wins.size() * sizeof(PrefixWin));
+  }
   if (!TA.rgs.empty()) {
     TA.o_rg = o_cnt;
     TA.o_tile = align16(TA.o_rg + TA.rgs.size() * sizeof(TileAggRg));
@@ -2462,6 +2568,10 @@ int32_t run_scan(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, fgpu_result* re
         if (r.pred_runs[i]) r.pred_lut[i] = aux + o_lut + size_t(uintptr_t(r.pred_lut[i]));
     std::memcpy(hostaux.data() + B.o_rg, B.rgs.data(), B.rgs.size() * sizeof(RunsRg));
     std::memcpy(hostaux.data() + B.o_span, B.first_span.data(), B.first_span.size() * 4);
+  }
+  if (!PB.rgs.empty()) {
+    std::memcpy(hostaux.data() + PB.o_rg, PB.rgs.data(), PB.rgs.size() * sizeof(PrefixRg));
+    std::memcpy(hostaux.data() + PB.o_win, PB.wins.data(), PB.wins.size() * sizeof(PrefixWin));
   }
   if (!TA.rgs.empty()) {
     for (TileAggRg& r : TA.rgs)
@@ -2534,6 +2644,22 @@ int32_t run_scan(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, fgpu_result* re
       CUDA_TRY(launch_runs_tma(rd, B.nl, runs_nk, runs_na, ctx->sm_count, s));
       st.kernel_launches++;
       st.row_groups_runs += uint32_t(B.rgs.size());
+    }
+    if (!PB.rgs.empty()) {
+      PrefixDesc& pd = PB.pd;
+      pd.n_win = uint32_t(PB.wins.size());
+      pd.nk = uint32_t(runs_nk);
+      pd.na = uint32_t(runs_na);
+      for (int k = 0; k < runs_nk; k++) pd.stride[k] = qd.keys[k].dense_stride;
+      pd.rgs = reinterpret_cast<const PrefixRg*>(aux + PB.o_rg);
+      pd.wins = reinterpret_cast<const PrefixWin*>(aux + PB.o_win);
+      pd.t_rows = qd.t_rows;
+      for (int a = 0; a < runs_na; a++) pd.t_agg[a] = qd.t_agg[runs_agg_index[a]];
+      pd.counters = qd.counters;
+      CUDA_TRY(launch_runs_prefix(pd, ctx->sm_count, s));
+      st.kernel_launches++;
+      st.row_groups_runs += uint32_t(PB.rgs.size());
+      st.row_groups_prefix += uint32_t(PB.rgs.size());
     }
     if (!TA.rgs.empty()) {
       TileAggDesc& td = TA.td;
@@ -2621,6 +2747,8 @@ int32_t run_scan(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, fgpu_result* re
     x.runs_nl = batches[0].nl;
     x.runs_nk = runs_nk;
     x.runs_na = runs_na;
+    x.has_prefix = !PB.rgs.empty();
+    x.pd = PB.pd;
     x.has_ta = !TA.rgs.empty();
     x.td = TA.td;
     x.keys = c.keys;

@@ -2169,9 +2169,13 @@ cudaError_t launch_flatten(const FlatJob* d_jobs, uint32_t n_jobs, uint32_t tota
 }
 
 // ======================================================================================================
-// Frame-of-reference images of PLAIN int64 chunks for the sorted-run kernel (runs_tma.cu).
-//   k_chunk_minmax: min / max of every job's chunk into mm[2 j], mm[2 j + 1] (preset to INT64_MAX / INT64_MIN).
-//   k_narrow:       out[r] = uint{8,16,32}(src[r] - base) for the jobs whose range fits 32 bits.
+// Frame-of-reference and prefix-sum images of PLAIN int64 chunks for the sorted-run kernels (runs_tma.cu,
+// runs_prefix.cu).
+//   k_chunk_minmax: min / max of every job's chunk into mm[2 j], mm[2 j + 1] (preset to INT64_MAX / INT64_MIN), and
+//                   the wrapping sum of every block into bsum[block].
+//   k_narrow:       out[r] = uint{8,16,32}(src[r] - base) for the jobs whose range fits 32 bits; pre[r] = the wrapping
+//                   sum of src[0 .. r) for the jobs that want a prefix image (the block's offset is the sum of the
+//                   block sums before it).
 // One CTA per kNarrowRows-row block of one job.
 // ======================================================================================================
 __device__ __forceinline__ uint32_t narrow_job(const NarrowJob* jobs, uint32_t n_jobs, uint32_t blk) {
@@ -2183,58 +2187,108 @@ __device__ __forceinline__ uint32_t narrow_job(const NarrowJob* jobs, uint32_t n
   return lo;
 }
 
-__global__ void __launch_bounds__(NT) k_chunk_minmax(const NarrowJob* __restrict__ jobs, uint32_t n_jobs, long long* mm) {
+__global__ void __launch_bounds__(NT) k_chunk_minmax(const NarrowJob* __restrict__ jobs, uint32_t n_jobs, long long* mm,
+                                                     unsigned long long* bsum) {
   __shared__ long long s_lo[NWARP], s_hi[NWARP];
+  __shared__ unsigned long long s_sum[NWARP];
   const uint32_t j = narrow_job(jobs, n_jobs, blockIdx.x);
   const NarrowJob& J = jobs[j];
   const uint32_t r0 = (blockIdx.x - J.first_block) * kNarrowRows, r1 = min(J.n_rows, r0 + kNarrowRows);
   long long lo = LLONG_MAX, hi = LLONG_MIN;
+  unsigned long long sum = 0;
   for (uint32_t r = r0 + threadIdx.x; r < r1; r += NT) {
     const long long v = __ldg(J.src + r);
     lo = min(lo, v);
     hi = max(hi, v);
+    sum += (unsigned long long)v;
   }
   for (int o = 16; o; o >>= 1) {
     lo = min(lo, __shfl_xor_sync(0xffffffffu, lo, o));
     hi = max(hi, __shfl_xor_sync(0xffffffffu, hi, o));
+    sum += __shfl_xor_sync(0xffffffffu, sum, o);
   }
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   if (lane == 0) {
     s_lo[warp] = lo;
     s_hi[warp] = hi;
+    s_sum[warp] = sum;
   }
   __syncthreads();
   if (threadIdx.x == 0) {
     for (int w = 1; w < NWARP; w++) {
       lo = min(lo, s_lo[w]);
       hi = max(hi, s_hi[w]);
+      sum += s_sum[w];
     }
     atomicMin(mm + 2 * j, lo);
     atomicMax(mm + 2 * j + 1, hi);
+    bsum[blockIdx.x] = sum;
   }
 }
 
-__global__ void __launch_bounds__(NT) k_narrow(const NarrowJob* __restrict__ jobs, uint32_t n_jobs) {
+// exclusive sum over the CTA of one value per thread (wrapping); also returns the CTA total
+__device__ __forceinline__ unsigned long long cta_exclusive_sum(unsigned long long v, unsigned long long* s_warp, unsigned long long* total) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  unsigned long long inc = v;
+  for (int o = 1; o < 32; o <<= 1) {
+    const unsigned long long t = __shfl_up_sync(0xffffffffu, inc, o);
+    if (lane >= o) inc += t;
+  }
+  if (lane == 31) s_warp[warp] = inc;
+  __syncthreads();
+  unsigned long long before = 0, all = 0;
+  for (int w = 0; w < NWARP; w++) {
+    const unsigned long long t = s_warp[w];
+    before += w < warp ? t : 0ull;
+    all += t;
+  }
+  __syncthreads();  // s_warp is reused by the next call
+  *total = all;
+  return before + inc - v;
+}
+
+__global__ void __launch_bounds__(NT) k_narrow(const NarrowJob* __restrict__ jobs, uint32_t n_jobs, const unsigned long long* __restrict__ bsum) {
+  __shared__ unsigned long long s_warp[NWARP];
   const NarrowJob& J = jobs[narrow_job(jobs, n_jobs, blockIdx.x)];
-  const uint32_t r0 = (blockIdx.x - J.first_block) * kNarrowRows, r1 = min(J.n_rows, r0 + kNarrowRows), w = J.w;
+  const uint32_t blk = blockIdx.x - J.first_block;
+  const uint32_t r0 = blk * kNarrowRows, r1 = min(J.n_rows, r0 + kNarrowRows), w = J.w;
   const unsigned long long base = (unsigned long long)J.base;
-  for (uint32_t r = r0 + threadIdx.x; r < r1; r += NT) {
-    const unsigned long long d = (unsigned long long)__ldg(J.src + r) - base;  // < 2^(8 w): the host chose w from the range
-    if (w == 1) J.out[r] = uint8_t(d);
-    else if (w == 2) reinterpret_cast<uint16_t*>(J.out)[r] = uint16_t(d);
-    else reinterpret_cast<uint32_t*>(J.out)[r] = uint32_t(d);
+  long long* const pre = J.pre;
+  unsigned long long carry = 0;  // prefix image: the wrapping sum of the rows before the current step
+  if (pre) {
+    unsigned long long t = 0;
+    for (uint32_t b = threadIdx.x; b < blk; b += NT) t += __ldg(bsum + J.sum_block + b);
+    cta_exclusive_sum(t, s_warp, &carry);
   }
+  for (uint32_t s = r0; s < r1; s += NT) {  // uniform trip count: the prefix steps synchronise the CTA
+    const uint32_t r = s + threadIdx.x;
+    const unsigned long long v = r < r1 ? (unsigned long long)__ldg(J.src + r) : 0ull;
+    if (w && r < r1) {
+      const unsigned long long d = v - base;  // < 2^(8 w): the host chose w from the range
+      if (w == 1) J.out[r] = uint8_t(d);
+      else if (w == 2) reinterpret_cast<uint16_t*>(J.out)[r] = uint16_t(d);
+      else reinterpret_cast<uint32_t*>(J.out)[r] = uint32_t(d);
+    }
+    if (pre) {
+      unsigned long long step = 0;
+      const unsigned long long ex = cta_exclusive_sum(v, s_warp, &step);
+      if (r < r1) pre[r] = (long long)(carry + ex);
+      carry += step;
+    }
+  }
+  if (pre && r1 == J.n_rows && threadIdx.x == 0) pre[r1] = (long long)carry;  // P[n]: the chunk's sum
 }
 
-cudaError_t launch_chunk_minmax(const NarrowJob* d_jobs, uint32_t n_jobs, uint32_t total_blocks, long long* d_mm, cudaStream_t st) {
+cudaError_t launch_chunk_minmax(const NarrowJob* d_jobs, uint32_t n_jobs, uint32_t total_blocks, long long* d_mm, unsigned long long* d_bsum,
+                                cudaStream_t st) {
   if (n_jobs == 0 || total_blocks == 0) return cudaSuccess;
-  k_chunk_minmax<<<total_blocks, NT, 0, st>>>(d_jobs, n_jobs, d_mm);
+  k_chunk_minmax<<<total_blocks, NT, 0, st>>>(d_jobs, n_jobs, d_mm, d_bsum);
   return cudaGetLastError();
 }
 
-cudaError_t launch_narrow(const NarrowJob* d_jobs, uint32_t n_jobs, uint32_t total_blocks, cudaStream_t st) {
+cudaError_t launch_narrow(const NarrowJob* d_jobs, uint32_t n_jobs, uint32_t total_blocks, const unsigned long long* d_bsum, cudaStream_t st) {
   if (n_jobs == 0 || total_blocks == 0) return cudaSuccess;
-  k_narrow<<<total_blocks, NT, 0, st>>>(d_jobs, n_jobs);
+  k_narrow<<<total_blocks, NT, 0, st>>>(d_jobs, n_jobs, d_bsum);
   return cudaGetLastError();
 }
 

@@ -25,6 +25,9 @@ void runs_tma_plan(RunsDesc& d, int nq, uint32_t max_tile, uint32_t col_region, 
 size_t runs_tma_smem_bytes(const RunsDesc& d);
 int runs_tma_ctas_per_sm(const RunsDesc& d);
 cudaError_t launch_runs_tma(const RunsDesc& d, int nl, int nk, int na, int sm_count, cudaStream_t st);
+// all-pass sorted row groups from the key run directories and prefix-sum images (runs_prefix.cu)
+uint32_t runs_prefix_window_rows(uint32_t n_rows, uint32_t sum_runs);  // rows per window of one row group
+cudaError_t launch_runs_prefix(const PrefixDesc& d, int sm_count, cudaStream_t st);
 // filter-only plans over PLAIN columns (take_rows.cu): count per span, scan, ordered write
 cudaError_t launch_take(const TakeDesc& d, int sm_count, cudaStream_t st);
 int take_resident_warps(int sm_count);
@@ -33,9 +36,11 @@ cudaError_t launch_tile_agg(const TileAggDesc& d, int sm_count, cudaStream_t st)
 size_t tile_agg_smem_bytes(const TileAggDesc& d);
 // dictionary column chunks -> flat code arrays (kernels.cu)
 cudaError_t launch_flatten(const FlatJob* d_jobs, uint32_t n_jobs, uint32_t total_blocks, int sm_count, cudaStream_t st);
-// PLAIN int64 column chunks -> frame-of-reference images (kernels.cu): min / max per job, then the narrowing pass
-cudaError_t launch_chunk_minmax(const NarrowJob* d_jobs, uint32_t n_jobs, uint32_t total_blocks, long long* d_mm, cudaStream_t st);
-cudaError_t launch_narrow(const NarrowJob* d_jobs, uint32_t n_jobs, uint32_t total_blocks, cudaStream_t st);
+// PLAIN int64 column chunks -> frame-of-reference and prefix-sum images (kernels.cu): min / max per job and the sum of
+// every block, then the narrowing / prefix pass
+cudaError_t launch_chunk_minmax(const NarrowJob* d_jobs, uint32_t n_jobs, uint32_t total_blocks, long long* d_mm, unsigned long long* d_bsum,
+                                cudaStream_t st);
+cudaError_t launch_narrow(const NarrowJob* d_jobs, uint32_t n_jobs, uint32_t total_blocks, const unsigned long long* d_bsum, cudaStream_t st);
 // partial-table exchange over peer-mapped mailboxes (comm.cu)
 cudaError_t launch_comm_push(const CommPush& p, int sm_count, cudaStream_t st);
 cudaError_t launch_comm_wait(const CommWait& w, cudaStream_t st);

@@ -60,6 +60,9 @@ struct ChunkHost {
   const uint8_t* narrow = nullptr;
   uint8_t narrow_w = 0;
   int64_t narrow_base = 0;
+  // exclusive prefix sums of a PLAIN non-null INT64 chunk, n_rows + 1 entries modulo 2^64 (device pointer; derived on
+  // first use by the prefix path of the sorted-run scan, see ensure_narrow)
+  const long long* prefix = nullptr;
 };
 
 struct RowGroupHost {
@@ -89,6 +92,8 @@ struct ColumnImage {
   void* flat_dev = nullptr;      // flat code arrays of every row group of this column (one allocation) + the job table
   bool narrowed = false;         // ensure_narrow ran (narrow_dev stays null when no chunk fits 32 bits)
   void* narrow_dev = nullptr;    // frame-of-reference images of every narrowed chunk of this column (one allocation)
+  bool prefixed = false;         // ensure_narrow built the prefix-sum images
+  void* prefix_dev = nullptr;    // prefix-sum images of every PLAIN non-null INT64 chunk of this column (one allocation)
 };
 
 struct Part {

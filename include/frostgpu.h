@@ -170,7 +170,7 @@ typedef struct fgpu_stats {
   uint32_t row_groups_pruned; /* ruled out by chunk statistics before upload (index/lsm.go:437)      */
   uint32_t row_groups_runs;   /* scanned by the sorted-run kernel                                   */
   uint32_t row_groups_tiles;  /* scanned by the tile-aggregate kernel (the rest: general scan kernel) */
-  uint32_t _reserved;
+  uint32_t row_groups_prefix; /* of row_groups_runs: all-pass row groups answered from prefix sums     */
   uint64_t rows_touched;      /* rows of the row groups that survived pruning (what the kernels read)  */
 } fgpu_stats;
 

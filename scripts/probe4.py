@@ -1,6 +1,6 @@
-"""Probe of the sorted-run kernel k_runs_tma on PROBE_ROWS (default 32 Mi) sorted rows (runs on a GPU): kernel time of
-a set of plan shapes, then a sweep of tile bytes / ring stages / consumer warps / chunk tiles (FROSTGPU_RT_*), every
-result compared row by row with the default shape's."""
+"""Probe of the sorted-run kernels k_runs_tma / k_runs_prefix on PROBE_ROWS (default 32 Mi) sorted rows (runs on a GPU):
+kernel time of a set of plan shapes with and without the prefix path (FROSTGPU_NO_PREFIX), then a sweep of tile bytes /
+ring stages / consumer warps / chunk tiles (FROSTGPU_RT_*), every result compared row by row with the default shape's."""
 import ctypes as C, os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
@@ -60,7 +60,7 @@ def run(table, name, kind, f, groups, aggs, env=None):
         ref = results.setdefault((table, name), got)
         same = "same" if ref == got else "DIFFERENT"
         print(f"{name:44s} {tag:30s} kernel_ms {k:7.4f} exec_ms {min(wall[1:]):7.3f} GB/s {st['algorithmic_bytes'] / k / 1e6:7.1f} "
-              f"sel {st['rows_selected']:>9d} groups {st['groups']:>6d} rg runs/tiles/all {st['row_groups_runs']}/{st['row_groups_tiles']}/{st['row_groups']} {same}", flush=True)
+              f"sel {st['rows_selected']:>9d} groups {st['groups']:>6d} rg prefix/runs/tiles/all {st['row_groups_prefix']}/{st['row_groups_runs']}/{st['row_groups_tiles']}/{st['row_groups']} {same}", flush=True)
         lib.fgpu_query_free(q)
     finally:
         for a in env:
@@ -88,6 +88,7 @@ cases = [
 ]
 for name, f, g, a in cases:
     run("s", name, AGG, f, g, a)
+    run("s", name, AGG, f, g, a, {"FROSTGPU_NO_PREFIX": "1"})  # the same row groups through k_runs_tma
 if os.environ.get("PROBE_NOSWEEP"):
     sys.exit(0)
 def sweep(ci, combos):
