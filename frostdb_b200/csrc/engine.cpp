@@ -236,33 +236,66 @@ struct fgpu_ctx {
   }
 };
 
-// FROSTGPU_PROFILE=1: host-side phase times of every Execute on stderr (development aid).
+// The FROSTGPU_* development switches (tests and measurements use them to force a kernel or a layout), parsed.  A
+// NO_* switch, TA_GLOBAL, TA_CARRY and PROFILE are on when they are set at all.  `key` lists every switch that is set
+// (NAME=value;): a compiled plan is only reused under the key it was compiled with.
+struct Switches {
+  bool no_tile = false, no_runs = false, no_prune = false, no_fast = false, no_fuse = false, no_take = false, no_prefix = false;
+  bool no_exec_cache = false, no_plan_cache = false, profile = false;  // profile: host phase times of every Execute on stderr
+  bool ta_global = false, ta_carry = false;      // tile kernel: table in global memory; never the carry-free 32-bit Sums
+  int ta_tile = 0, ta_stages = 0, ta_chunk = 0;  // tile kernel: forced tile rows, ring depth, tiles per CTA turn (0: chosen)
+  int vl = 256, ring = 3;                        // scan kernel: rows per warp vector, ring depth
+  int rt_tile = 4096, rt_stages = 0, rt_span = 0, rt_warps = 0;  // sorted-run kernel: tile rows, forced layout (0: chosen)
+  std::string key;
+};
+
+Switches read_switches() {
+  Switches w;
+  auto get = [&w](const char* name) {  // every switch read lands in the key
+    const char* v = getenv(name);
+    if (v) { w.key += name; w.key += '='; w.key += v; w.key += ';'; }
+    return v;
+  };
+  auto num = [&get](const char* name, int d) { const char* v = get(name); return v ? atoi(v) : d; };
+  static const std::pair<const char*, bool Switches::*> kFlags[] = {
+      {"FROSTGPU_NO_TILE", &Switches::no_tile},     {"FROSTGPU_NO_RUNS", &Switches::no_runs},     {"FROSTGPU_NO_PRUNE", &Switches::no_prune},
+      {"FROSTGPU_NO_FAST", &Switches::no_fast},     {"FROSTGPU_NO_FUSE", &Switches::no_fuse},     {"FROSTGPU_NO_TAKE", &Switches::no_take},
+      {"FROSTGPU_NO_PREFIX", &Switches::no_prefix}, {"FROSTGPU_TA_GLOBAL", &Switches::ta_global}, {"FROSTGPU_TA_CARRY", &Switches::ta_carry},
+      {"FROSTGPU_NO_EXEC_CACHE", &Switches::no_exec_cache}, {"FROSTGPU_NO_PLAN_CACHE", &Switches::no_plan_cache}, {"FROSTGPU_PROFILE", &Switches::profile}};
+  for (const auto& f : kFlags) w.*f.second = get(f.first) != nullptr;
+  w.ta_tile = num("FROSTGPU_TA_TILE", 0);
+  w.ta_stages = num("FROSTGPU_TA_STAGES", 0);
+  if (const char* v = get("FROSTGPU_TA_CHUNK")) w.ta_chunk = std::max(1, atoi(v));
+  w.vl = num("FROSTGPU_VL", 256);
+  if (w.vl != 128 && w.vl != 256 && w.vl != 512 && w.vl != 1024) w.vl = 512;
+  w.ring = std::min(4, std::max(2, num("FROSTGPU_RING", 3)));
+  const int rt = num("FROSTGPU_RT_TILE", 0);
+  if (rt == 1024 || rt == 2048 || rt == 4096 || rt == 8192) w.rt_tile = rt;
+  w.rt_stages = num("FROSTGPU_RT_STAGES", 0);
+  w.rt_span = num("FROSTGPU_RT_SPAN", 0);
+  w.rt_warps = num("FROSTGPU_RT_WARPS", 0);
+  return w;
+}
+
 extern "C" char** environ;
-// The FROSTGPU_* development switches as one string.  Called per Execute: the scan of the environment is skipped
-// while the environment block looks unchanged (same array, same entry pointers: setenv / putenv replace an entry).
-const std::string& env_switches() {
-  static const char* const kNames[] = {"FROSTGPU_NO_TILE", "FROSTGPU_NO_RUNS", "FROSTGPU_NO_PRUNE", "FROSTGPU_NO_FAST", "FROSTGPU_NO_FUSE",
-                                       "FROSTGPU_NO_TAKE", "FROSTGPU_NO_PREFIX", "FROSTGPU_TA_TILE", "FROSTGPU_TA_STAGES", "FROSTGPU_TA_GLOBAL", "FROSTGPU_TA_CHUNK", "FROSTGPU_TA_CARRY",
-                                       "FROSTGPU_VL", "FROSTGPU_RING", "FROSTGPU_RT_TILE", "FROSTGPU_RT_STAGES", "FROSTGPU_RT_SPAN", "FROSTGPU_RT_WARPS",
-                                       "FROSTGPU_NO_EXEC_CACHE", "FROSTGPU_NO_PLAN_CACHE", "FROSTGPU_PROFILE"};
+// Called per Execute: the environment is only parsed again when its block looks changed (same array, same entry
+// pointers: setenv / putenv replace an entry).
+Switches switches() {
   static std::mutex mu;
-  static std::string cached;
+  static Switches cached;
   static uint64_t cached_sig = 0;
   uint64_t sig = 0x9e3779b97f4a7c15ull ^ uint64_t(reinterpret_cast<uintptr_t>(environ));
   for (char** e = environ; e && *e; e++) sig = (sig ^ uint64_t(reinterpret_cast<uintptr_t>(*e))) * 0x100000001b3ull;
   std::lock_guard<std::mutex> lk(mu);
   if (sig != cached_sig || cached_sig == 0) {
-    cached.clear();
-    for (const char* n : kNames) {
-      const char* v = getenv(n);
-      if (v) { cached += n; cached += '='; cached += v; cached += ';'; }
-    }
+    cached = read_switches();
     cached_sig = sig;
   }
   return cached;
 }
+
 struct PhaseClock {
-  bool on = env_switches().find("FROSTGPU_PROFILE") != std::string::npos;
+  bool on = switches().profile;
   std::chrono::steady_clock::time_point t0 = std::chrono::steady_clock::now();
   std::string line;
   void mark(const char* what) {
@@ -790,6 +823,16 @@ uint8_t chunk_leaf_mode(int64_t lo, int64_t hi, bool neg, bool has_bounds, int64
   return stats_leaf_mode(lo, hi, neg, mn, mx, null_count == 0);
 }
 
+// The launches of an aggregate scan between k_table_init and the general k_scan, in issue order: sorted runs
+// (k_runs_tma), prefix sums (k_runs_prefix), tile aggregate (k_tile_agg).
+struct ScanLaunch {
+  bool runs = false, prefix = false, tile = false;
+  RunsDesc rd{};
+  int runs_nl = 0, runs_nk = 0, runs_na = 0;
+  PrefixDesc pd{};
+  TileAggDesc td{};
+};
+
 // Device and page-locked state of a compiled plan that every Execute of a prepared query reuses while the plan is
 // valid (same table epoch, same read transaction): the descriptor block is uploaded once, the aggregate table and
 // its counters are one persistent allocation, and the table comes back to page-locked memory with ONE copy and ONE
@@ -806,15 +849,9 @@ struct ExecCache {
   bool ready = false;
   QueryDesc qd{};
   const QueryDesc* qdesc_dev = nullptr;
-  bool has_runs = false, has_ta = false;
-  RunsDesc rd{};
-  int runs_nl = 0, runs_nk = 0, runs_na = 0;
-  bool has_prefix = false;
-  PrefixDesc pd{};
-  TileAggDesc td{};
+  ScanLaunch launch;
   fgpu_stats stats{};             // everything about the scan that does not change between Executes
   std::vector<KeyOut> keys;       // with the dictionary snapshots
-  std::vector<uint32_t> dense_radix;
   std::vector<std::string> agg_names;
   std::vector<uint8_t> agg_is_float;
   std::shared_ptr<PinnedPool> pool;
@@ -840,7 +877,7 @@ struct Compiled {
   uint64_t h2d_bytes = 0;  // column uploads this query triggered
   uint32_t pruned_row_groups = 0;
   uint64_t touched_rows = ~uint64_t(0);  // rows of the row groups that survive pruning (~0: nothing was pruned)
-  bool runs_shape = false;  // dense keys, conjunction of numeric leaves, plain aggregate inputs (any number of them)
+  uint32_t radix(int k) const { return dense_radix[size_t(k)] ? dense_radix[size_t(k)] : 1; }  // (int64 keys have none)
 };
 
 int32_t compile_filter(const QueryPlan& q, int node, Compiled* c, std::map<std::string, int>& slot_of) {
@@ -1028,7 +1065,7 @@ bool rg_may_match(const QueryPlan& q, int node, const RowGroupHost& rg) {
 
 // Resolves the plan against the visible row groups and fills everything of QueryDesc that does
 // not need device memory.
-int32_t compile(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, Compiled* c) {
+int32_t compile(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, const Switches& w, Compiled* c) {
   Table& table = ctx->tables[q.table];  // a table without parts scans nothing (empty LSM)
   for (auto& p : table.parts) {
     if (p->tx > tx) continue;  // index/lsm.go:416
@@ -1210,7 +1247,7 @@ int32_t compile(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, Compiled* c) {
   // Conjunction: comparisons on the same numeric column intersect into one range leaf
   // (timestamp >= a AND timestamp < b  ->  timestamp in [a, b-1]); a missing column keeps the
   // strictest of the merged leaves' missing-column behaviours.
-  if (qd.filter_kind == FK_AND && !getenv("FROSTGPU_NO_FUSE")) {
+  if (qd.filter_kind == FK_AND && !w.no_fuse) {
     std::vector<LeafHost> fused;
     for (LeafHost& lh : c->leaves) {
       bool merged = false;
@@ -1275,7 +1312,7 @@ int32_t compile(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, Compiled* c) {
       }
     }
     std::vector<VisibleRG> kept;
-    const bool prune_on = !getenv("FROSTGPU_NO_PRUNE");
+    const bool prune_on = !w.no_prune;
     // AggFuncPushDown (logicalplan/optimize.go:166-193) + MaxAgg (expr/filter.go:156-207): a global Max(column)
     // directly above the scan, without filter, turns into a row-group filter that memoises the largest chunk
     // maximum seen so far, in scan order, and only lets row groups through that exceed it.
@@ -1576,12 +1613,7 @@ int32_t compile(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, Compiled* c) {
   }
   // ---- scan kernel: vector length, ring depth and the per-warp shared-memory layout ----------------
   {
-    auto envi = [](const char* n, int d) { const char* e = getenv(n); return e ? atoi(e) : d; };
-    int vl = envi("FROSTGPU_VL", 256);
-    if (vl != 128 && vl != 256 && vl != 512 && vl != 1024) vl = 512;
-    int ring = envi("FROSTGPU_RING", 3);
-    if (ring < 2) ring = 2;
-    if (ring > 4) ring = 4;
+    int vl = w.vl, ring = w.ring;
     bool any_expr = false;
     for (int k = 0; k < qd.n_keys; k++)
       if (qd.keys[k].prog_len) any_expr = true;
@@ -1613,7 +1645,7 @@ int32_t compile(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, Compiled* c) {
     qd.n_ring = ring;
     // fused fast path: conjunction of numeric leaves, dense dictionary keys, simple aggregates
     bool fast = qd.table_mode == TM_DENSE && (qd.n_filter_prog == 0 || qd.filter_kind == FK_AND) && qd.n_leaves <= 2 && qd.n_keys <= 3 &&
-                !getenv("FROSTGPU_NO_FAST");
+                !w.no_fast;
     for (int l = 0; l < qd.n_leaves && fast; l++) {
       const LeafHost& lh = c->leaves[size_t(l)];
       if (lh.slot >= 0 && c->slot_types[size_t(lh.slot)] == ST_DICT) fast = false;
@@ -1624,15 +1656,6 @@ int32_t compile(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, Compiled* c) {
       if (qd.aggs[a].func == FGPU_AGG_COUNT) continue;
       stored++;
       if (!(qd.aggs[a].prog_len == 1 && qd.prog[qd.aggs[a].prog_off].op == PO_LOAD)) fast = false;
-    }
-    {  // the sorted-run kernel: up to kRunsAggs reducers, and dictionary leaves evaluated once per run
-      bool rs = qd.table_mode == TM_DENSE && (qd.n_filter_prog == 0 || qd.filter_kind == FK_AND) && qd.n_keys <= kRunsKeys &&
-                qd.n_leaves <= kRunsLeaves + kRunsPreds && !getenv("FROSTGPU_NO_FAST");
-      for (int l = 0; l < qd.n_leaves && rs; l++)
-        if (c->leaves[size_t(l)].slot >= 0 && c->leaves[size_t(l)].numeric && c->leaves[size_t(l)].null_literal) rs = false;
-      for (int a = 0; a < qd.n_aggs && rs; a++)
-        if (qd.aggs[a].func != FGPU_AGG_COUNT && !(qd.aggs[a].prog_len == 1 && qd.prog[qd.aggs[a].prog_off].op == PO_LOAD)) rs = false;
-      c->runs_shape = rs;
     }
     if (stored > 2) fast = false;
     qd.fast_ok = fast ? 1 : 0;
@@ -1669,13 +1692,21 @@ void bind_table(QueryDesc* qd, uint8_t* base) {
   qd->t_keys = qd->table_mode == TM_HASH ? reinterpret_cast<unsigned long long*>(base + off_keys) : nullptr;
 }
 
-// Runs init + scan.  On success the result owns the device table.
-// The development / test switches that change how a plan is compiled or launched: a cached plan is only reused
-// under the switches it was built with.
-inline bool env_has(const std::string& env, const char* name) { return env.find(name) != std::string::npos; }
+void bind_finalize(FinalizeDesc* fd, const QueryDesc& qd) {  // the table bind_table placed
+  fd->t_rows = qd.t_rows;
+  for (int a = 0; a < kMaxAggs; a++) fd->t_agg[a] = qd.t_agg[a];
+  fd->t_tag = qd.t_tag;
+  fd->t_keys = qd.t_keys;
+}
 
 int32_t finalize_dense_host(fgpu_ctx* ctx, fgpu_result* res, ExecCache& x);
-void bind_table(QueryDesc* qd, uint8_t* base);
+
+// FROSTGPU_COMM_TIMEOUT_MS: how long a collective Execute waits for its peers (default 10 s).  It changes no plan, so
+// it is not one of the Switches.
+uint64_t comm_timeout_ns() {
+  const char* to = getenv("FROSTGPU_COMM_TIMEOUT_MS");
+  return uint64_t(to ? std::max(1, atoi(to)) : 10000) * 1000000ull;
+}
 
 // First half of the exchange, enqueued behind the scan: this rank's partial table goes into slot [rank] of every
 // rank's mailbox, then the flags are raised (comm.cu).
@@ -1710,8 +1741,7 @@ int32_t comm_wait_merge(fgpu_ctx* ctx, const QueryDesc& qd, void* table, uint64_
   w.flags = reinterpret_cast<const unsigned long long*>(cm.mailbox + cm.flag_off(set, 0));
   w.seq = seq;
   w.bytes = bytes;
-  const char* to = getenv("FROSTGPU_COMM_TIMEOUT_MS");
-  w.timeout_ns = uint64_t(to ? std::max(1, atoi(to)) : 10000) * 1000000ull;
+  w.timeout_ns = comm_timeout_ns();
   w.counters = qd.counters;
   w.n = cm.n;
   CUDA_TRY(launch_comm_wait(w, ctx->stream));
@@ -1732,7 +1762,16 @@ int32_t comm_check(unsigned long long code) {
   return FGPU_OK;
 }
 
-// Re-issues the launches of a cached plan (see ExecCache): table init, scans, one copy back, one synchronisation.
+// k_finalize with max_out == 0 only counts the groups of the table, into *out.
+cudaError_t launch_count_groups(FinalizeDesc fd, unsigned int* out, cudaStream_t s) {
+  fd.out_count = out;
+  fd.max_out = 0;
+  fd.out_keys = nullptr;
+  fd.out_aggs = nullptr;
+  fd.out_rows = nullptr;
+  return launch_finalize(fd, s);
+}
+
 // Tail of a cached Execute: compact the (final) dense table into result columns on the device and bring them back.
 // The result image is written by the kernel straight into a page-locked block of the context's pool (host memory the
 // device addresses directly): no copy operation, and the block later travels to the Arrow consumer as it is.
@@ -1749,10 +1788,10 @@ int32_t cached_tail(fgpu_ctx* ctx, ExecCache& x) {
   return FGPU_OK;
 }
 
-// Collective tail of a cached Execute: ONE launch waits for the peers' flags, folds the n partial tables of this rank's
-// mailbox and compacts the result into the page-locked block (synchronize.go:16-53 + the final aggregate of
-// physicalplan.go:438-471).
-int32_t cached_tail_merged(fgpu_ctx* ctx, ExecCache& x, uint64_t seq, uint64_t bytes) {
+// Collective tail of a cached Execute (cached plans have dense tables): ONE launch waits for the peers' flags, folds
+// the n partial tables of this rank's mailbox and compacts the result into the page-locked block (synchronize.go:16-53
+// + the final aggregate of physicalplan.go:438-471).
+int32_t cached_merge_tail(fgpu_ctx* ctx, ExecCache& x, uint64_t seq, uint64_t bytes) {
   Comm& cm = ctx->comm;
   const uint64_t set = seq & 1u;
   DenseOut& f = x.dout;
@@ -1761,14 +1800,27 @@ int32_t cached_tail_merged(fgpu_ctx* ctx, ExecCache& x, uint64_t seq, uint64_t b
   f.flags = reinterpret_cast<const unsigned long long*>(cm.mailbox + cm.flag_off(set, 0));
   f.seq = seq;
   f.bytes = bytes;
-  const char* to = getenv("FROSTGPU_COMM_TIMEOUT_MS");
-  f.timeout_ns = uint64_t(to ? std::max(1, atoi(to)) : 10000) * 1000000ull;
+  f.timeout_ns = comm_timeout_ns();
   f.err = x.qd.counters + 3;
   const int32_t rc = cached_tail(ctx, x);
   f.n_src = 0;
   return rc;
 }
 
+// k_table_init, the aggregate-scan launches, k_scan; ev[1] and ev[2] bracket the scan kernels.
+int32_t launch_aggregate_scan(fgpu_ctx* ctx, const QueryDesc& qd, const QueryDesc* qdesc_dev, const ScanLaunch& L) {
+  cudaStream_t s = ctx->stream;
+  CUDA_TRY(launch_table_init(qd, s));
+  CUDA_TRY(cudaEventRecord(ctx->ev[1], s));
+  if (L.runs) CUDA_TRY(launch_runs_tma(L.rd, L.runs_nl, L.runs_nk, L.runs_na, ctx->sm_count, s));
+  if (L.prefix) CUDA_TRY(launch_runs_prefix(L.pd, ctx->sm_count, s));
+  if (L.tile) CUDA_TRY(launch_tile_agg(L.td, ctx->sm_count, s));
+  CUDA_TRY(launch_scan(qdesc_dev, qd, ctx->sm_count, s));
+  CUDA_TRY(cudaEventRecord(ctx->ev[2], s));
+  return FGPU_OK;
+}
+
+// Re-issues the launches of a cached plan (see ExecCache): table init, scans, one copy back, one synchronisation.
 // collective: 0 no exchange, 1 push + wait + merge in one go, 2 push only (fgpu_query_execute_collective_begin)
 int32_t run_cached(fgpu_ctx* ctx, ExecCache& x, fgpu_result* res, int collective) {
   PhaseClock pc;
@@ -1777,19 +1829,10 @@ int32_t run_cached(fgpu_ctx* ctx, ExecCache& x, fgpu_result* res, int collective
   res->stats = x.stats;
   fgpu_stats& st = res->stats;
   CUDA_TRY(cudaEventRecord(ctx->ev[0], s));
-  CUDA_TRY(launch_table_init(x.qd, s));
-  CUDA_TRY(cudaEventRecord(ctx->ev[1], s));
-  if (x.has_runs) {
-    CUDA_TRY(launch_runs_tma(x.rd, x.runs_nl, x.runs_nk, x.runs_na, ctx->sm_count, s));
-  }
-  if (x.has_prefix) CUDA_TRY(launch_runs_prefix(x.pd, ctx->sm_count, s));
-  if (x.has_ta) CUDA_TRY(launch_tile_agg(x.td, ctx->sm_count, s));
-  CUDA_TRY(launch_scan(x.qdesc_dev, x.qd, ctx->sm_count, s));
-  CUDA_TRY(cudaEventRecord(ctx->ev[2], s));
+  if (int32_t rc = launch_aggregate_scan(ctx, x.qd, x.qdesc_dev, x.launch)) return rc;
   if (collective) {
     uint64_t seq = 0, bytes = 0;
-    int32_t rc = comm_push(ctx, x.table.p, x.table_bytes, &seq, &bytes);
-    if (rc) return rc;
+    if (int32_t rc = comm_push(ctx, x.table.p, x.table_bytes, &seq, &bytes)) return rc;
     st.kernel_launches++;  // k_comm_push
     if (collective == 2) {  // the merge half follows in fgpu_query_execute_collective_end
       res->pending = true;
@@ -1798,13 +1841,7 @@ int32_t run_cached(fgpu_ctx* ctx, ExecCache& x, fgpu_result* res, int collective
       res->pending_bytes = bytes;
       return FGPU_OK;
     }
-    if (x.qd.table_mode == TM_DENSE) {
-      if (int32_t rcm = cached_tail_merged(ctx, x, seq, bytes)) return rcm;
-    } else {
-      rc = comm_wait_merge(ctx, x.qd, x.table.p, seq, bytes);
-      if (rc) return rc;
-      if (int32_t rct = cached_tail(ctx, x)) return rct;
-    }
+    if (int32_t rc = cached_merge_tail(ctx, x, seq, bytes)) return rc;
   } else if (int32_t rc = cached_tail(ctx, x)) {
     return rc;
   }
@@ -1826,6 +1863,797 @@ int32_t run_cached(fgpu_ctx* ctx, ExecCache& x, fgpu_result* res, int collective
   return rc;
 }
 
+// ---- Execute planning -----------------------------------------------------------------------------------------------
+// Every row group gets a row of the general tables that k_scan / k_rows read.  The specialised kernels may then take it,
+// in run_scan's order; each has a planner of three steps: a query-level check that fills its plan (or says no), an
+// admit step over the row group's rows of the general tables, and a layout step once every row group is placed.
+
+struct GeneralTables {
+  std::vector<ChunkDesc> chunks;  // [row group][slot]
+  std::vector<LeafRt> lrt;        // [row group][leaf]
+  std::vector<uint32_t> first_tile, rg_rows;
+  std::vector<uint8_t> lutbytes;                   // dictionary leaves: one result byte per global dictionary id
+  std::vector<std::pair<size_t, size_t>> lut_fix;  // (index into lrt, offset into lutbytes)
+  uint32_t tiles = 0;
+  int n = 0;  // row groups that stay with the general kernel
+  GeneralTables(int n_rg, int n_slots, int n_leaves)
+      : chunks(size_t(n_rg) * std::max(n_slots, 1)), lrt(size_t(n_rg) * std::max(n_leaves, 1)), first_tile(size_t(n_rg) + 1), rg_rows(std::max(n_rg, 1)) {}
+};
+
+// Fills row G.n of the general tables from row group g0 of the plan.
+int32_t describe_row_group(fgpu_ctx* ctx, const QueryPlan& q, Compiled& c, int g0, GeneralTables& G, fgpu_stats& st) {
+  const int n_slots = c.qd.n_slots, n_leaves = c.qd.n_leaves;
+  const VisibleRG& v = c.rgs[size_t(g0)];
+  const size_t g = size_t(G.n);
+  for (int s = 0; s < n_slots; s++) {
+    ChunkDesc d{};
+    d.kind = CK_ABSENT;
+    d.n_rows = v.rg->n_rows;
+    auto it = ((v.skip_slots >> s) & 1) ? v.rg->cols.end() : v.rg->cols.find(c.slot_names[size_t(s)]);
+    if (it != v.rg->cols.end()) {
+      ChunkHost& ch = it->second;
+      if (!ch.error.empty())
+        return fail(FGPU_ERR_UNSUPPORTED, "column " + c.slot_names[size_t(s)] + ": " + ch.error);
+      d = ch.desc;
+      st.algorithmic_bytes += ch.stored_bytes;
+      st.metadata_bytes += ch.meta_bytes;
+    }
+    G.chunks[g * n_slots + s] = d;
+  }
+  for (int l = 0; l < n_leaves; l++) {
+    LeafHost& lh = c.leaves[size_t(l)];
+    LeafRt rt{};
+    auto it = lh.slot < 0 ? v.rg->cols.end() : v.rg->cols.find(lh.column);
+    if (it == v.rg->cols.end()) {
+      rt.mode = lh.missing_mode;
+    } else if (c.slot_types[size_t(lh.slot)] == ST_DICT) {
+      rt.mode = LM_EVAL;
+      rt.null_result = (lh.op == FGPU_OP_EQ && lh.lit->lit_type == FGPU_SCALAR_NULL) ? 1 : 0;
+      if (lh.lut_off == size_t(-1)) {
+        // one result byte per GLOBAL dictionary id, evaluated once per distinct dictionary entry
+        const GlobalDict& gd = ctx->tables[q.table].dicts[lh.column];
+        lh.lut_off = G.lutbytes.size();
+        G.lutbytes.resize(lh.lut_off + gd.values.size() + 1);
+        for (size_t i = 0; i < gd.values.size(); i++) G.lutbytes[lh.lut_off + i] = dict_leaf_value(lh, gd.values[i]) ? 1 : 0;
+      }
+      G.lut_fix.emplace_back(g * n_leaves + l, lh.lut_off);
+    } else {
+      rt.mode = lh.null_literal ? LM_NONE : LM_EVAL;
+    }
+    if (v.leaf_mode[l] != LM_EVAL) rt.mode = v.leaf_mode[l];
+    G.lrt[g * n_leaves + l] = rt;
+  }
+  return FGPU_OK;
+}
+
+// The per-row-group descriptors of the specialised kernels refer to the LUT block before it has a device address: they
+// hold its byte offset + 1 (null: no LUT) until lut_rebase turns that into a pointer.
+const uint8_t* lut_ref(size_t off) { return reinterpret_cast<const uint8_t*>(uintptr_t(off) + 1); }
+void lut_rebase(const uint8_t*& p, const uint8_t* lut) {
+  if (p) p = lut + (size_t(uintptr_t(p)) - 1);
+}
+
+// Index of `slot` in slots[0, *n), appended when missing (-1: the list is full at cap).
+int find_or_add(int* slots, uint32_t* n, int cap, int slot) {
+  for (uint32_t i = 0; i < *n; i++)
+    if (slots[i] == slot) return int(i);
+  if (*n >= uint32_t(cap)) return -1;
+  slots[*n] = slot;
+  return int((*n)++);
+}
+
+// A dictionary column whose runs are long enough that a 32-row step rarely holds two run ends (row_runs: the
+// directory in row space; it exists when the column chunk is run-length only, NULLs included).  Short runs — a leaf
+// on a column far down the sort order — are the tile-aggregate kernel's business: its per-row result byte costs one
+// shared load where a cursor would move every few rows.
+bool long_runs(const ChunkDesc& d, uint32_t n_rows) {
+  return d.kind == CK_DICT_STR && d.row_runs != nullptr && uint64_t(d.n_row_runs) * 32 <= uint64_t(n_rows) + 1024;
+}
+
+// ---- sorted-run scan (runs_tma.cu) ----
+// One launch over the qualifying row groups; a row group whose statistics already decided every leaf is flagged
+// all_pass (its leaf columns are neither uploaded nor staged).
+struct RunsRgCols {  // the chunks behind RunsRg::col (null: not staged)
+  Part* part = nullptr;
+  ChunkHost* ch[kRunsCols] = {nullptr};
+};
+struct RunsCand {  // a row group the sorted-run kernel admitted
+  RunsRg rr{};
+  RunsRgCols cols{};
+};
+struct RunsPlan {
+  RunsDesc rd{};
+  int nl = 0, nk = 0, na = 0, np = 0;
+  int leaf_index[kRunsLeaves] = {0}, pred_leaf[kRunsPreds] = {0};  // query leaf behind every range / dictionary leaf
+  int agg_slot[kRunsAggs] = {0}, agg_index[kRunsAggs] = {0};
+  int col_slot[kRunsCols] = {0};  // slot of every distinct staged column
+  std::vector<RunsRg> rgs;
+  std::vector<RunsRgCols> cols;
+  std::vector<uint32_t> first_span;
+};
+
+// Dense keys (up to kRunsKeys), a conjunction of int64 range leaves and of dictionary leaves (evaluated once per run),
+// up to kRunsAggs Sum / Min / Max of plain columns.
+bool runs_query(const Compiled& c, const QueryDesc& qd, const Switches& w, RunsPlan* P) {
+  if (w.no_fast || w.no_runs || qd.table_mode != TM_DENSE || (qd.n_filter_prog != 0 && qd.filter_kind != FK_AND) || qd.n_keys > kRunsKeys ||
+      qd.n_leaves > kRunsLeaves + kRunsPreds)
+    return false;
+  RunsDesc& rd = P->rd;
+  auto col_of = [&](int slot) { return uint32_t(find_or_add(P->col_slot, &rd.n_cols, kRunsCols, slot)); };
+  for (int l = 0; l < qd.n_leaves; l++) {
+    const LeafHost& lh = c.leaves[size_t(l)];
+    const LeafDesc& ld = qd.leaves[l];
+    if (lh.slot >= 0 && lh.numeric && lh.null_literal) return false;
+    if (ld.slot == 0xff || qd.slot_type[ld.slot] == ST_DICT) {  // dictionary leaf, or a column absent from every row group
+      if (P->np >= kRunsPreds) return false;
+      P->pred_leaf[P->np++] = l;
+    } else if (ld.cmp_float || ld.neg || qd.slot_type[ld.slot] != ST_I64 || P->nl >= kRunsLeaves) {
+      return false;
+    } else {
+      P->leaf_index[P->nl] = l;
+      rd.leaf_col[P->nl++] = col_of(ld.slot);
+    }
+  }
+  for (int a = 0; a < qd.n_aggs; a++) {
+    const AggDesc& ad = qd.aggs[a];
+    if (ad.func == FGPU_AGG_COUNT) continue;
+    if (!(ad.prog_len == 1 && qd.prog[ad.prog_off].op == PO_LOAD)) return false;
+    if ((ad.func != FGPU_AGG_SUM && ad.func != FGPU_AGG_MIN && ad.func != FGPU_AGG_MAX) || P->na >= kRunsAggs) return false;
+    P->agg_slot[P->na] = qd.prog[ad.prog_off].slot;
+    rd.agg_col[P->na] = col_of(P->agg_slot[P->na]);
+    rd.agg_func[P->na] = uint32_t(ad.func) | (ad.is_float ? 0x100u : 0u);
+    P->agg_index[P->na++] = a;
+  }
+  P->nk = qd.n_keys;
+  for (int k = 0; k < P->nk; k++) rd.stride[k] = qd.keys[k].dense_stride;
+  rd.n_pred = uint32_t(P->np);
+  return true;
+}
+
+bool runs_admit(RunsPlan& P, const Compiled& c, const QueryDesc& qd, const VisibleRG& v, const ChunkDesc* chunks, const LeafRt* lrt, RunsCand* out) {
+  const uint32_t n_rows = v.rg->n_rows;
+  if (n_rows == 0) return false;
+  bool all_pass = P.nl > 0;
+  for (int l = 0; l < P.nl; l++) {
+    const uint8_t m = lrt[P.leaf_index[l]].mode;
+    if (m != LM_ALL) all_pass = false;
+    if (m == LM_NONE) return false;  // (only with pruning switched off)
+  }
+  RunsRg& rr = out->rr;
+  rr.n_rows = n_rows;
+  for (int l = 0; l < P.nl; l++) {
+    const int ql = P.leaf_index[l];
+    const bool all = lrt[ql].mode == LM_ALL;
+    rr.lo[l] = all ? std::numeric_limits<int64_t>::min() : qd.leaves[ql].lo_i;
+    rr.hi[l] = all ? std::numeric_limits<int64_t>::max() : qd.leaves[ql].hi_i;
+  }
+  for (int i = 0; i < P.np; i++) {  // dictionary leaves: one result per run
+    const int ql = P.pred_leaf[i];
+    const LeafRt& rt = lrt[ql];
+    rr.pred_runs[i] = nullptr;
+    if (rt.mode == LM_ALL) continue;         // decided: passes everywhere in this row group
+    if (rt.mode == LM_NONE) return false;    // (only with pruning switched off)
+    const ChunkDesc& d = chunks[qd.leaves[ql].slot];
+    if (!long_runs(d, n_rows)) return false;
+    rr.pred_runs[i] = d.row_runs;
+    rr.pred_seeds[i] = d.row_seeds;
+    rr.pred_n_runs[i] = d.n_row_runs;
+    rr.pred_lut[i] = lut_ref(c.leaves[size_t(ql)].lut_off);
+    P.rd.pred_null[i] = rt.null_result;
+  }
+  rr.all_pass = all_pass ? 1 : 0;
+  bool any_col = false;
+  out->cols.part = v.part;
+  for (uint32_t i = 0; i < P.rd.n_cols; i++) {
+    const ChunkDesc& d = chunks[P.col_slot[i]];
+    rr.col[i] = nullptr;
+    if ((v.skip_slots >> P.col_slot[i]) & 1) continue;  // a decided leaf's own column
+    if (d.kind != CK_PLAIN64 || d.has_nulls) return false;
+    rr.col[i] = d.values;
+    out->cols.ch[i] = &v.rg->cols.at(c.slot_names[size_t(P.col_slot[i])]);
+    any_col = true;
+  }
+  // all_pass: the leaf columns stay null (not staged).  Otherwise a decided leaf still runs its (widened) range test:
+  // a staged column stands in for the one that was not uploaded (see the tile plan).
+  if (!all_pass && !any_col && P.rd.n_cols > 0) return false;
+  if (all_pass)  // aggregate inputs must be there
+    for (int a = 0; a < P.na; a++)
+      if (!rr.col[P.rd.agg_col[a]]) return false;
+  for (int k = 0; k < P.nk; k++) {  // keys: run-length only, long runs
+    const ChunkDesc& d = chunks[qd.keys[k].slot];
+    if (!long_runs(d, n_rows)) return false;
+    rr.runs[k] = d.row_runs;
+    rr.seeds[k] = d.row_seeds;
+    rr.n_runs[k] = d.n_row_runs;
+  }
+  return true;
+}
+
+// ---- prefix sums (runs_prefix.cu) ----
+// Row groups of the sorted-run shape whose filter the statistics decided, without undecided dictionary leaves and with
+// Sum(int64) as the only stored aggregates, are answered from prefix sums instead when their runs average at least
+// kPrefixRunRows rows: then a step per group run is cheaper than reading its rows.
+constexpr uint64_t kPrefixRunRows = 64;
+struct PrefixPlan {
+  PrefixDesc pd{};
+  std::vector<PrefixRg> rgs;
+  std::vector<std::array<ChunkHost*, kRunsAggs>> sums;  // per row group: the chunk of every Sum input
+  std::vector<Part*> parts;
+  std::vector<PrefixWin> wins;
+};
+
+bool prefix_query(const RunsPlan& R, const Switches& w) {
+  if (w.no_prefix) return false;
+  for (int a = 0; a < R.na; a++)
+    if (R.rd.agg_func[a] != uint32_t(FGPU_AGG_SUM)) return false;  // Min / Max / float64 Sum stay with k_runs_tma
+  return true;
+}
+
+// A row group the sorted-run kernel admitted.
+bool prefix_admit(PrefixPlan& P, const RunsPlan& R, const RunsCand& rc, fgpu_stats& st) {
+  const RunsRg& rr = rc.rr;
+  if (R.nl > 0 && !rr.all_pass) return false;  // (the kernel treats a launch without range leaves as all-pass)
+  for (int i = 0; i < R.np; i++)
+    if (rr.pred_runs[i]) return false;  // an undecided dictionary leaf
+  uint64_t sum_runs = 0;
+  for (int k = 0; k < R.nk; k++) sum_runs += rr.n_runs[k];
+  std::array<ChunkHost*, kRunsAggs> sums{};
+  for (int a = 0; a < R.na; a++) {
+    sums[size_t(a)] = rc.cols.ch[R.rd.agg_col[a]];
+    if (!sums[size_t(a)] || sums[size_t(a)]->phys != PT_INT64) return false;
+  }
+  if (uint64_t(rr.n_rows) < kPrefixRunRows * sum_runs) return false;
+  PrefixRg pr{};
+  pr.n_rows = rr.n_rows;
+  for (int k = 0; k < R.nk; k++) {
+    pr.runs[k] = rr.runs[k];
+    pr.seeds[k] = rr.seeds[k];
+    pr.n_runs[k] = rr.n_runs[k];
+    st.algorithmic_bytes += uint64_t(rr.n_runs[k]) * sizeof(Run);  // the directories, read whole
+  }
+  const uint32_t win = runs_prefix_window_rows(rr.n_rows, uint32_t(sum_runs));
+  uint32_t n_win = 0;
+  for (uint32_t r0 = 0; r0 < rr.n_rows; r0 += win, n_win++)
+    P.wins.push_back(PrefixWin{uint32_t(P.rgs.size()), r0, std::min(win, rr.n_rows - r0), 0u});
+  // a Sum input is read at the segment boundaries (at most every run start, every window start and the end), not
+  // row by row
+  for (int a = 0; a < R.na; a++) {
+    bool first = true;
+    for (int a2 = 0; a2 < a; a2++) first = first && sums[size_t(a2)] != sums[size_t(a)];
+    if (first) st.algorithmic_bytes = st.algorithmic_bytes - sums[size_t(a)]->stored_bytes + (sum_runs + n_win + 1) * 8;
+  }
+  P.rgs.push_back(pr);
+  P.sums.push_back(sums);
+  P.parts.push_back(rc.cols.part);
+  return true;
+}
+
+// Layout of both run kernels: the frame-of-reference and prefix-sum images (one batch over every staged int64 column
+// and every Sum input of the prefix path of every part), then the tile rows and stage layout of k_runs_tma.
+int32_t runs_layout(fgpu_ctx* ctx, const Compiled& c, const Switches& w, RunsPlan& R, PrefixPlan& P, fgpu_stats& st) {
+  {
+    std::set<std::pair<Part*, std::string>> seen, pseen;
+    std::vector<std::pair<Part*, std::string>> want, want_prefix;
+    for (const RunsRgCols& rc : R.cols)
+      for (uint32_t i = 0; i < R.rd.n_cols; i++)
+        if (rc.ch[i] && rc.ch[i]->phys == PT_INT64 && seen.emplace(rc.part, c.slot_names[size_t(R.col_slot[i])]).second)
+          want.emplace_back(rc.part, c.slot_names[size_t(R.col_slot[i])]);
+    for (size_t k = 0; k < P.rgs.size(); k++)
+      for (int a = 0; a < R.na; a++)
+        if (pseen.emplace(P.parts[k], c.slot_names[size_t(R.agg_slot[a])]).second) want_prefix.emplace_back(P.parts[k], c.slot_names[size_t(R.agg_slot[a])]);
+    if (!want.empty() || !want_prefix.empty())
+      if (int32_t rc = ensure_narrow(ctx, want, want_prefix)) return rc;
+    for (size_t k = 0; k < P.rgs.size(); k++)
+      for (int a = 0; a < R.na; a++) {
+        P.rgs[k].pre[a] = P.sums[k][size_t(a)]->prefix;
+        if (!P.rgs[k].pre[a]) return fail(FGPU_ERR_INVALID, "prefix-sum image missing for column " + c.slot_names[size_t(R.agg_slot[a])]);
+      }
+  }
+  if (!P.rgs.empty()) {
+    PrefixDesc& pd = P.pd;
+    pd.n_win = uint32_t(P.wins.size());
+    pd.nk = uint32_t(R.nk);
+    pd.na = uint32_t(R.na);
+    for (int k = 0; k < R.nk; k++) pd.stride[k] = R.rd.stride[k];
+  }
+  if (R.rgs.empty()) return FGPU_OK;
+  RunsDesc& rd = R.rd;
+  rd.n_rg = uint32_t(R.rgs.size());
+  // every row group is cut into tiles of about tile_bytes of staged column data; the launch's tile table {row group,
+  // first row} is dealt to the CTAs in chunks of consecutive entries
+  const uint32_t tile_bytes = uint32_t(w.rt_tile) * 8u;  // (rows of 8 bytes)
+  uint32_t tiles_rt = 0, gidx = 0, col_region = 0, max_tile = 1024;
+  uint64_t total = 0;
+  for (const RunsRg& r : R.rgs) total += r.n_rows;
+  // small launches: at least one tile per resident CTA (three per SM), or the grid is not filled
+  const uint32_t fill_rows = uint32_t(std::min<uint64_t>(1u << 20, std::max<uint64_t>(1024, (total / (uint64_t(ctx->sm_count) * 3)) & ~uint64_t(1023))));
+  for (size_t k = 0; k < R.rgs.size(); k++) {
+    RunsRg& r = R.rgs[k];
+    uint32_t row_bytes = 0, max_runs = 0;
+    for (uint32_t i = 0; i < rd.n_cols; i++) {
+      const ChunkHost* ch = R.cols[k].ch[i];
+      r.cl[i] = RunsCol{0, 3, 0};
+      if (ch && ch->narrow) {
+        r.col[i] = ch->narrow;
+        r.cl[i].lg = ch->narrow_w == 1 ? 0 : (ch->narrow_w == 2 ? 1 : 2);
+        r.cl[i].base = ch->narrow_base;
+        st.algorithmic_bytes = st.algorithmic_bytes - ch->stored_bytes + uint64_t(r.n_rows) * ch->narrow_w;
+      }
+      if (r.col[i]) row_bytes += 1u << r.cl[i].lg;
+    }
+    for (int i = 0; i < R.nk; i++) max_runs = std::max(max_runs, r.n_runs[i]);
+    for (int i = 0; i < R.np; i++)
+      if (r.pred_runs[i]) max_runs = std::max(max_runs, r.pred_n_runs[i]);
+    r.tile_rows = std::min(runs_tma_tile_rows(tile_bytes, row_bytes, r.n_rows, max_runs), fill_rows);
+    int first = -1;
+    uint32_t off = 0;
+    for (uint32_t i = 0; i < rd.n_cols; i++) {
+      if (!r.col[i]) continue;
+      if (first < 0) first = int(i);
+      r.cl[i].soff = off;
+      off += ((r.tile_rows << r.cl[i].lg) + 127u) & ~127u;
+    }
+    for (uint32_t i = 0; i < rd.n_cols && first >= 0; i++)  // a column that is not staged reads a staged one
+      if (!r.col[i]) r.cl[i] = r.cl[first];
+    col_region = std::max(col_region, off);
+    max_tile = std::max(max_tile, r.tile_rows);
+    for (uint32_t r0 = 0; r0 < r.n_rows; r0 += r.tile_rows) {
+      R.first_span.push_back(gidx);
+      R.first_span.push_back(r0);
+      tiles_rt++;
+    }
+    gidx++;
+  }
+  runs_tma_plan(rd, R.nk + R.np, max_tile, col_region, w.rt_stages, w.rt_warps, w.rt_span);
+  rd.n_spans = tiles_rt;
+  return FGPU_OK;
+}
+
+// ---- tile aggregate (tile_agg.cu) ----
+// Row groups the sorted-run kernel does not take (bit-packed / short-run / nullable keys, L0 records) go to the
+// tile-aggregate kernel when the plan is a conjunction of range + dictionary leaves over a dense table with plain
+// aggregate inputs.
+struct TilePlan {
+  TileAggDesc td{};
+  std::vector<TileAggRg> rgs;
+  std::vector<uint32_t> first_tile;
+  int plain_slot[kTaPlain] = {0}, code_slot[kTaCodes] = {0};
+  uint32_t code_wmax[kTaCodes] = {0};
+  int leaf_q[kTaLeaves] = {0}, pred_q[kTaPreds] = {0}, agg_index[kTaAggs] = {0};
+  bool agg_bounded = true;  // every int64 Sum input of every row group has statistics inside [0, 2^32)
+  uint64_t agg_max = 0;     // the largest of those chunk maxima
+};
+
+bool tile_query(const Compiled& c, const QueryDesc& qd, const Switches& w, TilePlan* T) {
+  if (w.no_tile || qd.table_mode != TM_DENSE || (qd.n_filter_prog != 0 && qd.filter_kind != FK_AND) || qd.n_keys > kTaKeys) return false;
+  TileAggDesc& td = T->td;
+  auto plain_of = [&](int slot) { return find_or_add(T->plain_slot, &td.n_plain, kTaPlain, slot); };
+  auto code_of = [&](int slot) { return find_or_add(T->code_slot, &td.n_codes, kTaCodes, slot); };
+  for (int l = 0; l < qd.n_leaves; l++) {
+    const LeafDesc& ld = qd.leaves[l];
+    if (ld.slot == 0xff) continue;  // column absent from every row group: ALL / NONE per row group, nothing to evaluate
+    if (qd.slot_type[ld.slot] == ST_DICT) {
+      const int cc = code_of(ld.slot);
+      if (td.np >= uint32_t(kTaPreds) || cc < 0) return false;
+      T->pred_q[td.np] = l;
+      td.pred_code[td.np++] = uint32_t(cc);
+    } else {
+      const int pp = plain_of(ld.slot);
+      if (c.leaves[size_t(l)].null_literal || td.nl >= uint32_t(kTaLeaves) || pp < 0) return false;
+      T->leaf_q[td.nl] = l;
+      td.leaf_plain[td.nl] = uint32_t(pp);
+      td.leaf_flags[td.nl++] = (ld.cmp_float ? 1u : 0u) | (qd.slot_type[ld.slot] == ST_F64 ? 2u : 0u) | (ld.neg ? 4u : 0u);
+    }
+  }
+  for (int k = 0; k < qd.n_keys; k++) {
+    const int cc = code_of(qd.keys[k].slot);
+    if (qd.keys[k].is_int64 || cc < 0) return false;
+    td.key_code[td.nk] = uint32_t(cc);
+    td.key_stride[td.nk++] = qd.keys[k].dense_stride;
+  }
+  for (int a = 0; a < qd.n_aggs; a++) {
+    const AggDesc& ad = qd.aggs[a];
+    if (ad.func == FGPU_AGG_COUNT) continue;
+    const bool simple = ad.prog_len == 1 && qd.prog[ad.prog_off].op == PO_LOAD;
+    const int pp = simple ? plain_of(qd.prog[ad.prog_off].slot) : -1;
+    if ((ad.func != FGPU_AGG_SUM && ad.func != FGPU_AGG_MIN && ad.func != FGPU_AGG_MAX) || td.na >= uint32_t(kTaAggs) || pp < 0) return false;
+    T->agg_index[td.na] = a;
+    td.agg_plain[td.na] = uint32_t(pp);
+    td.cell64[td.na] = (ad.func == FGPU_AGG_SUM && !ad.is_float) ? 0u : 1u;
+    td.agg_func[td.na++] = uint32_t(ad.func) | (ad.is_float ? 0x100u : 0u);
+  }
+  return true;
+}
+
+// *took: the kernel took the row group.  A row group where a leaf selects nothing is taken and dropped: under the
+// conjunction no row of it passes.
+int32_t tile_admit(TilePlan& T, fgpu_ctx* ctx, const Compiled& c, const QueryDesc& qd, const VisibleRG& v, const ChunkDesc* chunks, const LeafRt* lrt,
+                   bool* took) {
+  *took = false;
+  const RowGroupHost& rg = *v.rg;
+  if (rg.n_rows == 0) return FGPU_OK;
+  const TileAggDesc& td = T.td;
+  bool none = false;
+  for (int l = 0; l < qd.n_leaves; l++)
+    if (lrt[l].mode == LM_NONE) none = true;
+  TileAggRg tr{};
+  tr.n_rows = rg.n_rows;
+  bool plain_needed[kTaPlain] = {false};
+  for (uint32_t i = 0; i < td.nl; i++) {
+    const int ql = T.leaf_q[i];
+    const LeafDesc& ld = qd.leaves[ql];
+    if (lrt[ql].mode == LM_ALL) { tr.leaf_skip[i] = 1; continue; }
+    plain_needed[td.leaf_plain[i]] = true;
+    if (ld.cmp_float) { std::memcpy(&tr.lo[i], &ld.lo_f, 8); std::memcpy(&tr.hi[i], &ld.hi_f, 8); }
+    else { tr.lo[i] = ld.lo_i; tr.hi[i] = ld.hi_i; }
+  }
+  for (uint32_t i = 0; i < td.na; i++) plain_needed[td.agg_plain[i]] = true;
+  for (uint32_t i = 0; i < td.n_plain && !none; i++) {
+    const ChunkDesc& d = chunks[T.plain_slot[i]];
+    tr.plain[i] = nullptr;
+    if (!plain_needed[i]) continue;
+    if (d.kind != CK_PLAIN64 || d.has_nulls) return FGPU_OK;
+    tr.plain[i] = d.values;
+  }
+  bool code_needed[kTaCodes] = {false};
+  for (uint32_t i = 0; i < td.np; i++) {
+    const int ql = T.pred_q[i];
+    const LeafRt& rt = lrt[ql];
+    tr.pred_lut[i] = nullptr;
+    if (rt.mode != LM_EVAL) continue;  // decided: passes (a NONE row group is dropped as a whole)
+    code_needed[td.pred_code[i]] = true;
+    tr.pred_lut[i] = lut_ref(c.leaves[size_t(ql)].lut_off);
+    T.td.pred_null[i] = rt.null_result;
+  }
+  for (uint32_t i = 0; i < td.nk; i++) code_needed[td.key_code[i]] = true;
+  for (uint32_t i = 0; i < td.n_codes && !none; i++) {
+    const ChunkDesc& d = chunks[T.code_slot[i]];
+    tr.codes[i] = nullptr;
+    if (!code_needed[i] || d.kind == CK_ABSENT) continue;  // absent column: NULL for every row
+    if (d.kind != CK_DICT_STR) return FGPU_OK;
+    const std::string& name = c.slot_names[size_t(T.code_slot[i])];
+    if (int32_t rc = ensure_flat(ctx, v.part, name)) return rc;
+    const ChunkHost& ch = rg.cols.at(name);
+    if (!ch.flat) return FGPU_OK;
+    tr.codes[i] = ch.flat;
+    tr.code_w[i] = ch.flat_w;
+    tr.code_bias[i] = ch.flat_bias;
+    T.code_wmax[i] = std::max<uint32_t>(T.code_wmax[i], ch.flat_w);
+  }
+  *took = true;
+  if (none) return FGPU_OK;
+  for (uint32_t i = 0; i < td.na; i++) {  // bounds of the int64 Sum inputs (see TileAggDesc::sums_fit32)
+    if (td.cell64[i]) continue;
+    const ChunkHost& ch = rg.cols.at(c.slot_names[size_t(T.plain_slot[td.agg_plain[i]])]);
+    if (!ch.has_minmax || ch.phys != PT_INT64 || ch.min_bits < 0 || ch.max_bits > 0xffffffffll) T.agg_bounded = false;
+    else T.agg_max = std::max<uint64_t>(T.agg_max, uint64_t(ch.max_bits));
+  }
+  T.rgs.push_back(tr);
+  return FGPU_OK;
+}
+
+// Tile size, ring depth and the shared-memory table; the chunk of tiles a CTA takes at a time.
+int32_t tile_layout(TilePlan& T, const QueryDesc& qd, const Switches& w, int sm_count) {
+  TileAggDesc& td = T.td;
+  td.n_rg = uint32_t(T.rgs.size());
+  td.table_slots = qd.table_slots;
+  // replicas of small tables: same-address CAS on 64-bit cells serialises, 32 lanes on 17 slots
+  uint32_t rl = 0;
+  while (rl < 5 && (uint64_t(qd.table_slots) << (rl + 1)) <= 2048) rl++;
+  td.rep_log2 = rl;
+  const uint64_t cells = uint64_t(qd.table_slots) << rl;
+  uint64_t tb = (cells * 4 + 7) & ~uint64_t(7);
+  for (uint32_t a = 0; a < td.na; a++) {
+    td.cell_off[a] = uint32_t(tb);
+    tb += (cells * (td.cell64[a] ? 8 : 4) + 7) & ~uint64_t(7);
+  }
+  const uint64_t kSmemMax = 227 * 1024;
+  // tile rows: multiples of the rows the consumer threads take per turn (kTaConsumerWarps * 32 lanes * 4 rows)
+  const int cand[10][2] = {{6144, 3}, {3072, 4}, {3072, 3}, {6144, 2}, {3072, 2}, {1536, 4}, {1536, 3}, {1536, 2}, {768, 3}, {768, 2}};
+  auto slot_bytes_for = [&](uint32_t rows) {
+    uint64_t off = 0;
+    for (uint32_t i = 0; i < td.n_plain; i++) { td.plain_off[i] = uint32_t(off); off += uint64_t(rows) * 8; }
+    for (uint32_t i = 0; i < td.n_codes; i++) {
+      td.code_off[i] = uint32_t(off);
+      off += (uint64_t(rows) * std::max<uint32_t>(T.code_wmax[i], 8) / 8 + 127) & ~uint64_t(127);
+    }
+    return std::max<uint64_t>(off, 128);
+  };
+  bool fits = false;
+  for (int smem_table = tb < kSmemMax && !w.ta_global ? 1 : 0; smem_table >= 0 && !fits; smem_table--) {
+    for (const auto& cs : cand) {
+      if ((w.ta_tile && cs[0] != w.ta_tile) || (w.ta_stages && cs[1] != w.ta_stages)) continue;
+      const uint64_t sb = slot_bytes_for(uint32_t(cs[0]));
+      const uint64_t total = 128 + uint64_t(cs[1]) * (256 + sb) + (smem_table ? tb : 0);
+      if (total > kSmemMax) continue;
+      td.tile_rows = uint32_t(cs[0]);
+      td.n_stages = uint32_t(cs[1]);
+      td.slot_bytes = uint32_t(sb);
+      td.smem_table = uint32_t(smem_table);
+      fits = true;
+      break;
+    }
+  }
+  if (!fits) return fail(FGPU_ERR_UNSUPPORTED, "tile aggregate: the projected columns do not fit the shared-memory ring");
+  td.table_bytes = uint32_t(td.smem_table ? tb : 0);
+  uint32_t t = 0;
+  for (const TileAggRg& r : T.rgs) {
+    T.first_tile.push_back(t);
+    t += (r.n_rows + td.tile_rows - 1) / td.tile_rows;
+  }
+  T.first_tile.push_back(t);
+  td.n_tiles = t;
+  td.chunk_tiles = std::max<uint32_t>(1, t / (uint32_t(sm_count) * 4));  // ~4 turns per CTA: a CTA stays inside one row group for a whole chunk
+  // (the override comes first: the 32-bit Sum bound below depends on the chunk length the launch uses)
+  if (w.ta_chunk) td.chunk_tiles = uint32_t(w.ta_chunk);
+  td.keys8 = 1;
+  for (uint32_t i = 0; i < td.nk; i++)
+    if (T.code_wmax[td.key_code[i]] > 8) td.keys8 = 0;
+  {  // can a Sum leave 32 bits inside one CTA?  rows per CTA <= its share of the tiles (+ one chunk), all in one slot
+    const uint64_t grid = uint64_t(std::max(1, sm_count));
+    const uint64_t rows_per_cta = std::min<uint64_t>(uint64_t(t), uint64_t(t) / grid + 2 * uint64_t(td.chunk_tiles) + 1) * td.tile_rows;
+    // agg_max * rows_per_cta <= 2^32 - 1, without the product (a large chunk override would overflow it)
+    td.sums_fit32 = (T.agg_bounded && !w.ta_carry && (T.agg_max == 0 || rows_per_cta <= 0xffffffffull / T.agg_max)) ? 1u : 0u;
+  }
+  return FGPU_OK;
+}
+
+// ---- filter-only plans over PLAIN columns: ordered take (take_rows.cu) instead of k_rows ----
+struct TakePlan {
+  TakeDesc td{};
+  std::vector<TakeRg> rgs;
+  std::vector<uint32_t> first_span;
+  int range[kTakeLeaves] = {0}, pred[kTakePreds] = {0};  // range leaves (PLAIN int64 columns) and dictionary leaves (flat
+  int n_range = 0, n_pred = 0;                           // codes + result byte per dictionary id) of the plan
+};
+
+// general: row groups left with the general kernel (all of them unless pruning dropped some).
+bool take_query(const Compiled& c, const QueryDesc& qd, const Switches& w, int general, TakePlan* P) {
+  if (w.no_take || qd.n_out < 1 || qd.n_out > kTakeOut || qd.n_leaves > kTakeLeaves + kTakePreds || (qd.n_filter_prog != 0 && qd.filter_kind != FK_AND) ||
+      general == 0)
+    return false;
+  for (int l = 0; l < qd.n_leaves; l++) {
+    const LeafDesc& ld = qd.leaves[l];
+    if (ld.slot == 0xff) return false;
+    if (qd.slot_type[ld.slot] == ST_DICT) {
+      if (P->n_pred >= kTakePreds || general != c.qd.n_rg) return false;
+      P->pred[P->n_pred++] = l;
+    } else if (ld.cmp_float || ld.neg || qd.slot_type[ld.slot] != ST_I64 || c.leaves[size_t(l)].null_literal || P->n_range >= kTakeLeaves) {
+      return false;
+    } else {
+      P->range[P->n_range++] = l;
+    }
+  }
+  for (int o = 0; o < qd.n_out; o++)
+    if (qd.slot_type[qd.out_slot[o]] == ST_DICT) return false;
+  return true;
+}
+
+// *ok: the take kernels can read row group g (rows plans: every row group is a general one, g == its index in c.rgs).
+int32_t take_admit(TakePlan& P, fgpu_ctx* ctx, const Compiled& c, const QueryDesc& qd, int g, const GeneralTables& G, bool* ok) {
+  *ok = false;
+  const ChunkDesc* chunks = &G.chunks[size_t(g) * qd.n_slots];
+  const LeafRt* lrt = &G.lrt[size_t(g) * qd.n_leaves];
+  TakeRg tr{};
+  tr.n_rows = G.rg_rows[size_t(g)];
+  bool all = qd.n_leaves > 0;
+  for (int l = 0; l < qd.n_leaves; l++) {
+    if (lrt[l].mode == LM_NONE) return FGPU_OK;  // (only with pruning switched off)
+    if (lrt[l].mode != LM_ALL) all = false;
+  }
+  tr.all_pass = all ? 1 : 0;
+  for (int i = 0; i < P.n_range; i++) {
+    const int l = P.range[i];
+    const bool decided = lrt[l].mode == LM_ALL;
+    tr.lo[i] = decided ? std::numeric_limits<int64_t>::min() : qd.leaves[l].lo_i;
+    tr.hi[i] = decided ? std::numeric_limits<int64_t>::max() : qd.leaves[l].hi_i;
+    tr.leaf_col[i] = nullptr;  // decided (or nothing to evaluate at all): the kernels skip the leaf
+    if (all || decided) continue;
+    const ChunkDesc& d = chunks[qd.leaves[l].slot];
+    if (d.kind != CK_PLAIN64 || d.has_nulls) return FGPU_OK;
+    tr.leaf_col[i] = d.values;
+  }
+  for (int i = 0; i < P.n_pred; i++) {
+    const int l = P.pred[i];
+    const LeafRt& rt = lrt[l];
+    tr.pred_codes[i] = nullptr;
+    if (all || rt.mode == LM_ALL) continue;
+    const ChunkDesc& d = chunks[qd.leaves[l].slot];
+    if (d.kind != CK_DICT_STR) return FGPU_OK;
+    const std::string& name = c.slot_names[size_t(qd.leaves[l].slot)];
+    if (int32_t rc = ensure_flat(ctx, c.rgs[size_t(g)].part, name)) return rc;
+    const ChunkHost& ch = c.rgs[size_t(g)].rg->cols.at(name);
+    if (!ch.flat) return FGPU_OK;
+    tr.pred_codes[i] = ch.flat;
+    tr.pred_w[i] = ch.flat_w;
+    tr.pred_bias[i] = ch.flat_bias;
+    tr.pred_null[i] = rt.null_result;
+    tr.pred_lut[i] = lut_ref(c.leaves[size_t(l)].lut_off);
+  }
+  for (int o = 0; o < qd.n_out; o++) {
+    const ChunkDesc& d = chunks[qd.out_slot[o]];
+    if (d.kind != CK_PLAIN64 || d.has_nulls) return FGPU_OK;
+    tr.out_col[o] = d.values;
+  }
+  P.rgs.push_back(tr);
+  *ok = true;
+  return FGPU_OK;
+}
+
+// Spans of span_blocks * 256 rows, about four per resident warp.
+void take_layout(TakePlan& P, const QueryDesc& qd, int sm_count) {
+  TakeDesc& td = P.td;
+  const uint64_t warps = uint64_t(take_resident_warps(sm_count));
+  uint64_t total = 0;
+  for (const TakeRg& r : P.rgs) total += r.n_rows;
+  uint64_t span_blocks = std::min<uint64_t>(64, std::max<uint64_t>(4, total / (warps * 4 * 256)));
+  td.span_blocks = uint32_t(span_blocks);
+  const uint64_t span_rows = span_blocks * 256;
+  uint32_t spans = 0;
+  for (const TakeRg& r : P.rgs) {
+    P.first_span.push_back(spans);
+    spans += uint32_t((uint64_t(r.n_rows) + span_rows - 1) / span_rows);
+  }
+  P.first_span.push_back(spans);
+  td.n_spans = spans;
+  td.n_rg = uint32_t(P.rgs.size());
+  td.nl = uint32_t(P.n_range);
+  td.np = uint32_t(P.n_pred);
+  td.n_out = uint32_t(qd.n_out);
+}
+
+// The host image of an Execute's descriptor block: pieces at 16-byte aligned offsets, in the order they are added,
+// copied into page-locked scratch and uploaded with one copy.  A piece without a source is left zero.
+struct HostImage {
+  struct Piece { const void* src; size_t bytes, off; };
+  std::vector<Piece> pieces;
+  size_t end = 0;
+  static size_t align16(size_t x) { return (x + 15) & ~size_t(15); }
+  size_t add(const void* src, size_t bytes) {
+    const size_t off = align16(end);
+    pieces.push_back({src, bytes, off});
+    end = off + bytes;
+    return off;
+  }
+  template <class T> size_t add(const std::vector<T>& v) { return add(v.data(), v.size() * sizeof(T)); }
+  void copy_to(uint8_t* dst) const {
+    for (const Piece& p : pieces)
+      if (p.src && p.bytes) std::memcpy(dst + p.off, p.src, p.bytes);
+  }
+};
+
+// The result's columns: the keys with their dictionaries snapshotted now (the plan may be reused while they grow),
+// then the aggregates' names and types.
+void result_shape(const QueryPlan& q, const Compiled& c, std::vector<KeyOut>* keys, std::vector<std::string>* agg_names, std::vector<uint8_t>* agg_is_float) {
+  *keys = c.keys;
+  for (KeyOut& k : *keys) {
+    if (k.dict) {
+      const uint32_t card = k.dict->cardinality();
+      k.dict_snapshot.reserve(card);
+      for (uint32_t i = 0; i < card; i++) k.dict_snapshot.push_back(k.dict->value(i));
+      k.dict = nullptr;
+    }
+  }
+  for (size_t a = 0; a < q.aggs.size(); a++) {
+    agg_names->push_back(std::string(agg_string(q.aggs[a].func)) + "(" + q.expr_name(q.aggs[a].expr) + ")");
+    // Count yields int64; Sum/Min/Max keep the input type (aggregate.go:734-950)
+    agg_is_float->push_back(c.qd.aggs[a].func != FGPU_AGG_COUNT && c.qd.aggs[a].is_float);
+  }
+}
+
+// A utf8 dictionary column of the entries `ids` of `values` (all of them when null), in that order.
+std::unique_ptr<OwnedColumn> dict_column(const std::vector<std::string>& values, const std::vector<uint32_t>* ids) {
+  auto d = std::make_unique<OwnedColumn>();
+  d->format = "z";
+  d->length = int64_t(ids ? ids->size() : values.size());
+  d->offsets.push_back(0);
+  for (size_t i = 0; i < size_t(d->length); i++) {
+    const std::string& v = values[ids ? (*ids)[i] : i];
+    d->data.insert(d->data.end(), v.begin(), v.end());
+    d->offsets.push_back(int32_t(d->data.size()));
+  }
+  return d;
+}
+
+// First Execute of a cached plan: the plan keeps the device state; the dense table comes back compacted by
+// k_finalize_dense (see ExecCache).
+int32_t keep_exec_cache(fgpu_ctx* ctx, const QueryPlan& q, Compiled& c, const QueryDesc& qd, fgpu_result* res, PhaseClock& pc) {
+  cudaStream_t s = ctx->stream;
+  fgpu_stats& st = res->stats;
+  ExecCache& x = *c.exec;
+  DenseOut& f = x.dout;
+  f.table_slots = qd.table_slots;
+  f.max_out = qd.table_slots;
+  f.n_keys = uint32_t(qd.n_keys);
+  f.n_aggs = uint32_t(qd.n_aggs);
+  for (int k = 0; k < qd.n_keys; k++) {
+    f.stride[k] = qd.keys[k].dense_stride;
+    f.radix[k] = c.radix(k);
+  }
+  f.t_rows = qd.t_rows;
+  for (int a = 0; a < kMaxAggs; a++) f.t_agg[a] = qd.t_agg[a];
+  f.counters = qd.counters;
+  {  // what the collective tail needs to fold partial tables itself (layout of table_layout())
+    int pos = 0;
+    for (int a = 0; a < qd.n_aggs; a++) {
+      f.agg_func[a] = qd.aggs[a].func;
+      f.agg_is_float[a] = qd.aggs[a].is_float;
+      f.agg_pos[a] = qd.aggs[a].func == FGPU_AGG_COUNT ? int8_t(-1) : int8_t(pos++);
+    }
+  }
+  x.out_bytes = 256 + size_t(qd.n_keys) * ((size_t(f.max_out) * 4 + 7) & ~size_t(7)) + size_t(qd.n_aggs) * f.max_out * 8;
+  CUDA_TRY(x.out.alloc(256, s));  // working header (k_finalize_dense leaves it zero)
+  CUDA_TRY(cudaMemsetAsync(x.out.p, 0, 256, s));
+  f.hdr = static_cast<uint32_t*>(x.out.p);
+  f.out = nullptr;  // a page-locked block per Execute (cached_tail)
+  x.pool = ctx->pinned;
+  x.pinned = ctx->pinned_take(x.out_bytes, &x.pinned_cap);
+  if (!x.pinned) return fail(FGPU_ERR_OOM, "page-locked memory for the result image");
+  if (!res->pending) {
+    if (int32_t rc = cached_tail(ctx, x)) return rc;
+  } else {
+    CUDA_TRY(cudaMemcpyAsync(x.pinned + 32, qd.counters, 32, cudaMemcpyDeviceToHost, s));  // (rows selected by this rank's scan)
+  }
+  CUDA_TRY(cudaEventRecord(ctx->ev[3], s));
+  pc.mark("launch");
+  CUDA_TRY(cudaStreamSynchronize(s));  // the host image stays valid until here
+  pc.mark("sync");
+  release_staging(ctx);
+  st.h2d_bytes += c.h2d_bytes;
+  float ms = 0;
+  CUDA_TRY(cudaEventElapsedTime(&ms, ctx->ev[1], ctx->ev[2]));
+  st.scan_kernel_ms = ms;
+  CUDA_TRY(cudaEventElapsedTime(&ms, ctx->ev[0], ctx->ev[3]));
+  st.total_device_ms = ms;
+  const unsigned long long* cnts = reinterpret_cast<const unsigned long long*>(x.pinned + 32);
+  st.rows_selected = cnts[0];
+  x.qd = qd;
+  result_shape(q, c, &x.keys, &x.agg_names, &x.agg_is_float);
+  for (const KeyOut& k : x.keys) {  // small dictionaries are exported whole: the host then only copies index columns
+    x.dict_template.push_back(k.dict_snapshot.size() <= 4096 ? dict_column(k.dict_snapshot, nullptr) : nullptr);
+  }
+  st.kernel_launches++;  // k_finalize_dense (cached_tail)
+  x.stats = st;  // what a cached Execute reports: no uploads, no compile
+  x.stats.h2d_bytes = 0;
+  x.stats.d2h_bytes = 0;
+  x.stats.rows_selected = 0;
+  x.ready = true;
+  st.d2h_bytes += x.out_bytes;
+  res->qd = qd;
+  pc.mark("keep");
+  pc.flush("scan");
+  if (res->pending) {
+    res->pending_cached = &x;
+    return FGPU_OK;
+  }
+  return finalize_dense_host(ctx, res, x);
+}
+
+// Rows plan: one output array per projected column (worst case every row is selected) + look-back state per tile.
+int32_t alloc_rows_out(fgpu_ctx* ctx, uint64_t total_rows, uint32_t tiles, DevBuf& buf, QueryDesc* qd) {
+  std::vector<size_t> out_off(size_t(qd->n_out)), valid_off(size_t(qd->n_out));
+  size_t out_bytes = 0;
+  auto al = [](size_t x) { return (x + 255) & ~size_t(255); };
+  for (int o = 0; o < qd->n_out; o++) {
+    bool dict = qd->slot_type[qd->out_slot[o]] == ST_DICT;
+    out_off[size_t(o)] = out_bytes;
+    out_bytes = al(out_bytes + size_t(total_rows) * (dict ? 4 : 8));
+    valid_off[size_t(o)] = out_bytes;
+    if (!dict) out_bytes = al(out_bytes + size_t(total_rows));
+  }
+  const size_t state_off = out_bytes;
+  out_bytes = al(out_bytes + size_t(tiles) * 8);
+  CUDA_TRY(buf.alloc(out_bytes, ctx->stream));
+  uint8_t* ob = static_cast<uint8_t*>(buf.p);
+  for (int o = 0; o < qd->n_out; o++) {
+    qd->out_data[o] = ob + out_off[size_t(o)];
+    qd->out_valid[o] = ob + valid_off[size_t(o)];
+  }
+  qd->tile_state = reinterpret_cast<unsigned long long*>(ob + state_off);
+  return FGPU_OK;
+}
+
+// Plans and launches one Execute.  On success the result owns the device table (or, for a cached plan, the plan does).
 // collective: 0 no exchange; 1 / 2: the first run of a plan pushes its partial table and leaves the result pending
 // (the merge half is collective_end); a cached plan does what run_cached does for the mode.
 int32_t run_scan(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, fgpu_result* res, bool count_groups = false, bool cacheable = false,
@@ -1833,655 +2661,83 @@ int32_t run_scan(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, fgpu_result* re
   PhaseClock pc;
   Table& plan_table = ctx->tables[q.table];
   if (plan_table.epoch == 0) plan_table.epoch = ++ctx->epoch_counter;
-  const std::string env_now = env_switches();
-  if (!q.plan_cache || q.cache_epoch != plan_table.epoch || q.cache_tx != tx || q.cache_env != env_now || env_has(env_now, "FROSTGPU_NO_PLAN_CACHE")) {
+  const Switches w = switches();
+  if (!q.plan_cache || q.cache_epoch != plan_table.epoch || q.cache_tx != tx || q.cache_env != w.key || w.no_plan_cache) {
     std::shared_ptr<void> fresh(new Compiled(), [](void* p) { delete static_cast<Compiled*>(p); });
-    int32_t rc0 = compile(ctx, q, tx, static_cast<Compiled*>(fresh.get()));
+    int32_t rc0 = compile(ctx, q, tx, w, static_cast<Compiled*>(fresh.get()));
     q.plan_cache.reset();
     if (rc0) return rc0;
     q.plan_cache = std::move(fresh);
     q.cache_epoch = plan_table.epoch;
     q.cache_tx = tx;
-    q.cache_env = env_now;
+    q.cache_env = w.key;
   } else {
     static_cast<Compiled*>(q.plan_cache.get())->h2d_bytes = 0;  // nothing is uploaded by a cached plan
   }
   Compiled& c = *static_cast<Compiled*>(q.plan_cache.get());
-  if (cacheable && c.exec && c.exec->ready && !env_has(env_now, "FROSTGPU_NO_EXEC_CACHE")) return run_cached(ctx, *c.exec, res, collective);
+  if (cacheable && c.exec && c.exec->ready && !w.no_exec_cache) return run_cached(ctx, *c.exec, res, collective);
   c.exec.reset();
   for (LeafHost& lh : c.leaves) lh.lut_off = size_t(-1);  // per-Execute state of the plan
-  int32_t rc = FGPU_OK;
-  (void)rc;
   pc.mark("compile");
   QueryDesc qd = c.qd;  // a copy: the plan in `c` may be reused by the next Execute
   const int n_rg = qd.n_rg, n_slots = qd.n_slots, n_leaves = qd.n_leaves;
+  const bool rows_plan = q.kind == FGPU_PLAN_FILTER;
   fgpu_stats& st = res->stats;
   st.rows_scanned = c.total_rows;
   st.rows_touched = c.touched_rows == ~uint64_t(0) ? c.total_rows : c.touched_rows;
   st.row_groups = uint32_t(n_rg);
   st.row_groups_pruned = c.pruned_row_groups;
 
-  // ---- per row group tables: chunk descriptors, leaf runtime, leaf LUTs, tile prefix -----------
-  std::vector<ChunkDesc> chunks(size_t(n_rg) * std::max(n_slots, 1));
-  std::vector<LeafRt> lrt(size_t(n_rg) * std::max(n_leaves, 1));
-  std::vector<uint32_t> first_tile(size_t(n_rg) + 1), rg_rows(std::max(n_rg, 1));
-  std::vector<uint8_t> lutbytes;
-  std::vector<std::pair<size_t, size_t>> lut_fix;  // (index into lrt, offset into lutbytes)
-  uint32_t tiles = 0;
-  const uint32_t tile_len = q.kind == FGPU_PLAN_FILTER ? uint32_t(kTileRows) : uint32_t(qd.vl);  // rows plan: CTA tiles; scan: warp vectors
-  // ---- sorted-run scan: query-level eligibility (see runs_tma.cu) --------------------------------
-  // One launch over the qualifying row groups; a row group whose statistics already decided every
-  // leaf is flagged all_pass (its leaf columns are neither uploaded nor staged).
-  struct RunsRgCols {  // the chunks behind RunsRg::col (null: not staged)
-    Part* part = nullptr;
-    ChunkHost* ch[kRunsCols] = {nullptr};
-  };
-  struct RunsBatch {
-    RunsDesc rd{};
-    int nl = 0;
-    int col_slot[kRunsCols] = {0};
-    std::vector<RunsRg> rgs;
-    std::vector<RunsRgCols> cols;
-    std::vector<uint32_t> rows, first_span;
-    size_t o_rg = 0, o_span = 0;
-  };
-  RunsBatch batches[1];
-  // Row groups of the sorted-run shape whose filter the statistics decided, without undecided dictionary leaves and with
-  // Sum(int64) as the only stored aggregates, are answered from prefix sums instead (k_runs_prefix, runs_prefix.cu) when
-  // their runs average at least kPrefixRunRows rows: then a step per group run is cheaper than reading its rows.
-  constexpr uint64_t kPrefixRunRows = 64;
-  struct PrefixBatch {
-    PrefixDesc pd{};
-    std::vector<PrefixRg> rgs;
-    std::vector<std::array<ChunkHost*, kRunsAggs>> sums;  // per row group: the chunk of every Sum input
-    std::vector<Part*> parts;
-    std::vector<PrefixWin> wins;
-    size_t o_rg = 0, o_win = 0;
-  } PB;
-  int runs_nl = 0, runs_nk = 0, runs_na = 0, runs_np = 0;
-  int runs_leaf_index[kRunsLeaves] = {0}, runs_pred_leaf[kRunsPreds] = {0};  // query leaf behind every range / dictionary leaf
-  int runs_leaf_slot[kRunsLeaves] = {0}, runs_agg_slot[kRunsAggs] = {0}, runs_agg_index[kRunsAggs] = {0};
-  uint32_t runs_agg_func[kRunsAggs] = {0};
-  bool runs_q = q.kind != FGPU_PLAN_FILTER && c.runs_shape && !getenv("FROSTGPU_NO_RUNS");
-  if (runs_q) {
-    for (int l = 0; l < n_leaves && runs_q; l++) {
-      const LeafDesc& ld = qd.leaves[l];
-      if (ld.slot != 0xff && qd.slot_type[ld.slot] == ST_DICT) {  // dictionary leaf: evaluated once per run
-        if (runs_np >= kRunsPreds) runs_q = false;
-        else runs_pred_leaf[runs_np++] = l;
-      } else if (ld.slot == 0xff) {  // column absent from every row group: ALL / NONE everywhere, nothing to evaluate
-        if (runs_np >= kRunsPreds) runs_q = false;
-        else runs_pred_leaf[runs_np++] = l;
-      } else if (ld.cmp_float || ld.neg || qd.slot_type[ld.slot] != ST_I64 || runs_nl >= kRunsLeaves) {
-        runs_q = false;
-      } else {
-        runs_leaf_index[runs_nl] = l;
-        runs_leaf_slot[runs_nl++] = ld.slot;
-      }
-    }
-    for (int a = 0; a < qd.n_aggs && runs_q; a++) {
-      if (qd.aggs[a].func == FGPU_AGG_COUNT) continue;
-      if ((qd.aggs[a].func != FGPU_AGG_SUM && qd.aggs[a].func != FGPU_AGG_MIN && qd.aggs[a].func != FGPU_AGG_MAX) || runs_na >= kRunsAggs) { runs_q = false; break; }
-      runs_agg_slot[runs_na] = qd.prog[qd.aggs[a].prog_off].slot;
-      runs_agg_func[runs_na] = uint32_t(qd.aggs[a].func) | (qd.aggs[a].is_float ? 0x100u : 0u);
-      runs_agg_index[runs_na++] = a;
-    }
-    if (qd.n_keys > kRunsKeys) runs_q = false;
-    runs_nk = qd.n_keys;
-  }
-  bool prefix_q = runs_q && !getenv("FROSTGPU_NO_PREFIX");
-  for (int a = 0; a < runs_na && prefix_q; a++)
-    if (runs_agg_func[a] != uint32_t(FGPU_AGG_SUM)) prefix_q = false;  // Min / Max / float64 Sum stay with k_runs_tma
-  if (runs_q) {  // distinct staged columns of each batch
-    for (int bi = 0; bi < 1; bi++) {
-      RunsBatch& B = batches[bi];
-      auto col_of = [&](int slot) {
-        for (uint32_t i = 0; i < B.rd.n_cols; i++)
-          if (B.col_slot[i] == slot) return i;
-        B.col_slot[B.rd.n_cols] = slot;
-        return B.rd.n_cols++;
-      };
-      B.nl = runs_nl;
-      for (int l = 0; l < B.nl; l++) B.rd.leaf_col[l] = col_of(runs_leaf_slot[l]);
-      for (int a = 0; a < runs_na; a++) {
-        B.rd.agg_col[a] = col_of(runs_agg_slot[a]);
-        B.rd.agg_func[a] = runs_agg_func[a];
-      }
-      for (int k = 0; k < runs_nk; k++) B.rd.stride[k] = qd.keys[k].dense_stride;
-      B.rd.n_pred = uint32_t(runs_np);
-    }
-  }
-  // ---- tile aggregate: query-level eligibility (see tile_agg.cu) -------------------------------------
-  // Row groups the sorted-run kernel does not take (bit-packed / short-run / nullable keys, L0 records) go to
-  // the tile-aggregate kernel when the plan is a conjunction of range + dictionary leaves over a dense table
-  // with plain aggregate inputs; what is left after that stays with the general scan kernel.
-  struct TaBatch {
-    TileAggDesc td{};
-    std::vector<TileAggRg> rgs;
-    std::vector<uint32_t> rows, first_tile;
-    size_t o_rg = 0, o_tile = 0;
-    int plain_slot[kTaPlain] = {0}, code_slot[kTaCodes] = {0};
-    uint32_t code_wmax[kTaCodes] = {0};
-    int leaf_q[kTaLeaves] = {0}, pred_q[kTaPreds] = {0}, agg_index[kTaAggs] = {0};
-    bool agg_bounded = true;          // every int64 Sum input of every row group has statistics inside [0, 2^32)
-    uint64_t agg_max = 0;             // the largest of those chunk maxima
-  } TA;
-  bool ta_q = q.kind != FGPU_PLAN_FILTER && qd.table_mode == TM_DENSE && (qd.n_filter_prog == 0 || qd.filter_kind == FK_AND) &&
-              qd.n_keys <= kTaKeys && !getenv("FROSTGPU_NO_TILE");
-  {
-    TileAggDesc& td = TA.td;
-    auto plain_of = [&](int slot) -> int {
-      for (uint32_t i = 0; i < td.n_plain; i++)
-        if (TA.plain_slot[i] == slot) return int(i);
-      if (td.n_plain >= uint32_t(kTaPlain)) return -1;
-      TA.plain_slot[td.n_plain] = slot;
-      return int(td.n_plain++);
-    };
-    auto code_of = [&](int slot) -> int {
-      for (uint32_t i = 0; i < td.n_codes; i++)
-        if (TA.code_slot[i] == slot) return int(i);
-      if (td.n_codes >= uint32_t(kTaCodes)) return -1;
-      TA.code_slot[td.n_codes] = slot;
-      return int(td.n_codes++);
-    };
-    for (int l = 0; l < n_leaves && ta_q; l++) {
-      const LeafDesc& ld = qd.leaves[l];
-      if (ld.slot == 0xff) continue;  // column absent from every row group: ALL / NONE per row group, nothing to evaluate
-      if (qd.slot_type[ld.slot] == ST_DICT) {
-        const int cc = code_of(ld.slot);
-        if (td.np >= uint32_t(kTaPreds) || cc < 0) { ta_q = false; break; }
-        TA.pred_q[td.np] = l;
-        td.pred_code[td.np++] = uint32_t(cc);
-      } else {
-        const int pp = plain_of(ld.slot);
-        if (c.leaves[size_t(l)].null_literal || td.nl >= uint32_t(kTaLeaves) || pp < 0) { ta_q = false; break; }
-        TA.leaf_q[td.nl] = l;
-        td.leaf_plain[td.nl] = uint32_t(pp);
-        td.leaf_flags[td.nl++] = (ld.cmp_float ? 1u : 0u) | (qd.slot_type[ld.slot] == ST_F64 ? 2u : 0u) | (ld.neg ? 4u : 0u);
-      }
-    }
-    for (int k = 0; k < qd.n_keys && ta_q; k++) {
-      const int cc = code_of(qd.keys[k].slot);
-      if (qd.keys[k].is_int64 || cc < 0) { ta_q = false; break; }
-      td.key_code[td.nk] = uint32_t(cc);
-      td.key_stride[td.nk++] = qd.keys[k].dense_stride;
-    }
-    for (int a = 0; a < qd.n_aggs && ta_q; a++) {
-      const AggDesc& ad = qd.aggs[a];
-      if (ad.func == FGPU_AGG_COUNT) continue;
-      const bool simple = ad.prog_len == 1 && qd.prog[ad.prog_off].op == PO_LOAD;
-      const int pp = simple ? plain_of(qd.prog[ad.prog_off].slot) : -1;
-      if ((ad.func != FGPU_AGG_SUM && ad.func != FGPU_AGG_MIN && ad.func != FGPU_AGG_MAX) || td.na >= uint32_t(kTaAggs) || pp < 0) { ta_q = false; break; }
-      TA.agg_index[td.na] = a;
-      td.agg_plain[td.na] = uint32_t(pp);
-      td.cell64[td.na] = (ad.func == FGPU_AGG_SUM && !ad.is_float) ? 0u : 1u;
-      td.agg_func[td.na++] = uint32_t(ad.func) | (ad.is_float ? 0x100u : 0u);
-    }
-  }
-  uint32_t ta_empty_rgs = 0;
-  int gi = 0;  // row groups that stay with the general scan kernel
+  // ---- where every row group goes ----
+  GeneralTables G(n_rg, n_slots, n_leaves);
+  const uint32_t tile_len = rows_plan ? uint32_t(kTileRows) : uint32_t(qd.vl);  // rows plan: CTA tiles; scan: warp vectors
+  RunsPlan R;
+  PrefixPlan P;
+  TilePlan T;
+  const bool runs_q = !rows_plan && runs_query(c, qd, w, &R);
+  const bool prefix_q = runs_q && prefix_query(R, w);
+  const bool tile_q = !rows_plan && tile_query(c, qd, w, &T);
   for (int g0 = 0; g0 < n_rg; g0++) {
-    RowGroupHost& rg = *c.rgs[size_t(g0)].rg;
-    const int g = gi;
-    for (int s = 0; s < n_slots; s++) {
-      ChunkDesc d{};
-      d.kind = CK_ABSENT;
-      d.n_rows = rg.n_rows;
-      auto it = ((c.rgs[size_t(g0)].skip_slots >> s) & 1) ? rg.cols.end() : rg.cols.find(c.slot_names[size_t(s)]);
-      if (it != rg.cols.end()) {
-        ChunkHost& ch = it->second;
-        if (!ch.error.empty())
-          return fail(FGPU_ERR_UNSUPPORTED, "column " + c.slot_names[size_t(s)] + ": " + ch.error);
-        d = ch.desc;
-        st.algorithmic_bytes += ch.stored_bytes;
-        st.metadata_bytes += ch.meta_bytes;
+    const size_t lut_mark = G.lut_fix.size();
+    if (int32_t rc = describe_row_group(ctx, q, c, g0, G, st)) return rc;
+    const VisibleRG& v = c.rgs[size_t(g0)];
+    const ChunkDesc* row_chunks = &G.chunks[size_t(G.n) * n_slots];
+    const LeafRt* row_lrt = &G.lrt[size_t(G.n) * n_leaves];
+    bool took = false;
+    RunsCand rc;
+    if (runs_q && runs_admit(R, c, qd, v, row_chunks, row_lrt, &rc)) {
+      if (!(prefix_q && prefix_admit(P, R, rc, st))) {
+        R.rgs.push_back(rc.rr);
+        R.cols.push_back(rc.cols);
       }
-      chunks[size_t(g) * n_slots + s] = d;
+      took = true;
+    } else if (tile_q) {
+      if (int32_t e = tile_admit(T, ctx, c, qd, v, row_chunks, row_lrt, &took)) return e;
     }
-    for (int l = 0; l < n_leaves; l++) {
-      LeafHost& lh = c.leaves[size_t(l)];
-      LeafRt rt{};
-      auto it = lh.slot < 0 ? rg.cols.end() : rg.cols.find(lh.column);
-      if (it == rg.cols.end()) {
-        rt.mode = lh.missing_mode;
-      } else if (c.slot_types[size_t(lh.slot)] == ST_DICT) {
-        rt.mode = LM_EVAL;
-        rt.null_result = (lh.op == FGPU_OP_EQ && lh.lit->lit_type == FGPU_SCALAR_NULL) ? 1 : 0;
-        if (lh.lut_off == size_t(-1)) {
-          // one result byte per GLOBAL dictionary id, evaluated once per distinct dictionary entry
-          const GlobalDict& gd = ctx->tables[q.table].dicts[lh.column];
-          lh.lut_off = lutbytes.size();
-          lutbytes.resize(lh.lut_off + gd.values.size() + 1);
-          for (size_t g = 0; g < gd.values.size(); g++) lutbytes[lh.lut_off + g] = dict_leaf_value(lh, gd.values[g]) ? 1 : 0;
-        }
-        lut_fix.emplace_back(size_t(g) * n_leaves + l, lh.lut_off);
-      } else {
-        rt.mode = lh.null_literal ? LM_NONE : LM_EVAL;
-      }
-      if (c.rgs[size_t(g0)].leaf_mode[l] != LM_EVAL) rt.mode = c.rgs[size_t(g0)].leaf_mode[l];
-      lrt[size_t(g) * n_leaves + l] = rt;
+    if (took) {  // slot G.n of the general tables is reused by the next row group
+      G.lut_fix.resize(lut_mark);
+      continue;
     }
-    // ---- does this row group qualify for the sorted-run kernel? ----
-    bool runs_ok = runs_q && rg.n_rows > 0;
-    const int bi = 0;
-    bool all_pass = false;
-    if (runs_ok) {
-      bool all_all = runs_nl > 0;
-      for (int l = 0; l < runs_nl; l++) {
-        const uint8_t m = lrt[size_t(g) * n_leaves + runs_leaf_index[l]].mode;
-        if (m != LM_ALL) all_all = false;
-        if (m == LM_NONE) runs_ok = false;  // (only with pruning switched off)
-      }
-      all_pass = all_all;
-    }
-    RunsRg rr{};
-    RunsRgCols rcols{};
-    if (runs_ok) {
-      RunsBatch& B = batches[bi];
-      rr.n_rows = rg.n_rows;
-      for (int l = 0; l < B.nl; l++) {
-        const int ql = runs_leaf_index[l];
-        const bool all = lrt[size_t(g) * n_leaves + ql].mode == LM_ALL;
-        rr.lo[l] = all ? std::numeric_limits<int64_t>::min() : qd.leaves[ql].lo_i;
-        rr.hi[l] = all ? std::numeric_limits<int64_t>::max() : qd.leaves[ql].hi_i;
-      }
-      for (int i = 0; i < runs_np && runs_ok; i++) {  // dictionary leaves: one result per run
-        const int ql = runs_pred_leaf[i];
-        const LeafRt& rt = lrt[size_t(g) * n_leaves + ql];
-        rr.pred_runs[i] = nullptr;
-        if (rt.mode == LM_ALL) continue;                      // decided: passes everywhere in this row group
-        if (rt.mode == LM_NONE) { runs_ok = false; break; }   // (only with pruning switched off)
-        const ChunkDesc& d = chunks[size_t(g) * n_slots + qd.leaves[ql].slot];
-        // (short runs — a leaf on a column far down the sort order — are the tile-aggregate kernel's business: its
-        // per-row result byte costs one shared load where a cursor would move every few rows)
-        if (d.kind != CK_DICT_STR || d.row_runs == nullptr || uint64_t(d.n_row_runs) * 32 > uint64_t(rg.n_rows) + 1024) { runs_ok = false; break; }
-        rr.pred_runs[i] = d.row_runs;
-        rr.pred_seeds[i] = d.row_seeds;
-        rr.pred_n_runs[i] = d.n_row_runs;
-        rr.pred_lut[i] = reinterpret_cast<const uint8_t*>(uintptr_t(c.leaves[size_t(ql)].lut_off));  // offset, rebased below
-        B.rd.pred_null[i] = rt.null_result;
-      }
-      rr.all_pass = all_pass ? 1 : 0;
-      bool any_col = false;
-      rcols.part = c.rgs[size_t(g0)].part;
-      for (uint32_t i = 0; i < B.rd.n_cols && runs_ok; i++) {
-        const ChunkDesc& d = chunks[size_t(g) * n_slots + B.col_slot[i]];
-        rr.col[i] = nullptr;
-        if ((c.rgs[size_t(g0)].skip_slots >> B.col_slot[i]) & 1) continue;  // a decided leaf's own column
-        if (d.kind != CK_PLAIN64 || d.has_nulls) runs_ok = false;
-        rr.col[i] = d.values;
-        rcols.ch[i] = &rg.cols.at(c.slot_names[size_t(B.col_slot[i])]);
-        any_col = true;
-      }
-      // all_pass: the leaf columns stay null (not staged).  Otherwise a decided leaf still runs its
-      // (widened) range test: a staged column stands in for the one that was not uploaded (see the tile plan).
-      for (uint32_t i = 0; i < B.rd.n_cols && runs_ok && !all_pass; i++)
-        if (!rr.col[i] && !any_col) runs_ok = false;
-      if (all_pass)  // aggregate inputs must be there
-        for (int a = 0; a < runs_na && runs_ok; a++)
-          if (!rr.col[B.rd.agg_col[a]]) runs_ok = false;
-      for (int k = 0; k < runs_nk && runs_ok; k++) {
-        const ChunkDesc& d = chunks[size_t(g) * n_slots + qd.keys[k].slot];
-        // run-length only, and runs long enough that a 32-row step rarely holds two run ends
-        // (row_runs: the directory in row space; it exists when the column chunk is run-length only, NULLs included)
-        if (d.kind != CK_DICT_STR || d.row_runs == nullptr || uint64_t(d.n_row_runs) * 32 > uint64_t(rg.n_rows) + 1024) runs_ok = false;
-        rr.runs[k] = d.row_runs;
-        rr.seeds[k] = d.row_seeds;
-        rr.n_runs[k] = d.n_row_runs;
-      }
-    }
-    if (runs_ok && prefix_q && (runs_nl == 0 || all_pass)) {  // (the kernel treats a launch without range leaves as all-pass)
-      bool ok = true;
-      uint64_t sum_runs = 0;
-      for (int i = 0; i < runs_np; i++)
-        if (rr.pred_runs[i]) ok = false;  // an undecided dictionary leaf
-      for (int k = 0; k < runs_nk; k++) sum_runs += rr.n_runs[k];
-      std::array<ChunkHost*, kRunsAggs> sums{};
-      for (int a = 0; a < runs_na && ok; a++) {
-        sums[size_t(a)] = rcols.ch[batches[bi].rd.agg_col[a]];
-        if (!sums[size_t(a)] || sums[size_t(a)]->phys != PT_INT64) ok = false;
-      }
-      if (ok && uint64_t(rg.n_rows) >= kPrefixRunRows * sum_runs) {
-        PrefixRg pr{};
-        pr.n_rows = rg.n_rows;
-        for (int k = 0; k < runs_nk; k++) {
-          pr.runs[k] = rr.runs[k];
-          pr.seeds[k] = rr.seeds[k];
-          pr.n_runs[k] = rr.n_runs[k];
-          st.algorithmic_bytes += uint64_t(rr.n_runs[k]) * sizeof(Run);  // the directories, read whole
-        }
-        const uint32_t win = runs_prefix_window_rows(rg.n_rows, uint32_t(sum_runs));
-        uint32_t n_win = 0;
-        for (uint32_t r0 = 0; r0 < rg.n_rows; r0 += win, n_win++)
-          PB.wins.push_back(PrefixWin{uint32_t(PB.rgs.size()), r0, std::min(win, rg.n_rows - r0), 0u});
-        // a Sum input is read at the segment boundaries (at most every run start, every window start and the end), not
-        // row by row
-        for (int a = 0; a < runs_na; a++) {
-          bool first = true;
-          for (int a2 = 0; a2 < a; a2++) first = first && sums[size_t(a2)] != sums[size_t(a)];
-          if (first) st.algorithmic_bytes = st.algorithmic_bytes - sums[size_t(a)]->stored_bytes + (sum_runs + n_win + 1) * 8;
-        }
-        PB.rgs.push_back(pr);
-        PB.sums.push_back(sums);
-        PB.parts.push_back(rcols.part);
-        lut_fix.erase(std::remove_if(lut_fix.begin(), lut_fix.end(), [&](const std::pair<size_t, size_t>& f) { return f.first >= size_t(g) * n_leaves; }), lut_fix.end());
-        continue;  // slot g of the general tables is reused by the next row group
-      }
-    }
-    if (runs_ok) {
-      batches[bi].rgs.push_back(rr);
-      batches[bi].cols.push_back(rcols);
-      batches[bi].rows.push_back(rg.n_rows);
-      lut_fix.erase(std::remove_if(lut_fix.begin(), lut_fix.end(), [&](const std::pair<size_t, size_t>& f) { return f.first >= size_t(g) * n_leaves; }), lut_fix.end());
-      continue;  // slot g of the general tables is reused by the next row group
-    }
-    // ---- does this row group go to the tile-aggregate kernel? ----
-    if (ta_q && rg.n_rows > 0) {
-      const TileAggDesc& td = TA.td;
-      bool ok = true, none = false;
-      for (int l = 0; l < n_leaves; l++)
-        if (lrt[size_t(g) * n_leaves + l].mode == LM_NONE) none = true;  // conjunction: no row of this row group passes
-      TileAggRg tr{};
-      tr.n_rows = rg.n_rows;
-      bool plain_needed[kTaPlain] = {false};
-      for (uint32_t i = 0; i < td.nl && ok; i++) {
-        const int ql = TA.leaf_q[i];
-        const LeafDesc& ld = qd.leaves[ql];
-        if (lrt[size_t(g) * n_leaves + ql].mode == LM_ALL) { tr.leaf_skip[i] = 1; continue; }
-        plain_needed[td.leaf_plain[i]] = true;
-        if (ld.cmp_float) { std::memcpy(&tr.lo[i], &ld.lo_f, 8); std::memcpy(&tr.hi[i], &ld.hi_f, 8); }
-        else { tr.lo[i] = ld.lo_i; tr.hi[i] = ld.hi_i; }
-      }
-      for (uint32_t i = 0; i < td.na; i++) plain_needed[td.agg_plain[i]] = true;
-      for (uint32_t i = 0; i < td.n_plain && ok && !none; i++) {
-        const ChunkDesc& d = chunks[size_t(g) * n_slots + TA.plain_slot[i]];
-        tr.plain[i] = nullptr;
-        if (!plain_needed[i]) continue;
-        if (d.kind != CK_PLAIN64 || d.has_nulls) { ok = false; break; }
-        tr.plain[i] = d.values;
-      }
-      bool code_needed[kTaCodes] = {false};
-      for (uint32_t i = 0; i < td.np && ok; i++) {
-        const int ql = TA.pred_q[i];
-        const LeafRt& rt = lrt[size_t(g) * n_leaves + ql];
-        tr.pred_lut[i] = nullptr;
-        if (rt.mode != LM_EVAL) continue;  // decided: passes (a NONE row group is dropped as a whole)
-        code_needed[td.pred_code[i]] = true;
-        tr.pred_lut[i] = reinterpret_cast<const uint8_t*>(uintptr_t(c.leaves[size_t(ql)].lut_off) + 1);  // offset + 1, rebased below
-        TA.td.pred_null[i] = rt.null_result;
-      }
-      for (uint32_t i = 0; i < td.nk; i++) code_needed[td.key_code[i]] = true;
-      for (uint32_t i = 0; i < td.n_codes && ok && !none; i++) {
-        const ChunkDesc& d = chunks[size_t(g) * n_slots + TA.code_slot[i]];
-        tr.codes[i] = nullptr;
-        if (!code_needed[i] || d.kind == CK_ABSENT) continue;  // absent column: NULL for every row
-        if (d.kind != CK_DICT_STR) { ok = false; break; }
-        const std::string& name = c.slot_names[size_t(TA.code_slot[i])];
-        int32_t frc = ensure_flat(ctx, c.rgs[size_t(g0)].part, name);
-        if (frc) return frc;
-        const ChunkHost& ch = rg.cols.at(name);
-        if (!ch.flat) { ok = false; break; }
-        tr.codes[i] = ch.flat;
-        tr.code_w[i] = ch.flat_w;
-        tr.code_bias[i] = ch.flat_bias;
-        TA.code_wmax[i] = std::max<uint32_t>(TA.code_wmax[i], ch.flat_w);
-      }
-      if (ok) {
-        lut_fix.erase(std::remove_if(lut_fix.begin(), lut_fix.end(), [&](const std::pair<size_t, size_t>& f) { return f.first >= size_t(g) * n_leaves; }), lut_fix.end());
-        if (none) { ta_empty_rgs++; continue; }
-        for (uint32_t i = 0; i < td.na; i++) {  // bounds of the int64 Sum inputs (see TileAggDesc::sums_fit32)
-          if (td.cell64[i]) continue;
-          const ChunkHost& ch = rg.cols.at(c.slot_names[size_t(TA.plain_slot[td.agg_plain[i]])]);
-          if (!ch.has_minmax || ch.phys != PT_INT64 || ch.min_bits < 0 || ch.max_bits > 0xffffffffll) TA.agg_bounded = false;
-          else TA.agg_max = std::max<uint64_t>(TA.agg_max, uint64_t(ch.max_bits));
-        }
-        TA.rgs.push_back(tr);
-        TA.rows.push_back(rg.n_rows);
-        continue;  // slot g of the general tables is reused by the next row group
-      }
-    }
-    first_tile[size_t(g)] = tiles;
-    rg_rows[size_t(g)] = rg.n_rows;
-    tiles += (rg.n_rows + tile_len - 1) / tile_len;
-    gi++;
+    G.first_tile[size_t(G.n)] = G.tiles;
+    G.rg_rows[size_t(G.n)] = v.rg->n_rows;
+    G.tiles += (v.rg->n_rows + tile_len - 1) / tile_len;
+    G.n++;
   }
-  first_tile[size_t(gi)] = tiles;
-  qd.n_rg = gi;
-  qd.n_tiles = tiles;
-  // ---- sorted-run kernels: frame-of-reference and prefix-sum images, tile rows, stage layout ------------------------
-  {  // every staged int64 column and every Sum input of the prefix path of every part, in one batch
-    std::set<std::pair<Part*, std::string>> seen, pseen;
-    std::vector<std::pair<Part*, std::string>> want, want_prefix;
-    for (const RunsBatch& B : batches)
-      for (const RunsRgCols& rc2 : B.cols)
-        for (uint32_t i = 0; i < B.rd.n_cols; i++)
-          if (rc2.ch[i] && rc2.ch[i]->phys == PT_INT64 && seen.emplace(rc2.part, c.slot_names[size_t(B.col_slot[i])]).second)
-            want.emplace_back(rc2.part, c.slot_names[size_t(B.col_slot[i])]);
-    for (size_t k = 0; k < PB.rgs.size(); k++)
-      for (int a = 0; a < runs_na; a++)
-        if (pseen.emplace(PB.parts[k], c.slot_names[size_t(runs_agg_slot[a])]).second) want_prefix.emplace_back(PB.parts[k], c.slot_names[size_t(runs_agg_slot[a])]);
-    if (!want.empty() || !want_prefix.empty())
-      if (int32_t rcn = ensure_narrow(ctx, want, want_prefix)) return rcn;
-    for (size_t k = 0; k < PB.rgs.size(); k++)
-      for (int a = 0; a < runs_na; a++) {
-        PB.rgs[k].pre[a] = PB.sums[k][size_t(a)]->prefix;
-        if (!PB.rgs[k].pre[a]) return fail(FGPU_ERR_INVALID, "prefix-sum image missing for column " + c.slot_names[size_t(runs_agg_slot[a])]);
-      }
-  }
-  for (RunsBatch& B : batches) {
-    if (B.rgs.empty()) continue;
-    RunsDesc& rd = B.rd;
-    auto envi = [](const char* n, int d) { const char* e = getenv(n); return e ? atoi(e) : d; };
-    rd.n_rg = uint32_t(B.rgs.size());
-    // every row group is cut into tiles of about tile_bytes of staged column data; the launch's tile table {row group,
-    // first row} is dealt to the CTAs in chunks of consecutive entries
-    uint32_t tile_bytes = 4096 * 8;
-    { const int f = envi("FROSTGPU_RT_TILE", 0); if (f == 1024 || f == 2048 || f == 4096 || f == 8192) tile_bytes = uint32_t(f) * 8u; }  // (rows of 8 bytes)
-    uint32_t tiles_rt = 0, gidx = 0, col_region = 0, max_tile = 1024;
-    uint64_t total = 0;
-    for (uint32_t r : B.rows) total += r;
-    // small launches: at least one tile per resident CTA (three per SM), or the grid is not filled
-    const uint32_t fill_rows = uint32_t(std::min<uint64_t>(1u << 20, std::max<uint64_t>(1024, (total / (uint64_t(ctx->sm_count) * 3)) & ~uint64_t(1023))));
-    for (size_t k = 0; k < B.rgs.size(); k++) {
-      RunsRg& r = B.rgs[k];
-      uint32_t row_bytes = 0, max_runs = 0;
-      for (uint32_t i = 0; i < rd.n_cols; i++) {
-        const ChunkHost* ch = B.cols[k].ch[i];
-        r.cl[i] = RunsCol{0, 3, 0};
-        if (ch && ch->narrow) {
-          r.col[i] = ch->narrow;
-          r.cl[i].lg = ch->narrow_w == 1 ? 0 : (ch->narrow_w == 2 ? 1 : 2);
-          r.cl[i].base = ch->narrow_base;
-          st.algorithmic_bytes = st.algorithmic_bytes - ch->stored_bytes + uint64_t(r.n_rows) * ch->narrow_w;
-        }
-        if (r.col[i]) row_bytes += 1u << r.cl[i].lg;
-      }
-      for (int q = 0; q < runs_nk; q++) max_runs = std::max(max_runs, r.n_runs[q]);
-      for (int q = 0; q < runs_np; q++)
-        if (r.pred_runs[q]) max_runs = std::max(max_runs, r.pred_n_runs[q]);
-      r.tile_rows = std::min(runs_tma_tile_rows(tile_bytes, row_bytes, r.n_rows, max_runs), fill_rows);
-      int first = -1;
-      uint32_t off = 0;
-      for (uint32_t i = 0; i < rd.n_cols; i++) {
-        if (!r.col[i]) continue;
-        if (first < 0) first = int(i);
-        r.cl[i].soff = off;
-        off += ((r.tile_rows << r.cl[i].lg) + 127u) & ~127u;
-      }
-      for (uint32_t i = 0; i < rd.n_cols && first >= 0; i++)  // a column that is not staged reads a staged one
-        if (!r.col[i]) r.cl[i] = r.cl[first];
-      col_region = std::max(col_region, off);
-      max_tile = std::max(max_tile, r.tile_rows);
-      for (uint32_t r0 = 0; r0 < r.n_rows; r0 += r.tile_rows) {
-        B.first_span.push_back(gidx);
-        B.first_span.push_back(r0);
-        tiles_rt++;
-      }
-      gidx++;
-    }
-    runs_tma_plan(rd, runs_nk + runs_np, max_tile, col_region, envi("FROSTGPU_RT_STAGES", 0), envi("FROSTGPU_RT_WARPS", 0), envi("FROSTGPU_RT_SPAN", 0));
-    rd.n_spans = tiles_rt;
-  }
-
-  // ---- tile aggregate: tile size, ring depth and the shared-memory table -------------------------------
-  if (!TA.rgs.empty()) {
-    TileAggDesc& td = TA.td;
-    auto envi = [](const char* n, int d) { const char* e = getenv(n); return e ? atoi(e) : d; };
-    td.n_rg = uint32_t(TA.rgs.size());
-    td.table_slots = qd.table_slots;
-    // replicas of small tables: same-address CAS on 64-bit cells serialises, 32 lanes on 17 slots
-    uint32_t rl = 0;
-    while (rl < 5 && (uint64_t(qd.table_slots) << (rl + 1)) <= 2048) rl++;
-    td.rep_log2 = rl;
-    const uint64_t cells = uint64_t(qd.table_slots) << rl;
-    uint64_t tb = (cells * 4 + 7) & ~uint64_t(7);
-    for (uint32_t a = 0; a < td.na; a++) {
-      td.cell_off[a] = uint32_t(tb);
-      tb += (cells * (td.cell64[a] ? 8 : 4) + 7) & ~uint64_t(7);
-    }
-    const uint64_t kSmemMax = 227 * 1024;
-    // tile rows: multiples of the rows the consumer threads take per turn (kTaConsumerWarps * 32 lanes * 4 rows)
-    const int cand[10][2] = {{6144, 3}, {3072, 4}, {3072, 3}, {6144, 2}, {3072, 2}, {1536, 4}, {1536, 3}, {1536, 2}, {768, 3}, {768, 2}};
-    auto slot_bytes_for = [&](uint32_t T) {
-      uint64_t off = 0;
-      for (uint32_t i = 0; i < td.n_plain; i++) { td.plain_off[i] = uint32_t(off); off += uint64_t(T) * 8; }
-      for (uint32_t i = 0; i < td.n_codes; i++) {
-        td.code_off[i] = uint32_t(off);
-        off += (uint64_t(T) * std::max<uint32_t>(TA.code_wmax[i], 8) / 8 + 127) & ~uint64_t(127);
-      }
-      return std::max<uint64_t>(off, 128);
-    };
-    bool fits = false;
-    const int force_t = envi("FROSTGPU_TA_TILE", 0), force_s = envi("FROSTGPU_TA_STAGES", 0);
-    for (int smem_table = tb < kSmemMax && !getenv("FROSTGPU_TA_GLOBAL") ? 1 : 0; smem_table >= 0 && !fits; smem_table--) {
-      for (const auto& cs : cand) {
-        if ((force_t && cs[0] != force_t) || (force_s && cs[1] != force_s)) continue;
-        const uint64_t sb = slot_bytes_for(uint32_t(cs[0]));
-        const uint64_t total = 128 + uint64_t(cs[1]) * (256 + sb) + (smem_table ? tb : 0);
-        if (total > kSmemMax) continue;
-        td.tile_rows = uint32_t(cs[0]);
-        td.n_stages = uint32_t(cs[1]);
-        td.slot_bytes = uint32_t(sb);
-        td.smem_table = uint32_t(smem_table);
-        fits = true;
-        break;
-      }
-    }
-    if (!fits) return fail(FGPU_ERR_UNSUPPORTED, "tile aggregate: the projected columns do not fit the shared-memory ring");
-    td.table_bytes = uint32_t(td.smem_table ? tb : 0);
-    uint32_t t = 0;
-    for (uint32_t r : TA.rows) {
-      TA.first_tile.push_back(t);
-      t += (r + td.tile_rows - 1) / td.tile_rows;
-    }
-    TA.first_tile.push_back(t);
-    td.n_tiles = t;
-    td.chunk_tiles = std::max<uint32_t>(1, t / (uint32_t(ctx->sm_count) * 4));  // ~4 turns per CTA: a CTA stays inside one row group for a whole chunk
-    // (the override comes first: the 32-bit Sum bound below depends on the chunk length the launch uses)
-    if (const char* e = getenv("FROSTGPU_TA_CHUNK")) td.chunk_tiles = uint32_t(std::max(1, atoi(e)));
-    td.keys8 = 1;
-    for (uint32_t i = 0; i < td.nk; i++)
-      if (TA.code_wmax[td.key_code[i]] > 8) td.keys8 = 0;
-    {  // can a Sum leave 32 bits inside one CTA?  rows per CTA <= its share of the tiles (+ one chunk), all in one slot
-      const uint64_t grid = uint64_t(std::max(1, ctx->sm_count));
-      const uint64_t rows_per_cta = std::min<uint64_t>(uint64_t(t), uint64_t(t) / grid + 2 * uint64_t(td.chunk_tiles) + 1) * td.tile_rows;
-      // agg_max * rows_per_cta <= 2^32 - 1, without the product (a large chunk override would overflow it)
-      td.sums_fit32 = (TA.agg_bounded && !getenv("FROSTGPU_TA_CARRY") && (TA.agg_max == 0 || rows_per_cta <= 0xffffffffull / TA.agg_max)) ? 1u : 0u;
-    }
-  }
-
-  // ---- filter-only plans over PLAIN columns: ordered take (take_rows.cu) instead of k_rows ------------
-  TakeDesc td{};
-  std::vector<TakeRg> take_rgs;
-  std::vector<uint32_t> take_first_span;
-  bool take_q = q.kind == FGPU_PLAN_FILTER && qd.n_out >= 1 && qd.n_out <= kTakeOut && n_leaves <= kTakeLeaves + kTakePreds &&
-                (qd.n_filter_prog == 0 || qd.filter_kind == FK_AND) && gi > 0 && !getenv("FROSTGPU_NO_TAKE");
-  // range leaves (PLAIN int64 columns) and dictionary leaves (flat codes + result byte per dictionary id) of the plan
-  int take_range[kTakeLeaves] = {0}, take_pred[kTakePreds] = {0}, n_tr = 0, n_tp = 0;
-  for (int l = 0; l < n_leaves && take_q; l++) {
-    const LeafDesc& ld = qd.leaves[l];
-    if (ld.slot == 0xff) { take_q = false; break; }
-    if (qd.slot_type[ld.slot] == ST_DICT) {
-      if (n_tp >= kTakePreds || gi != n_rg) take_q = false;
-      else take_pred[n_tp++] = l;
-    } else if (ld.cmp_float || ld.neg || qd.slot_type[ld.slot] != ST_I64 || c.leaves[size_t(l)].null_literal || n_tr >= kTakeLeaves) {
-      take_q = false;
-    } else {
-      take_range[n_tr++] = l;
-    }
-  }
-  for (int o = 0; o < qd.n_out && take_q; o++)
-    if (qd.slot_type[qd.out_slot[o]] == ST_DICT) take_q = false;
-  for (int g = 0; g < gi && take_q; g++) {
-    TakeRg tr{};
-    tr.n_rows = rg_rows[size_t(g)];
-    bool all = n_leaves > 0;
-    for (int l = 0; l < n_leaves && take_q; l++) {
-      const uint8_t m = lrt[size_t(g) * n_leaves + l].mode;
-      if (m == LM_NONE) take_q = false;  // (only with pruning switched off)
-      if (m != LM_ALL) all = false;
-    }
-    tr.all_pass = all ? 1 : 0;
-    for (int i = 0; i < n_tr && take_q; i++) {
-      const int l = take_range[i];
-      const bool decided = lrt[size_t(g) * n_leaves + l].mode == LM_ALL;
-      tr.lo[i] = decided ? std::numeric_limits<int64_t>::min() : qd.leaves[l].lo_i;
-      tr.hi[i] = decided ? std::numeric_limits<int64_t>::max() : qd.leaves[l].hi_i;
-      tr.leaf_col[i] = nullptr;  // decided (or nothing to evaluate at all): the kernels skip the leaf
-      if (all || decided) continue;
-      const ChunkDesc& d = chunks[size_t(g) * n_slots + qd.leaves[l].slot];
-      if (d.kind != CK_PLAIN64 || d.has_nulls) take_q = false;
-      tr.leaf_col[i] = d.values;
-    }
-    for (int i = 0; i < n_tp && take_q; i++) {
-      const int l = take_pred[i];
-      const LeafRt& rt = lrt[size_t(g) * n_leaves + l];
-      tr.pred_codes[i] = nullptr;
-      if (all || rt.mode == LM_ALL) continue;
-      const ChunkDesc& d = chunks[size_t(g) * n_slots + qd.leaves[l].slot];
-      if (d.kind != CK_DICT_STR) { take_q = false; break; }
-      const std::string& name = c.slot_names[size_t(qd.leaves[l].slot)];
-      int32_t frc = ensure_flat(ctx, c.rgs[size_t(g)].part, name);  // (rows plans: every row group is a general one, g == its index in c.rgs)
-      if (frc) return frc;
-      const ChunkHost& ch = c.rgs[size_t(g)].rg->cols.at(name);
-      if (!ch.flat) { take_q = false; break; }
-      tr.pred_codes[i] = ch.flat;
-      tr.pred_w[i] = ch.flat_w;
-      tr.pred_bias[i] = ch.flat_bias;
-      tr.pred_null[i] = rt.null_result;
-      tr.pred_lut[i] = reinterpret_cast<const uint8_t*>(uintptr_t(c.leaves[size_t(l)].lut_off) + 1);  // offset + 1, rebased below
-    }
-    for (int o = 0; o < qd.n_out && take_q; o++) {
-      const ChunkDesc& d = chunks[size_t(g) * n_slots + qd.out_slot[o]];
-      if (d.kind != CK_PLAIN64 || d.has_nulls) take_q = false;
-      tr.out_col[o] = d.values;
-    }
-    take_rgs.push_back(tr);
-  }
-  if (take_q) {
-    const uint64_t warps = uint64_t(take_resident_warps(ctx->sm_count));
-    uint64_t total = 0;
-    for (const TakeRg& r : take_rgs) total += r.n_rows;
-    uint64_t span_blocks = std::min<uint64_t>(64, std::max<uint64_t>(4, total / (warps * 4 * 256)));
-    td.span_blocks = uint32_t(span_blocks);
-    const uint64_t span_rows = span_blocks * 256;
-    uint32_t spans = 0;
-    for (const TakeRg& r : take_rgs) {
-      take_first_span.push_back(spans);
-      spans += uint32_t((uint64_t(r.n_rows) + span_rows - 1) / span_rows);
-    }
-    take_first_span.push_back(spans);
-    td.n_spans = spans;
-    td.n_rg = uint32_t(take_rgs.size());
-    td.nl = uint32_t(n_tr);
-    td.np = uint32_t(n_tp);
-    td.n_out = uint32_t(qd.n_out);
-  }
+  G.first_tile[size_t(G.n)] = G.tiles;
+  qd.n_rg = G.n;
+  qd.n_tiles = G.tiles;
+  if (int32_t rc = runs_layout(ctx, c, w, R, P, st)) return rc;
+  if (!T.rgs.empty())
+    if (int32_t rc = tile_layout(T, qd, w, ctx->sm_count)) return rc;
+  TakePlan K;
+  bool take_q = rows_plan && take_query(c, qd, w, G.n, &K);
+  for (int g = 0; g < G.n && take_q; g++)
+    if (int32_t rc = take_admit(K, ctx, c, qd, g, G, &take_q)) return rc;
+  if (take_q) take_layout(K, qd, ctx->sm_count);
 
   // ---- device memory -----------------------------------------------------------------------
-  const bool rows_plan = q.kind == FGPU_PLAN_FILTER;
   // small dense tables of a re-executable query: persistent device state owned by the plan (ExecCache)
-  const bool cache_mode = cacheable && !rows_plan && qd.table_mode == TM_DENSE && qd.table_slots <= 65536 && !getenv("FROSTGPU_NO_EXEC_CACHE");
+  const bool cache_mode = cacheable && !rows_plan && qd.table_mode == TM_DENSE && qd.table_slots <= 65536 && !w.no_exec_cache;
   if (cache_mode) c.exec.reset(new ExecCache());
   DevBuf& tbuf = cache_mode ? c.exec->table : res->table;
   DevBuf& abuf = cache_mode ? c.exec->aux : res->aux;
@@ -2492,101 +2748,37 @@ int32_t run_scan(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, fgpu_result* re
     CUDA_TRY(tbuf.alloc(tbytes + 128, ctx->stream));  // (+ counters in cache mode; slack for the 16-byte exchange copies)
     res->table_bytes = tbytes;
     bind_table(&qd, static_cast<uint8_t*>(tbuf.p));
-  }
-  // rows plan: one output array per projected column (worst case every row is selected) + look-back state
-  std::vector<size_t> out_off(size_t(qd.n_out)), valid_off(size_t(qd.n_out));
-  size_t out_bytes = 0, state_off = 0;
-  if (rows_plan) {
-    auto al = [](size_t x) { return (x + 255) & ~size_t(255); };
-    for (int o = 0; o < qd.n_out; o++) {
-      bool dict = qd.slot_type[qd.out_slot[o]] == ST_DICT;
-      out_off[size_t(o)] = out_bytes;
-      out_bytes = al(out_bytes + size_t(c.total_rows) * (dict ? 4 : 8));
-      valid_off[size_t(o)] = out_bytes;
-      if (!dict) out_bytes = al(out_bytes + size_t(c.total_rows));
-    }
-    state_off = out_bytes;
-    out_bytes = al(out_bytes + size_t(tiles) * 8);
-    CUDA_TRY(tbuf.alloc(out_bytes, ctx->stream));
-    uint8_t* ob = static_cast<uint8_t*>(tbuf.p);
-    for (int o = 0; o < qd.n_out; o++) {
-      qd.out_data[o] = ob + out_off[size_t(o)];
-      qd.out_valid[o] = ob + valid_off[size_t(o)];
-    }
-    qd.tile_state = reinterpret_cast<unsigned long long*>(ob + state_off);
+  } else if (int32_t rc = alloc_rows_out(ctx, c.total_rows, G.tiles, tbuf, &qd)) {
+    return rc;
   }
 
-  auto align16 = [](size_t x) { return (x + 15) & ~size_t(15); };
-  size_t o_chunks = 0;
-  size_t o_lrt = align16(o_chunks + chunks.size() * sizeof(ChunkDesc));
-  size_t o_first = align16(o_lrt + lrt.size() * sizeof(LeafRt));
-  size_t o_rows = align16(o_first + first_tile.size() * 4);
-  size_t o_lut = align16(o_rows + rg_rows.size() * 4);
-  size_t o_cnt = align16(o_lut + lutbytes.size());
-  for (RunsBatch& B : batches) {
-    B.o_rg = o_cnt;
-    B.o_span = align16(B.o_rg + B.rgs.size() * sizeof(RunsRg));
-    o_cnt = align16(B.o_span + B.first_span.size() * 4);
-  }
-  if (!PB.rgs.empty()) {
-    PB.o_rg = o_cnt;
-    PB.o_win = align16(PB.o_rg + PB.rgs.size() * sizeof(PrefixRg));
-    o_cnt = align16(PB.o_win + PB.wins.size() * sizeof(PrefixWin));
-  }
-  if (!TA.rgs.empty()) {
-    TA.o_rg = o_cnt;
-    TA.o_tile = align16(TA.o_rg + TA.rgs.size() * sizeof(TileAggRg));
-    o_cnt = align16(TA.o_tile + TA.first_tile.size() * 4);
-  }
-  size_t o_take_rg = 0, o_take_span = 0, o_take_count = 0;
+  // device block: [tables | counters 64 B | group counter 16 B | QueryDesc]
+  HostImage img;
+  const size_t o_chunks = img.add(G.chunks), o_lrt = img.add(G.lrt), o_first = img.add(G.first_tile), o_rows = img.add(G.rg_rows);
+  const size_t o_lut = img.add(G.lutbytes);
+  const size_t o_runs = img.add(R.rgs), o_runs_span = img.add(R.first_span);
+  const size_t o_prefix = img.add(P.rgs), o_win = img.add(P.wins);
+  const size_t o_tile = img.add(T.rgs), o_tile_first = img.add(T.first_tile);
+  size_t o_take = 0, o_take_span = 0, o_take_count = 0;
   if (take_q) {
-    o_take_rg = o_cnt;
-    o_take_span = align16(o_take_rg + take_rgs.size() * sizeof(TakeRg));
-    o_take_count = align16(o_take_span + take_first_span.size() * 4);
-    o_cnt = align16(o_take_count + (size_t(td.n_spans) + 1) * 8);
+    o_take = img.add(K.rgs);
+    o_take_span = img.add(K.first_span);
+    o_take_count = img.add(nullptr, (size_t(K.td.n_spans) + 1) * 8);
   }
-  // device block: [tables | counters 64 B | group counter 16 B | QueryDesc]; the host image of it lives in
-  // page-locked scratch so that one asynchronous copy uploads everything
-  const size_t o_qd = align16(o_cnt + 64 + 16);
-  const size_t aux_bytes = o_qd + sizeof(QueryDesc);
-  const size_t o_ret = align16(aux_bytes);  // scratch only: counters + group count read back
+  const size_t o_cnt = img.add(nullptr, 64 + 16);
+  const size_t o_qd = img.add(&qd, sizeof(QueryDesc));
+  const size_t aux_bytes = img.end;
+  const size_t o_ret = HostImage::align16(aux_bytes);  // scratch only: counters + group count read back
   CUDA_TRY(abuf.alloc(aux_bytes, ctx->stream));
   uint8_t* aux = static_cast<uint8_t*>(abuf.p);
-  for (auto& fx : lut_fix) lrt[fx.first].lut = aux + o_lut + fx.second;
-  CUDA_TRY(ctx->ensure_scratch(o_ret + 128));
-  struct { uint8_t* p; uint8_t* data() { return p; } } hostaux{ctx->scratch};
-  std::memset(hostaux.data(), 0, o_ret + 128);
-  std::memcpy(hostaux.data() + o_chunks, chunks.data(), chunks.size() * sizeof(ChunkDesc));
-  std::memcpy(hostaux.data() + o_lrt, lrt.data(), lrt.size() * sizeof(LeafRt));
-  std::memcpy(hostaux.data() + o_first, first_tile.data(), first_tile.size() * 4);
-  std::memcpy(hostaux.data() + o_rows, rg_rows.data(), rg_rows.size() * 4);
-  if (!lutbytes.empty()) std::memcpy(hostaux.data() + o_lut, lutbytes.data(), lutbytes.size());
-  for (RunsBatch& B : batches) {
-    if (B.rgs.empty()) continue;
-    for (RunsRg& r : B.rgs)
-      for (int i = 0; i < runs_np; i++)
-        if (r.pred_runs[i]) r.pred_lut[i] = aux + o_lut + size_t(uintptr_t(r.pred_lut[i]));
-    std::memcpy(hostaux.data() + B.o_rg, B.rgs.data(), B.rgs.size() * sizeof(RunsRg));
-    std::memcpy(hostaux.data() + B.o_span, B.first_span.data(), B.first_span.size() * 4);
-  }
-  if (!PB.rgs.empty()) {
-    std::memcpy(hostaux.data() + PB.o_rg, PB.rgs.data(), PB.rgs.size() * sizeof(PrefixRg));
-    std::memcpy(hostaux.data() + PB.o_win, PB.wins.data(), PB.wins.size() * sizeof(PrefixWin));
-  }
-  if (!TA.rgs.empty()) {
-    for (TileAggRg& r : TA.rgs)
-      for (int i = 0; i < kTaPreds; i++)
-        if (r.pred_lut[i]) r.pred_lut[i] = aux + o_lut + (size_t(uintptr_t(r.pred_lut[i])) - 1);
-    std::memcpy(hostaux.data() + TA.o_rg, TA.rgs.data(), TA.rgs.size() * sizeof(TileAggRg));
-    std::memcpy(hostaux.data() + TA.o_tile, TA.first_tile.data(), TA.first_tile.size() * 4);
-  }
-  if (take_q) {
-    for (TakeRg& r : take_rgs)
-      for (int i = 0; i < kTakePreds; i++)
-        if (r.pred_lut[i]) r.pred_lut[i] = aux + o_lut + (size_t(uintptr_t(r.pred_lut[i])) - 1);
-    std::memcpy(hostaux.data() + o_take_rg, take_rgs.data(), take_rgs.size() * sizeof(TakeRg));
-    std::memcpy(hostaux.data() + o_take_span, take_first_span.data(), take_first_span.size() * 4);
-  }
+  const uint8_t* lut = aux + o_lut;
+  for (auto& fx : G.lut_fix) G.lrt[fx.first].lut = lut + fx.second;
+  for (RunsRg& r : R.rgs)
+    for (const uint8_t*& p : r.pred_lut) lut_rebase(p, lut);
+  for (TileAggRg& r : T.rgs)
+    for (const uint8_t*& p : r.pred_lut) lut_rebase(p, lut);
+  for (TakeRg& r : K.rgs)
+    for (const uint8_t*& p : r.pred_lut) lut_rebase(p, lut);
   qd.chunks = reinterpret_cast<const ChunkDesc*>(aux + o_chunks);
   qd.leaf_rt = reinterpret_cast<const LeafRt*>(aux + o_lrt);
   qd.rg_first_tile = reinterpret_cast<const uint32_t*>(aux + o_first);
@@ -2594,6 +2786,9 @@ int32_t run_scan(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, fgpu_result* re
   qd.counters = cache_mode ? reinterpret_cast<unsigned long long*>(static_cast<uint8_t*>(tbuf.p) + tbytes)  // behind the table: one copy brings both back
                            : reinterpret_cast<unsigned long long*>(aux + o_cnt);
   const QueryDesc* qdesc_dev = reinterpret_cast<const QueryDesc*>(aux + o_qd);
+  CUDA_TRY(ctx->ensure_scratch(o_ret + 128));
+  std::memset(ctx->scratch, 0, o_ret + 128);
+  img.copy_to(ctx->scratch);
 
   FinalizeDesc& fd = res->fd;
   fd = FinalizeDesc{};
@@ -2604,22 +2799,20 @@ int32_t run_scan(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, fgpu_result* re
   fd.table_slots = qd.table_slots;
   for (int k = 0; k < qd.n_keys; k++) {
     fd.keys[k] = qd.keys[k];
-    fd.dense_radix[k] = c.dense_radix[size_t(k)] ? c.dense_radix[size_t(k)] : 1;
+    fd.dense_radix[k] = c.radix(k);
   }
-  fd.t_rows = qd.t_rows;
-  for (int a = 0; a < kMaxAggs; a++) fd.t_agg[a] = qd.t_agg[a];
-  fd.t_tag = qd.t_tag;
-  fd.t_keys = qd.t_keys;
+  bind_finalize(&fd, qd);
   cudaStream_t s = ctx->stream;
   pc.mark("describe");
   CUDA_TRY(cudaEventRecord(ctx->ev[0], s));
-  std::memcpy(hostaux.data() + o_qd, &qd, sizeof(QueryDesc));
-  CUDA_TRY(cudaMemcpyAsync(aux, hostaux.data(), aux_bytes, cudaMemcpyHostToDevice, s));
+  CUDA_TRY(cudaMemcpyAsync(aux, ctx->scratch, aux_bytes, cudaMemcpyHostToDevice, s));
+  ScanLaunch L;
   if (rows_plan) {
-    CUDA_TRY(cudaMemsetAsync(qd.tile_state, 0, size_t(tiles) * 8, s));
+    CUDA_TRY(cudaMemsetAsync(qd.tile_state, 0, size_t(G.tiles) * 8, s));
     CUDA_TRY(cudaEventRecord(ctx->ev[1], s));
     if (take_q) {
-      td.rgs = reinterpret_cast<const TakeRg*>(aux + o_take_rg);
+      TakeDesc& td = K.td;
+      td.rgs = reinterpret_cast<const TakeRg*>(aux + o_take);
       td.rg_first_span = reinterpret_cast<const uint32_t*>(aux + o_take_span);
       td.span_count = reinterpret_cast<unsigned long long*>(aux + o_take_count);
       td.total = qd.counters;
@@ -2630,184 +2823,64 @@ int32_t run_scan(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, fgpu_result* re
     } else {
       CUDA_TRY(launch_rows(qdesc_dev, qd, ctx->sm_count, s));
     }
+    CUDA_TRY(cudaEventRecord(ctx->ev[2], s));
   } else {
-    CUDA_TRY(launch_table_init(qd, s));
-    CUDA_TRY(cudaEventRecord(ctx->ev[1], s));
-    for (RunsBatch& B : batches) {
-      if (B.rgs.empty()) continue;
-      RunsDesc& rd = B.rd;
-      rd.rgs = reinterpret_cast<const RunsRg*>(aux + B.o_rg);
-      rd.rg_first_span = reinterpret_cast<const uint32_t*>(aux + B.o_span);
-      rd.t_rows = qd.t_rows;
-      for (int a = 0; a < runs_na; a++) rd.t_agg[a] = qd.t_agg[runs_agg_index[a]];
-      rd.counters = qd.counters;
-      CUDA_TRY(launch_runs_tma(rd, B.nl, runs_nk, runs_na, ctx->sm_count, s));
-      st.kernel_launches++;
-      st.row_groups_runs += uint32_t(B.rgs.size());
-    }
-    if (!PB.rgs.empty()) {
-      PrefixDesc& pd = PB.pd;
-      pd.n_win = uint32_t(PB.wins.size());
-      pd.nk = uint32_t(runs_nk);
-      pd.na = uint32_t(runs_na);
-      for (int k = 0; k < runs_nk; k++) pd.stride[k] = qd.keys[k].dense_stride;
-      pd.rgs = reinterpret_cast<const PrefixRg*>(aux + PB.o_rg);
-      pd.wins = reinterpret_cast<const PrefixWin*>(aux + PB.o_win);
-      pd.t_rows = qd.t_rows;
-      for (int a = 0; a < runs_na; a++) pd.t_agg[a] = qd.t_agg[runs_agg_index[a]];
-      pd.counters = qd.counters;
-      CUDA_TRY(launch_runs_prefix(pd, ctx->sm_count, s));
-      st.kernel_launches++;
-      st.row_groups_runs += uint32_t(PB.rgs.size());
-      st.row_groups_prefix += uint32_t(PB.rgs.size());
-    }
-    if (!TA.rgs.empty()) {
-      TileAggDesc& td = TA.td;
-      td.rgs = reinterpret_cast<const TileAggRg*>(aux + TA.o_rg);
-      td.rg_first_tile = reinterpret_cast<const uint32_t*>(aux + TA.o_tile);
-      td.t_rows = qd.t_rows;
-      for (uint32_t a = 0; a < td.na; a++) td.t_agg[a] = qd.t_agg[TA.agg_index[a]];
-      td.counters = qd.counters;
-      CUDA_TRY(launch_tile_agg(td, ctx->sm_count, s));
-      st.kernel_launches++;
-      st.row_groups_tiles += uint32_t(TA.rgs.size());
-    }
-    CUDA_TRY(launch_scan(qdesc_dev, qd, ctx->sm_count, s));
+    L.runs = !R.rgs.empty();
+    L.rd = R.rd;
+    L.rd.rgs = reinterpret_cast<const RunsRg*>(aux + o_runs);
+    L.rd.rg_first_span = reinterpret_cast<const uint32_t*>(aux + o_runs_span);
+    L.rd.t_rows = qd.t_rows;
+    for (int a = 0; a < R.na; a++) L.rd.t_agg[a] = qd.t_agg[R.agg_index[a]];
+    L.rd.counters = qd.counters;
+    L.runs_nl = R.nl;
+    L.runs_nk = R.nk;
+    L.runs_na = R.na;
+    L.prefix = !P.rgs.empty();
+    L.pd = P.pd;
+    L.pd.rgs = reinterpret_cast<const PrefixRg*>(aux + o_prefix);
+    L.pd.wins = reinterpret_cast<const PrefixWin*>(aux + o_win);
+    L.pd.t_rows = qd.t_rows;
+    for (int a = 0; a < R.na; a++) L.pd.t_agg[a] = qd.t_agg[R.agg_index[a]];
+    L.pd.counters = qd.counters;
+    L.tile = !T.rgs.empty();
+    L.td = T.td;
+    L.td.rgs = reinterpret_cast<const TileAggRg*>(aux + o_tile);
+    L.td.rg_first_tile = reinterpret_cast<const uint32_t*>(aux + o_tile_first);
+    L.td.t_rows = qd.t_rows;
+    for (uint32_t a = 0; a < T.td.na; a++) L.td.t_agg[a] = qd.t_agg[T.agg_index[a]];
+    L.td.counters = qd.counters;
+    if (int32_t rc = launch_aggregate_scan(ctx, qd, qdesc_dev, L)) return rc;
+    st.kernel_launches += uint32_t(L.runs) + uint32_t(L.prefix) + uint32_t(L.tile);
+    st.row_groups_runs += uint32_t(R.rgs.size() + P.rgs.size());
+    st.row_groups_prefix += uint32_t(P.rgs.size());
+    st.row_groups_tiles += uint32_t(T.rgs.size());
   }
-  CUDA_TRY(cudaEventRecord(ctx->ev[2], s));
-  st.kernel_launches += (rows_plan ? 0 : 1) + (tiles ? 1 : 0);
+  st.kernel_launches += (rows_plan ? 0 : 1) + (G.tiles ? 1 : 0);
   st.h2d_bytes += aux_bytes + sizeof(QueryDesc);
-  unsigned long long* counters = reinterpret_cast<unsigned long long*>(hostaux.data() + o_ret);
+  unsigned long long* counters = reinterpret_cast<unsigned long long*>(ctx->scratch + o_ret);
   res->cnt_ptr = reinterpret_cast<unsigned int*>(qd.counters + 8);  // 16 bytes behind the counters, zeroed by the upload / the table init
   if (collective) {
     if (rows_plan) return fail(FGPU_ERR_INVALID, "rows plans have no partial table: execute them per rank");
-    int32_t rcx = comm_push(ctx, tbuf.p, tbytes, &res->pending_seq, &res->pending_bytes);
-    if (rcx) return rcx;
+    if (int32_t rc = comm_push(ctx, tbuf.p, tbytes, &res->pending_seq, &res->pending_bytes)) return rc;
     res->pending = true;
     res->plan_keep = q.plan_cache;
     count_groups = false;  // the table is not final yet
   }
   if (cache_mode) {
-    // ---- the plan keeps this device state; the table comes back with one copy and is compacted on the host ----
     ExecCache& x = *c.exec;
     x.table_bytes = tbytes;
-    x.ctx = ctx;
-    {
-      DenseOut& f = x.dout;
-      f.table_slots = qd.table_slots;
-      f.max_out = qd.table_slots;
-      f.n_keys = uint32_t(qd.n_keys);
-      f.n_aggs = uint32_t(qd.n_aggs);
-      for (int k = 0; k < qd.n_keys; k++) {
-        f.stride[k] = qd.keys[k].dense_stride;
-        f.radix[k] = c.dense_radix[size_t(k)] ? c.dense_radix[size_t(k)] : 1;
-      }
-      f.t_rows = qd.t_rows;
-      for (int a = 0; a < kMaxAggs; a++) f.t_agg[a] = qd.t_agg[a];
-      f.counters = qd.counters;
-      {  // what the collective tail needs to fold partial tables itself (layout of table_layout())
-        int pos = 0;
-        for (int a = 0; a < qd.n_aggs; a++) {
-          f.agg_func[a] = qd.aggs[a].func;
-          f.agg_is_float[a] = qd.aggs[a].is_float;
-          f.agg_pos[a] = qd.aggs[a].func == FGPU_AGG_COUNT ? int8_t(-1) : int8_t(pos++);
-        }
-      }
-      x.out_bytes = 256 + size_t(qd.n_keys) * ((size_t(f.max_out) * 4 + 7) & ~size_t(7)) + size_t(qd.n_aggs) * f.max_out * 8;
-      CUDA_TRY(x.out.alloc(256, s));  // working header (k_finalize_dense leaves it zero)
-      CUDA_TRY(cudaMemsetAsync(x.out.p, 0, 256, s));
-      f.hdr = static_cast<uint32_t*>(x.out.p);
-      f.out = nullptr;  // a page-locked block per Execute (cached_tail)
-    }
-    x.pool = ctx->pinned;
-    x.pinned = ctx->pinned_take(x.out_bytes, &x.pinned_cap);
-    if (!x.pinned) return fail(FGPU_ERR_OOM, "page-locked memory for the result image");
-    if (!res->pending) {
-      if (int32_t rct = cached_tail(ctx, x)) return rct;
-    } else {
-      CUDA_TRY(cudaMemcpyAsync(x.pinned + 32, qd.counters, 32, cudaMemcpyDeviceToHost, s));  // (rows selected by this rank's scan)
-    }
-    CUDA_TRY(cudaEventRecord(ctx->ev[3], s));
-    pc.mark("launch");
-    CUDA_TRY(cudaStreamSynchronize(s));  // hostaux stays valid until here
-    pc.mark("sync");
-    release_staging(ctx);
-    st.h2d_bytes += c.h2d_bytes;
-    float ms = 0;
-    CUDA_TRY(cudaEventElapsedTime(&ms, ctx->ev[1], ctx->ev[2]));
-    st.scan_kernel_ms = ms;
-    CUDA_TRY(cudaEventElapsedTime(&ms, ctx->ev[0], ctx->ev[3]));
-    st.total_device_ms = ms;
-    const unsigned long long* cnts = reinterpret_cast<const unsigned long long*>(x.pinned + 32);
-    st.rows_selected = cnts[0];
-    x.qd = qd;
     x.qdesc_dev = qdesc_dev;
-    x.has_runs = !batches[0].rgs.empty();
-    x.rd = batches[0].rd;
-    x.runs_nl = batches[0].nl;
-    x.runs_nk = runs_nk;
-    x.runs_na = runs_na;
-    x.has_prefix = !PB.rgs.empty();
-    x.pd = PB.pd;
-    x.has_ta = !TA.rgs.empty();
-    x.td = TA.td;
-    x.keys = c.keys;
-    for (KeyOut& k : x.keys) {
-      if (k.dict) {
-        const uint32_t card = k.dict->cardinality();
-        k.dict_snapshot.reserve(card);
-        for (uint32_t i = 0; i < card; i++) k.dict_snapshot.push_back(k.dict->value(i));
-        k.dict = nullptr;
-      }
-    }
-    x.dense_radix = c.dense_radix;
-    for (const KeyOut& k : x.keys) {  // small dictionaries are exported whole: the host then only copies index columns
-      std::unique_ptr<OwnedColumn> d;
-      if (k.dict_snapshot.size() <= 4096) {
-        d = std::make_unique<OwnedColumn>();
-        d->format = "z";
-        d->length = int64_t(k.dict_snapshot.size());
-        d->offsets.push_back(0);
-        for (const std::string& v : k.dict_snapshot) {
-          d->data.insert(d->data.end(), v.begin(), v.end());
-          d->offsets.push_back(int32_t(d->data.size()));
-        }
-      }
-      x.dict_template.push_back(std::move(d));
-    }
-    for (size_t a = 0; a < q.aggs.size(); a++) {
-      x.agg_names.push_back(std::string(agg_string(q.aggs[a].func)) + "(" + q.expr_name(q.aggs[a].expr) + ")");
-      x.agg_is_float.push_back(qd.aggs[a].func != FGPU_AGG_COUNT && qd.aggs[a].is_float);
-    }
-    st.kernel_launches++;  // k_finalize_dense (cached_tail)
-    x.stats = st;  // what a cached Execute reports: no uploads, no compile
-    x.stats.h2d_bytes = 0;
-    x.stats.d2h_bytes = 0;
-    x.stats.rows_selected = 0;
-    x.ready = true;
-    st.d2h_bytes += x.out_bytes;
-    res->qd = qd;
-    pc.mark("keep");
-    pc.flush("scan");
-    if (res->pending) {
-      res->pending_cached = &x;
-      return FGPU_OK;
-    }
-    return finalize_dense_host(ctx, res, x);
+    x.launch = L;
+    return keep_exec_cache(ctx, q, c, qd, res, pc);
   }
   if (count_groups && !rows_plan) {  // count the result rows behind the scan: one host round trip less
-    fd.out_count = res->cnt_ptr;
-    fd.max_out = 0;
-    fd.out_keys = nullptr;
-    fd.out_aggs = nullptr;
-    fd.out_rows = nullptr;
-    CUDA_TRY(launch_finalize(fd, s));
+    CUDA_TRY(launch_count_groups(fd, res->cnt_ptr, s));
     st.kernel_launches++;
     res->groups_known = true;
   }
   CUDA_TRY(cudaMemcpyAsync(counters, qd.counters, 64 + 16, cudaMemcpyDeviceToHost, s));
   pc.mark("launch");
-  CUDA_TRY(cudaStreamSynchronize(s));  // hostaux / counters stay valid until here
+  CUDA_TRY(cudaStreamSynchronize(s));  // the host image / counters stay valid until here
   pc.mark("sync");
   release_staging(ctx);
   st.h2d_bytes += c.h2d_bytes;
@@ -2818,25 +2891,12 @@ int32_t run_scan(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, fgpu_result* re
   if (res->groups_known) res->n_groups = static_cast<unsigned int>(counters[8] & 0xffffffffull);
   st.d2h_bytes += 64;
   if (counters[1]) return fail(FGPU_ERR_UNSUPPORTED, "aggregate hash table overflow (more groups than the sized capacity)");
-  if (int32_t rcc = comm_check(counters[3])) return rcc;
+  if (int32_t rc = comm_check(counters[3])) return rc;
 
   // keep what finalize / merge need
   res->qd = qd;
-  res->keys = c.keys;  // (the plan may be reused by the next Execute)
-  for (KeyOut& k : res->keys) {
-    if (k.dict) {
-      uint32_t card = k.dict->cardinality();
-      k.dict_snapshot.reserve(card);
-      for (uint32_t i = 0; i < card; i++) k.dict_snapshot.push_back(k.dict->value(i));
-      k.dict = nullptr;
-    }
-  }
   res->rows_plan = rows_plan;
-  for (size_t a = 0; a < q.aggs.size(); a++) {
-    res->agg_names.push_back(std::string(agg_string(q.aggs[a].func)) + "(" + q.expr_name(q.aggs[a].expr) + ")");
-    // Count yields int64; Sum/Min/Max keep the input type (aggregate.go:734-950)
-    res->agg_is_float.push_back(qd.aggs[a].func != FGPU_AGG_COUNT && qd.aggs[a].is_float);
-  }
+  result_shape(q, c, &res->keys, &res->agg_names, &res->agg_is_float);
   pc.mark("keep");
   pc.flush("scan");
   return FGPU_OK;
@@ -2886,8 +2946,9 @@ int32_t finalize_dense_host(fgpu_ctx* ctx, fgpu_result* res, ExecCache& x) {
         }
       }
     }
-    auto dict = std::make_unique<OwnedColumn>();
+    std::unique_ptr<OwnedColumn> dict;
     if (const OwnedColumn* t = x.dict_template[size_t(k)].get()) {
+      dict = std::make_unique<OwnedColumn>();
       dict->format = t->format;
       dict->length = t->length;
       dict->data = t->data;
@@ -2905,14 +2966,7 @@ int32_t finalize_dense_host(fgpu_ctx* ctx, fgpu_result* res, ExecCache& x) {
         }
       for (size_t i = 0; i < G; i++)
         if (is_valid(i)) idx[i] = remap[idx[i]];
-      dict->format = "z";
-      dict->length = int64_t(used.size());
-      dict->offsets.push_back(0);
-      for (uint32_t gid : used) {
-        const std::string& v = ko.dict_snapshot[gid];
-        dict->data.insert(dict->data.end(), v.begin(), v.end());
-        dict->offsets.push_back(int32_t(dict->data.size()));
-      }
+      dict = dict_column(ko.dict_snapshot, &used);
     }
     col.dictionary = std::move(dict);
     cols.push_back(std::move(col));
@@ -2996,24 +3050,18 @@ int32_t finalize_rows(fgpu_ctx* ctx, fgpu_result* res) {
         if (ids[i] >= 0) remap[size_t(ids[i])] = 0;
         else any_null = true;
       }
-      auto dict = std::make_unique<OwnedColumn>();
-      dict->format = "z";
-      dict->offsets.push_back(0);
-      int32_t next = 0;
-      for (size_t g = 0; g < remap.size(); g++) {
-        if (remap[g] < 0) continue;
-        remap[g] = next++;
-        const std::string& v = ko.dict_snapshot[g];
-        dict->data.insert(dict->data.end(), v.begin(), v.end());
-        dict->offsets.push_back(int32_t(dict->data.size()));
-      }
-      dict->length = next;
+      std::vector<uint32_t> used;
+      for (size_t g = 0; g < remap.size(); g++)
+        if (remap[g] >= 0) {
+          remap[g] = int32_t(used.size());
+          used.push_back(uint32_t(g));
+        }
       if (any_null) col.validity.assign((R + 7) / 8, 0);
       for (size_t i = 0; i < R; i++) {
         if (ids[i] < 0) { idx[i] = 0; col.null_count++; }
         else { idx[i] = uint32_t(remap[size_t(ids[i])]); if (any_null) set_bit(col.validity, int64_t(i)); }
       }
-      col.dictionary = std::move(dict);
+      col.dictionary = dict_column(ko.dict_snapshot, &used);
     } else {
       col.format = ko.is_float ? "g" : "l";
       if (valid[size_t(o)].p) {
@@ -3055,12 +3103,7 @@ int32_t finalize_result(fgpu_ctx* ctx, fgpu_result* res) {
     CUDA_TRY(cnt.alloc(16, ctx->stream));
     CUDA_TRY(cudaMemsetAsync(cnt.p, 0, 16, s));
     res->cnt_ptr = static_cast<unsigned int*>(cnt.p);
-    fd.out_count = static_cast<unsigned int*>(cnt.p);
-    fd.max_out = 0;
-    fd.out_keys = nullptr;
-    fd.out_aggs = nullptr;
-    fd.out_rows = nullptr;
-    CUDA_TRY(launch_finalize(fd, s));
+    CUDA_TRY(launch_count_groups(fd, res->cnt_ptr, s));
     CUDA_TRY(cudaMemcpyAsync(&n_groups, cnt.p, 4, cudaMemcpyDeviceToHost, s));
     CUDA_TRY(cudaStreamSynchronize(s));
     res->stats.kernel_launches += 1;
@@ -3140,16 +3183,7 @@ int32_t finalize_result(fgpu_ctx* ctx, fgpu_result* res) {
         }
       }
       if (col.null_count == 0) col.validity.clear();
-      auto dict = std::make_unique<OwnedColumn>();
-      dict->format = "z";
-      dict->length = int64_t(used.size());
-      dict->offsets.push_back(0);
-      for (uint32_t gid : used) {
-        const std::string& v = ko.dict_snapshot[gid];
-        dict->data.insert(dict->data.end(), v.begin(), v.end());
-        dict->offsets.push_back(int32_t(dict->data.size()));
-      }
-      col.dictionary = std::move(dict);
+      col.dictionary = dict_column(ko.dict_snapshot, &used);
       if (G) pool->give(blocks[size_t(k)].p, blocks[size_t(k)].cap);  // the codes are re-indexed into col.data
     }
     cols.push_back(std::move(col));
@@ -3186,13 +3220,7 @@ int32_t collective_end(fgpu_ctx* ctx, fgpu_result* res) {
   res->pending = false;
   cudaStream_t s = ctx->stream;
   if (ExecCache* x = static_cast<ExecCache*>(res->pending_cached)) {
-    if (x->qd.table_mode == TM_DENSE) {
-      if (int32_t rcm = cached_tail_merged(ctx, *x, res->pending_seq, res->pending_bytes)) return rcm;
-    } else {
-      int32_t rc = comm_wait_merge(ctx, x->qd, x->table.p, res->pending_seq, res->pending_bytes);
-      if (rc) return rc;
-      if (int32_t rct = cached_tail(ctx, *x)) return rct;
-    }
+    if (int32_t rc = cached_merge_tail(ctx, *x, res->pending_seq, res->pending_bytes)) return rc;
     CUDA_TRY(cudaStreamSynchronize(s));
     const unsigned long long* counters = reinterpret_cast<const unsigned long long*>(x->pinned + 32);
     res->stats.d2h_bytes += x->out_bytes;
@@ -3213,19 +3241,11 @@ int32_t collective_end(fgpu_ctx* ctx, fgpu_result* res) {
     std::swap(res->table.p, merged.p);
     std::swap(res->table.n, merged.n);
     qd = q2;
-    fd.t_rows = qd.t_rows;
-    for (int a = 0; a < kMaxAggs; a++) fd.t_agg[a] = qd.t_agg[a];
-    fd.t_tag = qd.t_tag;
-    fd.t_keys = qd.t_keys;
+    bind_finalize(&fd, qd);
   }
   if (res->cnt_ptr) {  // count the groups of the final table behind the merge
     CUDA_TRY(cudaMemsetAsync(res->cnt_ptr, 0, 16, s));
-    fd.out_count = res->cnt_ptr;
-    fd.max_out = 0;
-    fd.out_keys = nullptr;
-    fd.out_aggs = nullptr;
-    fd.out_rows = nullptr;
-    CUDA_TRY(launch_finalize(fd, s));
+    CUDA_TRY(launch_count_groups(fd, res->cnt_ptr, s));
     res->stats.kernel_launches++;
   }
   CUDA_TRY(ctx->ensure_scratch(128));
@@ -3597,18 +3617,10 @@ int32_t fgpu_result_merge_partials(fgpu_ctx* ctx, fgpu_result* r, const void* ga
     // the result now lives in the merged table; its groups are counted right behind the merges so that
     // finalisation needs one host round trip less
     FinalizeDesc& fd = r->fd;
-    fd.t_rows = qd.t_rows;
-    for (int a = 0; a < kMaxAggs; a++) fd.t_agg[a] = qd.t_agg[a];
-    fd.t_tag = qd.t_tag;
-    fd.t_keys = qd.t_keys;
+    bind_finalize(&fd, qd);
     if (r->cnt_ptr) {
       CUDA_TRY(cudaMemsetAsync(r->cnt_ptr, 0, 16, ctx->stream));
-      fd.out_count = r->cnt_ptr;
-      fd.max_out = 0;
-      fd.out_keys = nullptr;
-      fd.out_aggs = nullptr;
-      fd.out_rows = nullptr;
-      CUDA_TRY(launch_finalize(fd, ctx->stream));
+      CUDA_TRY(launch_count_groups(fd, r->cnt_ptr, ctx->stream));
       r->stats.kernel_launches++;
     }
     CUDA_TRY(ctx->ensure_scratch(128));
