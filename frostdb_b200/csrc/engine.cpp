@@ -806,6 +806,22 @@ void canonical_int_range(int op, int64_t v, int64_t* lo, int64_t* hi, bool* neg)
   }
 }
 
+// "column op literal" compared as float64, as an inclusive range, optionally negated (see LeafDesc).  A NaN literal
+// gives the empty range: x != NaN holds for every non-NULL x, every other comparison with NaN for none.
+void canonical_float_range(int op, double v, double* lo, double* hi, bool* neg) {
+  const double kInf = std::numeric_limits<double>::infinity();
+  *lo = kInf; *hi = -kInf;  // empty
+  *neg = op == FGPU_OP_NOT_EQ;
+  if (std::isnan(v)) return;
+  switch (op) {
+    case FGPU_OP_EQ: case FGPU_OP_NOT_EQ: *lo = *hi = v; break;
+    case FGPU_OP_LT: if (v != -kInf) { *lo = -kInf; *hi = std::nextafter(v, -kInf); } break;
+    case FGPU_OP_LT_EQ: *lo = -kInf; *hi = v; break;
+    case FGPU_OP_GT: if (v != kInf) { *lo = std::nextafter(v, kInf); *hi = kInf; } break;
+    default: *lo = v; *hi = kInf; break;
+  }
+}
+
 // What the chunk statistics [mn, mx] (bounds of the non-null values) decide about an int64 range leaf for a
 // whole row group: LM_NONE no row can pass, LM_ALL every row passes (needs a chunk without NULLs), LM_EVAL
 // undecided.  The row-group filter of the reference (expr/binaryscalarexpr.go:84-190) answers the first question.
@@ -816,7 +832,7 @@ uint8_t stats_leaf_mode(int64_t lo, int64_t hi, bool neg, int64_t mn, int64_t mx
   return inside ? LM_NONE : ((disjoint && no_nulls) ? LM_ALL : LM_EVAL);
 }
 
-// The decision compile() takes for an int64 range leaf on one chunk, also behind the host-only test hook
+// The decision leaf_mode() takes for an int64 range leaf on one chunk, also behind the host-only test hook
 // fgpu_rowgroup_leaf_mode: an all-NULL chunk has no usable bounds (nothing is decided from statistics).
 uint8_t chunk_leaf_mode(int64_t lo, int64_t hi, bool neg, bool has_bounds, int64_t mn, int64_t mx, int64_t null_count, int64_t num_values) {
   if (!has_bounds || (null_count >= 0 && null_count == num_values)) return LM_EVAL;
@@ -880,7 +896,7 @@ struct Compiled {
   uint32_t radix(int k) const { return dense_radix[size_t(k)] ? dense_radix[size_t(k)] : 1; }  // (int64 keys have none)
 };
 
-int32_t compile_filter(const QueryPlan& q, int node, Compiled* c, std::map<std::string, int>& slot_of) {
+int32_t compile_filter(const QueryPlan& q, int node, Compiled* c, const std::map<std::string, int>& slot_of) {
   const ExprNode& e = q.exprs[size_t(node)];
   if (e.kind != FGPU_EXPR_BINARY) return fail(FGPU_ERR_UNSUPPORTED, "unsupported boolean expression");
   if (e.op == FGPU_OP_AND || e.op == FGPU_OP_OR) {
@@ -917,7 +933,7 @@ int32_t compile_filter(const QueryPlan& q, int node, Compiled* c, std::map<std::
   return FGPU_OK;
 }
 
-int32_t compile_agg_expr(const QueryPlan& q, int node, std::map<std::string, int>& slot_of, const Compiled& c,
+int32_t compile_agg_expr(const QueryPlan& q, int node, const std::map<std::string, int>& slot_of, const Compiled& c,
                          std::vector<ProgOp>* prog, bool* any_float, bool* any_int_col) {
   const ExprNode& e = q.exprs[size_t(node)];
   if (e.kind == FGPU_EXPR_COLUMN) {
@@ -1063,26 +1079,35 @@ bool rg_may_match(const QueryPlan& q, int node, const RowGroupHost& rg) {
   }
 }
 
-// Resolves the plan against the visible row groups and fills everything of QueryDesc that does
-// not need device memory.
-int32_t compile(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, const Switches& w, Compiled* c) {
-  Table& table = ctx->tables[q.table];  // a table without parts scans nothing (empty LSM)
-  for (auto& p : table.parts) {
-    if (p->tx > tx) continue;  // index/lsm.go:416
-    for (auto& rg : p->rgs) {
-      c->rgs.push_back({p.get(), &rg});
-      c->total_rows += rg.n_rows;
+// The plan's columns resolved against the visible row groups.
+struct Columns {
+  std::map<std::string, int> slot_of;
+  std::vector<std::string> key_names;       // group-by / distinct / projected columns and computed keys, in plan order
+  std::map<std::string, int32_t> key_expr;  // computed keys: name -> expression node
+
+  // 1 for the slot of each column whose values the plan reads: keys, computed-key and aggregate inputs and,
+  // with_filter, the filter's.  Count(col) counts rows, NULLs included (aggregate.go:929-950): its input column is
+  // never read, so it is neither uploaded nor staged unless something else in the query needs it.
+  std::vector<uint8_t> value_slots(const QueryPlan& q, bool with_filter) const {
+    std::vector<std::string> need = key_names;
+    for (auto& kv : key_expr) collect_columns(q, kv.second, &need);
+    if (with_filter) collect_columns(q, q.filter, &need);
+    for (const fgpu_agg& a : q.aggs)
+      if (a.func != FGPU_AGG_COUNT) collect_columns(q, a.expr, &need);
+    std::vector<uint8_t> out(slot_of.size(), 0);
+    for (auto& n : need) {
+      auto it = slot_of.find(n);
+      if (it != slot_of.end()) out[size_t(it->second)] = 1;
     }
+    return out;
   }
-  if (c->rgs.empty()) {  // nothing to scan: no records, exactly like an Iterator over an empty LSM
-    c->qd.table_mode = TM_DENSE;
-    c->qd.key_words = 1;
-    c->qd.table_slots = 1;
-    c->qd.tile_rows = ctx->tile_rows;
-    return FGPU_OK;
-  }
-  // every column name present in a visible row group, in name order, with its type
-  std::map<std::string, uint8_t> present;
+};
+
+// Column types, group keys (a computed key, arithmetic over int64 columns like the sqlparse pre-projection
+// `(timestamp / 1000) * 1000 as bucket`, is named after its expression and carries the expression's node) and one
+// slot per column the keys, the filter, the aggregates and the computed keys name.
+int32_t resolve_columns(const QueryPlan& q, const Table& table, Compiled* c, Columns* k) {
+  std::map<std::string, uint8_t> present;  // every column name present in a visible row group, with its type (0xff: unreadable)
   for (const VisibleRG& v : c->rgs) {
     for (auto& kv : v.rg->cols) {
       uint8_t t = kv.second.phys == PT_BYTE_ARRAY ? ST_DICT : (kv.second.phys == PT_DOUBLE ? ST_F64 : ST_I64);
@@ -1097,80 +1122,126 @@ int32_t compile(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, const Switches& 
   // aggregate table, must not depend on which parts a rank happens to own
   for (auto& kv : table.dicts)
     if (kv.second.preloaded && !present.count(kv.first)) present.emplace(kv.first, uint8_t(ST_DICT));
-  std::map<std::string, int> slot_of;
-  auto want = [&](const std::string& name) -> int32_t {
-    if (slot_of.count(name)) return FGPU_OK;
-    auto it = present.find(name);
-    if (it == present.end()) return FGPU_OK;  // absent everywhere: handled by the callers
-    if (it->second == 0xff) return fail(FGPU_ERR_UNSUPPORTED, "column " + name + " has a type the GPU engine does not read");
-    if (c->slot_names.size() >= size_t(kMaxSlots)) return fail(FGPU_ERR_UNSUPPORTED, "query touches too many columns");
-    slot_of[name] = int(c->slot_names.size());
-    c->slot_names.push_back(name);
-    c->slot_types.push_back(it->second);
-    return FGPU_OK;
+  std::vector<std::string>& key_names = k->key_names;
+  auto add_key_name = [&](const std::string& name) {  // first occurrence only
+    if (std::find(key_names.begin(), key_names.end(), name) == key_names.end()) key_names.push_back(name);
   };
-  // group-by / distinct columns; a computed key (arithmetic over int64 columns, the sqlparse pre-projection
-  // `(timestamp / 1000) * 1000 as bucket`) is named after its expression and carries the expression's node
-  std::vector<std::string> key_names;
-  std::map<std::string, int32_t> key_expr;  // computed keys: name -> expression node
   for (int32_t g : q.group_by) {
     const ExprNode& e = q.exprs[size_t(g)];
     if (e.kind == FGPU_EXPR_COLUMN) {
-      if (present.count(e.name)) key_names.push_back(e.name);
+      if (present.count(e.name)) add_key_name(e.name);
     } else if (e.kind == FGPU_EXPR_DYNCOLUMN) {
       std::string prefix = e.name + ".";  // DynamicColumn.MatchColumn, expr.go:564
       for (auto& kv : present)
-        if (kv.first.compare(0, prefix.size(), prefix) == 0) key_names.push_back(kv.first);
+        if (kv.first.compare(0, prefix.size(), prefix) == 0) add_key_name(kv.first);
     } else if (e.kind == FGPU_EXPR_BINARY && e.op >= FGPU_OP_ADD && e.op <= FGPU_OP_DIV && q.kind == FGPU_PLAN_AGGREGATE) {
       const std::string name = q.expr_name(g);
       if (present.count(name)) return fail(FGPU_ERR_UNSUPPORTED, "computed group key shadows a column: " + name);
-      key_names.push_back(name);
-      key_expr[name] = g;
+      add_key_name(name);
+      k->key_expr[name] = g;
     } else {
       return fail(FGPU_ERR_UNSUPPORTED, "this group-by expression is not supported on the GPU path");
     }
   }
-  {
-    std::vector<std::string> uniq;
-    for (auto& n : key_names)
-      if (std::find(uniq.begin(), uniq.end(), n) == uniq.end()) uniq.push_back(n);
-    key_names.swap(uniq);
-  }
   if (key_names.size() > size_t(kMaxKeys)) return fail(FGPU_ERR_UNSUPPORTED, "too many group-by columns");
-  for (auto& n : key_names) {
-    if (key_expr.count(n)) continue;
-    int32_t rc = want(n);
-    if (rc) return rc;
-  }
-  // filter + aggregate + computed-key input columns
+  // slots: key columns first, then the computed keys', the filter's and the aggregates' input columns
   std::vector<std::string> cols;
-  for (auto& kv : key_expr) collect_columns(q, kv.second, &cols);
+  for (auto& n : key_names)
+    if (!k->key_expr.count(n)) cols.push_back(n);
+  for (auto& kv : k->key_expr) collect_columns(q, kv.second, &cols);
   collect_columns(q, q.filter, &cols);
   for (const fgpu_agg& a : q.aggs) collect_columns(q, a.expr, &cols);
-  for (auto& n : cols) {
-    int32_t rc = want(n);
-    if (rc) return rc;
+  for (auto& name : cols) {
+    auto it = present.find(name);
+    if (k->slot_of.count(name) || it == present.end()) continue;  // absent everywhere: handled by the callers
+    if (it->second == 0xff) return fail(FGPU_ERR_UNSUPPORTED, "column " + name + " has a type the GPU engine does not read");
+    if (c->slot_names.size() >= size_t(kMaxSlots)) return fail(FGPU_ERR_UNSUPPORTED, "query touches too many columns");
+    k->slot_of[name] = int(c->slot_names.size());
+    c->slot_names.push_back(name);
+    c->slot_types.push_back(it->second);
   }
+  c->qd.n_slots = int32_t(c->slot_names.size());
+  for (int s = 0; s < c->qd.n_slots; s++) c->qd.slot_type[s] = c->slot_types[size_t(s)];
+  c->slot_needed = q.kind == FGPU_PLAN_AGGREGATE ? k->value_slots(q, true) : std::vector<uint8_t>(c->slot_names.size(), 1);
+  return FGPU_OK;
+}
+
+// The only writer of the filter program in QueryDesc.  Pure conjunctions / disjunctions of leaves reduce to one mask
+// test per row.
+void set_filter_prog(Compiled* c) {
   QueryDesc& qd = c->qd;
-  qd.n_slots = int32_t(c->slot_names.size());
-  for (int s = 0; s < qd.n_slots; s++) {
-    qd.slot_type[s] = c->slot_types[size_t(s)];
+  qd.n_filter_prog = int32_t(c->filter_prog.size());
+  std::memset(qd.filter_prog, 0, sizeof qd.filter_prog);
+  std::memcpy(qd.filter_prog, c->filter_prog.data(), c->filter_prog.size());
+  bool all_and = true, all_or = true;
+  uint32_t mask = 0;
+  for (uint8_t op : c->filter_prog) {
+    if (op < 0x80) mask |= 1u << op;
+    else if (op == 0x80) all_or = false;
+    else all_and = false;
   }
-  // Count(col) counts rows, NULLs included (aggregate.go:929-950): its input column is never read,
-  // so it is neither uploaded nor staged unless something else in the query needs it.
-  {
-    std::vector<std::string> need = key_names;
-    for (auto& kv : key_expr) collect_columns(q, kv.second, &need);
-    collect_columns(q, q.filter, &need);
-    for (const fgpu_agg& a : q.aggs)
-      if (a.func != FGPU_AGG_COUNT) collect_columns(q, a.expr, &need);
-    c->slot_needed.assign(c->slot_names.size(), q.kind == FGPU_PLAN_AGGREGATE ? 0 : 1);
-    for (auto& n : need) {
-      auto it = slot_of.find(n);
-      if (it != slot_of.end()) c->slot_needed[size_t(it->second)] = 1;
+  qd.filter_mask = mask;
+  qd.filter_kind = all_and ? FK_AND : (all_or ? FK_OR : FK_PROGRAM);
+}
+
+// Checks a leaf against its column's type and puts a numeric leaf in canonical form (see LeafDesc).
+int32_t canonical_leaf(LeafHost* lh, uint8_t st) {
+  const ExprNode& lit = *lh->lit;
+  if (st == ST_DICT) {
+    switch (lh->op) {
+      case FGPU_OP_EQ: case FGPU_OP_NOT_EQ: case FGPU_OP_CONTAINS: case FGPU_OP_NOT_CONTAINS:
+        if (lit.lit_type != FGPU_SCALAR_NULL && lit.lit_type != FGPU_SCALAR_STRING)
+          return fail(FGPU_ERR_UNSUPPORTED, "dictionary column compared with a non-string literal");
+        return FGPU_OK;
+      case FGPU_OP_REGEX_MATCH: case FGPU_OP_REGEX_NOT_MATCH:
+        return FGPU_OK;
+      default:  // binaryscalarexpr.go:100-108
+        return fail(FGPU_ERR_INVALID, std::string("unsupported operator: ") + op_string(lh->op));
     }
   }
-  // filter
+  if (lh->op < FGPU_OP_EQ || lh->op > FGPU_OP_GT_EQ)
+    return fail(FGPU_ERR_UNSUPPORTED, std::string("operator ") + op_string(lh->op) + " on a numeric column");
+  if (lit.lit_type == FGPU_SCALAR_STRING) return fail(FGPU_ERR_UNSUPPORTED, "numeric column compared with a string literal");
+  lh->numeric = true;
+  lh->null_literal = lit.lit_type == FGPU_SCALAR_NULL;  // arrow compute against NULL: nothing selected (:143-150)
+  lh->cmp_float = (st == ST_F64) || lit.lit_type == FGPU_SCALAR_FLOAT64;
+  if (lh->cmp_float) canonical_float_range(lh->op, lit.lit_type == FGPU_SCALAR_FLOAT64 ? lit.lit_f : double(lit.lit_i), &lh->lo_f, &lh->hi_f, &lh->neg);
+  else canonical_int_range(lh->op, lit.lit_i, &lh->lo_i, &lh->hi_i, &lh->neg);
+  return FGPU_OK;
+}
+
+// Conjunction: comparisons on the same numeric column intersect into one range leaf
+// (timestamp >= a AND timestamp < b  ->  timestamp in [a, b-1]); a missing column keeps the
+// strictest of the merged leaves' missing-column behaviours.
+void fuse_conjunction(Compiled* c) {
+  std::vector<LeafHost> fused;
+  for (LeafHost& lh : c->leaves) {
+    bool merged = false;
+    if (lh.numeric && !lh.neg && !lh.null_literal && lh.slot >= 0) {
+      for (LeafHost& f : fused) {
+        if (!f.numeric || f.neg || f.null_literal || f.slot != lh.slot || f.cmp_float != lh.cmp_float) continue;
+        if (f.cmp_float) { f.lo_f = std::max(f.lo_f, lh.lo_f); f.hi_f = std::min(f.hi_f, lh.hi_f); }
+        else { f.lo_i = std::max(f.lo_i, lh.lo_i); f.hi_i = std::min(f.hi_i, lh.hi_i); }
+        if (lh.missing_mode == LM_NONE) f.missing_mode = LM_NONE;
+        merged = true;
+        break;
+      }
+    }
+    if (!merged) fused.push_back(lh);
+  }
+  if (fused.size() == c->leaves.size()) return;
+  c->leaves.swap(fused);
+  c->filter_prog.clear();
+  for (size_t l = 0; l < c->leaves.size(); l++) {
+    c->filter_prog.push_back(uint8_t(l));
+    if (l > 0) c->filter_prog.push_back(0x80);
+  }
+  set_filter_prog(c);
+}
+
+// The filter: its program, its leaves in canonical form, fused under a conjunction, and their descriptors.
+int32_t compile_predicate(const QueryPlan& q, const Switches& w, const std::map<std::string, int>& slot_of, Compiled* c) {
+  QueryDesc& qd = c->qd;
   if (q.filter >= 0) {
     int32_t rc = compile_filter(q, q.filter, c, slot_of);
     if (rc) return rc;
@@ -1182,100 +1253,15 @@ int32_t compile(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, const Switches& 
       maxd = std::max(maxd, depth);
     }
     if (maxd > 30) return fail(FGPU_ERR_UNSUPPORTED, "filter expression too deep");
-    qd.n_filter_prog = int32_t(c->filter_prog.size());
-    std::memcpy(qd.filter_prog, c->filter_prog.data(), c->filter_prog.size());
-    // pure conjunctions / disjunctions of leaves reduce to one mask test per row
-    bool all_and = true, all_or = true;
-    uint32_t mask = 0;
-    for (uint8_t op : c->filter_prog) {
-      if (op < 0x80) mask |= 1u << op;
-      else if (op == 0x80) all_or = false;
-      else all_and = false;
-    }
-    qd.filter_mask = mask;
-    qd.filter_kind = all_and ? FK_AND : (all_or ? FK_OR : FK_PROGRAM);
+    set_filter_prog(c);
   }
-  for (size_t l = 0; l < c->leaves.size(); l++) {
-    LeafHost& lh = c->leaves[l];
+  for (LeafHost& lh : c->leaves) {
     lh.missing_mode = missing_column_mode(lh);
     if (lh.slot < 0) continue;
-    uint8_t st = c->slot_types[size_t(lh.slot)];
-    const ExprNode& lit = *lh.lit;
-    if (st == ST_DICT) {
-      switch (lh.op) {
-        case FGPU_OP_EQ: case FGPU_OP_NOT_EQ: case FGPU_OP_CONTAINS: case FGPU_OP_NOT_CONTAINS:
-          if (lit.lit_type != FGPU_SCALAR_NULL && lit.lit_type != FGPU_SCALAR_STRING)
-            return fail(FGPU_ERR_UNSUPPORTED, "dictionary column compared with a non-string literal");
-          break;
-        case FGPU_OP_REGEX_MATCH: case FGPU_OP_REGEX_NOT_MATCH:
-          break;
-        default:  // binaryscalarexpr.go:100-108
-          return fail(FGPU_ERR_INVALID, std::string("unsupported operator: ") + op_string(lh.op));
-      }
-    } else {
-      if (lh.op < FGPU_OP_EQ || lh.op > FGPU_OP_GT_EQ)
-        return fail(FGPU_ERR_UNSUPPORTED, std::string("operator ") + op_string(lh.op) + " on a numeric column");
-      if (lit.lit_type == FGPU_SCALAR_STRING) return fail(FGPU_ERR_UNSUPPORTED, "numeric column compared with a string literal");
-      lh.numeric = true;
-      lh.null_literal = lit.lit_type == FGPU_SCALAR_NULL;  // arrow compute against NULL: nothing selected (:143-150)
-      lh.cmp_float = (st == ST_F64) || lit.lit_type == FGPU_SCALAR_FLOAT64;
-      const double kInf = std::numeric_limits<double>::infinity();
-      if (lh.cmp_float) {
-        const double v = lit.lit_type == FGPU_SCALAR_FLOAT64 ? lit.lit_f : double(lit.lit_i);
-        lh.lo_f = kInf; lh.hi_f = -kInf;  // empty
-        if (!std::isnan(v)) {
-          switch (lh.op) {
-            case FGPU_OP_EQ: lh.lo_f = lh.hi_f = v; break;
-            case FGPU_OP_NOT_EQ: lh.lo_f = lh.hi_f = v; lh.neg = true; break;
-            case FGPU_OP_LT: lh.lo_f = -kInf; lh.hi_f = std::nextafter(v, -kInf); break;
-            case FGPU_OP_LT_EQ: lh.lo_f = -kInf; lh.hi_f = v; break;
-            case FGPU_OP_GT: lh.lo_f = std::nextafter(v, kInf); lh.hi_f = kInf; break;
-            default: lh.lo_f = v; lh.hi_f = kInf; break;
-          }
-          if (lh.op == FGPU_OP_LT && v == -kInf) { lh.lo_f = kInf; lh.hi_f = -kInf; }
-          if (lh.op == FGPU_OP_GT && v == kInf) { lh.lo_f = kInf; lh.hi_f = -kInf; }
-        } else if (lh.op == FGPU_OP_NOT_EQ) {
-          lh.neg = true;  // x != NaN holds for every non-NULL x
-        }
-      } else {
-        bool neg = false;
-        canonical_int_range(lh.op, lit.lit_i, &lh.lo_i, &lh.hi_i, &neg);
-        lh.neg = neg;
-      }
-    }
+    int32_t rc = canonical_leaf(&lh, c->slot_types[size_t(lh.slot)]);
+    if (rc) return rc;
   }
-  // Conjunction: comparisons on the same numeric column intersect into one range leaf
-  // (timestamp >= a AND timestamp < b  ->  timestamp in [a, b-1]); a missing column keeps the
-  // strictest of the merged leaves' missing-column behaviours.
-  if (qd.filter_kind == FK_AND && !w.no_fuse) {
-    std::vector<LeafHost> fused;
-    for (LeafHost& lh : c->leaves) {
-      bool merged = false;
-      if (lh.numeric && !lh.neg && !lh.null_literal && lh.slot >= 0) {
-        for (LeafHost& f : fused) {
-          if (!f.numeric || f.neg || f.null_literal || f.slot != lh.slot || f.cmp_float != lh.cmp_float) continue;
-          if (f.cmp_float) { f.lo_f = std::max(f.lo_f, lh.lo_f); f.hi_f = std::min(f.hi_f, lh.hi_f); }
-          else { f.lo_i = std::max(f.lo_i, lh.lo_i); f.hi_i = std::min(f.hi_i, lh.hi_i); }
-          if (lh.missing_mode == LM_NONE) f.missing_mode = LM_NONE;
-          merged = true;
-          break;
-        }
-      }
-      if (!merged) fused.push_back(lh);
-    }
-    if (fused.size() != c->leaves.size()) {
-      c->leaves.swap(fused);
-      c->filter_prog.clear();
-      for (size_t l = 0; l < c->leaves.size(); l++) {
-        c->filter_prog.push_back(uint8_t(l));
-        if (l > 0) c->filter_prog.push_back(0x80);
-      }
-      qd.n_filter_prog = int32_t(c->filter_prog.size());
-      std::memset(qd.filter_prog, 0, sizeof qd.filter_prog);
-      std::memcpy(qd.filter_prog, c->filter_prog.data(), c->filter_prog.size());
-      qd.filter_mask = (c->leaves.size() >= 32) ? 0xffffffffu : ((1u << c->leaves.size()) - 1u);
-    }
-  }
+  if (qd.filter_kind == FK_AND && !w.no_fuse) fuse_conjunction(c);
   qd.n_leaves = int32_t(c->leaves.size());
   for (int l = 0; l < qd.n_leaves; l++) {
     const LeafHost& lh = c->leaves[size_t(l)];
@@ -1290,139 +1276,142 @@ int32_t compile(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, const Switches& 
     ld.lo_i = lh.lo_i; ld.hi_i = lh.hi_i;
     ld.lo_f = lh.lo_f; ld.hi_f = lh.hi_f;
   }
-  // ---- row-group pruning by chunk statistics ----------------------------------------------------------
-  // LSM.Scan asks the filter's TrueNegativeFilter whether a row group may hold matching rows before it
-  // hands the row group to the plan (index/lsm.go:401-454; expr/binaryscalarexpr.go:41-190 compares the
-  // literal with the chunk's min/max).  Same decision here, from the footer statistics, before anything
-  // is uploaded: an int64 range leaf whose chunk bounds miss the range selects nothing in that row group
-  // (under a conjunction the row group is dropped: never uploaded, never scanned); bounds inside the
-  // range of a chunk without NULLs select every row, and the leaf's column is then not read there.
-  {
-    const bool conj = qd.n_filter_prog > 0 && qd.filter_kind == FK_AND;
-    const bool may_skip = q.kind != FGPU_PLAN_FILTER;
-    std::vector<uint8_t> base(c->slot_names.size(), may_skip ? 0 : 1);  // needed regardless of the filter
-    if (may_skip) {
-      std::vector<std::string> need = key_names;
-      for (auto& kv : key_expr) collect_columns(q, kv.second, &need);
-      for (const fgpu_agg& a : q.aggs)
-        if (a.func != FGPU_AGG_COUNT) collect_columns(q, a.expr, &need);
-      for (auto& n : need) {
-        auto it = slot_of.find(n);
-        if (it != slot_of.end()) base[size_t(it->second)] = 1;
-      }
+  return FGPU_OK;
+}
+
+// AggFuncPushDown (logicalplan/optimize.go:166-193) + MaxAgg (expr/filter.go:156-207): a global Max(column)
+// directly above the scan, without filter, turns into a row-group filter that memoises the largest chunk
+// maximum seen so far, in scan order, and only lets row groups through that exceed it.
+struct MaxPushDown {
+  const std::string* column = nullptr;  // nullptr: the plan is not a global Max(column)
+  bool have = false;
+  int64_t max_i = 0;
+  double max_f = 0;
+
+  // false: the row group cannot raise the maximum (L0 Arrow records are never filtered, lsm.go:420-427)
+  bool admit(const VisibleRG& v) {
+    if (!column || v.part->arrow) return true;
+    auto it = v.rg->cols.find(*column);
+    if (it == v.rg->cols.end()) return false;  // no such field in this row group: nothing to contribute
+    const ChunkHost& ch = it->second;
+    if (ch.null_count >= 0 && uint64_t(ch.null_count) == v.rg->n_rows) return false;
+    if (!ch.has_minmax || (ch.phys != PT_INT64 && ch.phys != PT_DOUBLE)) return true;
+    bool greater;
+    if (ch.phys == PT_INT64) {
+      greater = !have || ch.max_bits > max_i;
+      if (greater) max_i = ch.max_bits;
+    } else {
+      double mx;
+      std::memcpy(&mx, &ch.max_bits, 8);
+      greater = !have || mx > max_f;
+      if (greater) max_f = mx;
     }
-    std::vector<VisibleRG> kept;
-    const bool prune_on = !w.no_prune;
-    // AggFuncPushDown (logicalplan/optimize.go:166-193) + MaxAgg (expr/filter.go:156-207): a global Max(column)
-    // directly above the scan, without filter, turns into a row-group filter that memoises the largest chunk
-    // maximum seen so far, in scan order, and only lets row groups through that exceed it.
-    bool max_agg = prune_on && q.kind == FGPU_PLAN_AGGREGATE && q.group_by.empty() && q.aggs.size() == 1 && q.aggs[0].func == FGPU_AGG_MAX &&
-                   q.filter < 0 && q.exprs[size_t(q.aggs[0].expr)].kind == FGPU_EXPR_COLUMN;
-    const std::string max_col = max_agg ? q.exprs[size_t(q.aggs[0].expr)].name : std::string();
-    bool have_max = false;
-    int64_t max_i = 0;
-    double max_f = 0;
-    for (VisibleRG& v : c->rgs) {
-      if (max_agg && !v.part->arrow) {
-        auto it = v.rg->cols.find(max_col);
-        if (it == v.rg->cols.end()) continue;  // no such field in this row group: nothing to contribute
-        const ChunkHost& ch = it->second;
-        const bool all_null = ch.null_count >= 0 && uint64_t(ch.null_count) == v.rg->n_rows;
-        if (all_null) continue;
-        if (ch.has_minmax && (ch.phys == PT_INT64 || ch.phys == PT_DOUBLE)) {
-          bool greater;
-          if (ch.phys == PT_INT64) {
-            greater = !have_max || ch.max_bits > max_i;
-            if (greater) max_i = ch.max_bits;
-          } else {
-            double mx;
-            std::memcpy(&mx, &ch.max_bits, 8);
-            greater = !have_max || mx > max_f;
-            if (greater) max_f = mx;
-          }
-          if (!greater) continue;
-          have_max = true;
-        }
-      }
-      // Parquet parts: the reference's own row-group filter first (L0 Arrow records are never filtered, lsm.go:420-427)
-      if (prune_on && !v.part->arrow && q.filter >= 0 && !rg_may_match(q, q.filter, *v.rg)) continue;
-      bool drop = false;
-      for (size_t l = 0; l < c->leaves.size() && prune_on; l++) {
-        const LeafHost& lh = c->leaves[l];
-        uint8_t mode = LM_EVAL;
-        auto it = lh.slot < 0 ? v.rg->cols.end() : v.rg->cols.find(lh.column);
-        if (it == v.rg->cols.end()) {
-          mode = lh.missing_mode;  // the physical plan's rule for the rows of a row group that got this far (physicalplan/binaryscalarexpr.go:47-73)
-        } else if (lh.numeric && !lh.cmp_float && !lh.null_literal && c->slot_types[size_t(lh.slot)] == ST_I64 && it->second.has_minmax) {
-          mode = chunk_leaf_mode(lh.lo_i, lh.hi_i, lh.neg, true, it->second.min_bits, it->second.max_bits, it->second.null_count, int64_t(v.rg->n_rows));
-        }
-        else if (it != v.rg->cols.end() && c->slot_types[size_t(lh.slot)] == ST_DICT && lh.op == FGPU_OP_EQ &&
-                 lh.lit->lit_type == FGPU_SCALAR_STRING && it->second.has_minmax_str) {
-          // string equality against the chunk's bounding strings (binaryscalarexpr.go:98-104; bounds may be
-          // truncated by the writer, they still bound): outside them no value can be equal
-          const std::string& lit = lh.lit->lit_bytes;
-          if (lit < it->second.min_str || lit > it->second.max_str) mode = LM_NONE;
-        }
-        // equality with a value the chunk's bloom filter rules out: the leaf is false on every row of the row group
-        // (also under a disjunction, where the row group itself stays)
-        if (mode == LM_EVAL && it != v.rg->cols.end() && lh.op == FGPU_OP_EQ && !lh.null_literal && !v.part->arrow &&
-            !bloom_may_contain(it->second, *lh.lit))
-          mode = LM_NONE;
-        v.leaf_mode[l] = mode;
-        if (conj && mode == LM_NONE) drop = true;
-      }
-      if (drop) continue;
-      for (size_t s = 0; s < c->slot_names.size(); s++) {
-        bool needed = base[s] != 0;
-        for (size_t l = 0; l < c->leaves.size() && !needed; l++)
-          if (c->leaves[l].slot == int(s) && v.leaf_mode[l] == LM_EVAL) needed = true;
-        if (!needed || !c->slot_needed[s]) v.skip_slots |= 1ull << s;
-      }
-      kept.push_back(v);
-    }
-    c->pruned_row_groups = uint32_t(c->rgs.size() - kept.size());
-    c->rgs.swap(kept);
-    c->touched_rows = 0;
-    for (const VisibleRG& v : c->rgs) c->touched_rows += v.rg->n_rows;
-    // Every row group ruled out: nothing is scanned, but the plan keeps its full shape (keys, aggregates, table
-    // slots): a rank whose time range misses the filter must still produce a partial table its peers can merge.
+    if (greater) have = true;
+    return greater;
   }
-  // Lazy residency: the columns this query projects are built and uploaded now (parts put with
-  // FGPU_PUT_BORROW_PINNED upload nothing until a query needs it; optimize.go:36-73 physical projection).
-  {
-    PhaseClock pc;
-    double build_us = 0, upload_us = 0;
-    // numeric columns first: their bytes are the bulk of the transfer, which then runs while the host
-    // assembles the dictionary columns' run directories
-    for (int pass = 0; pass < 2; pass++) {
-    Part* last = nullptr;
-    for (const VisibleRG& v : c->rgs) {
-      if (v.part == last) continue;
-      last = v.part;
+};
+
+// What the chunk statistics of one row group decide about one leaf (LM_EVAL: undecided).
+uint8_t leaf_mode(const Compiled& c, const LeafHost& lh, const VisibleRG& v) {
+  auto it = lh.slot < 0 ? v.rg->cols.end() : v.rg->cols.find(lh.column);
+  // the physical plan's rule for the rows of a row group that got this far (physicalplan/binaryscalarexpr.go:47-73)
+  if (it == v.rg->cols.end()) return lh.missing_mode;
+  const ChunkHost& ch = it->second;
+  const uint8_t st = c.slot_types[size_t(lh.slot)];
+  uint8_t mode = LM_EVAL;
+  if (lh.numeric && !lh.cmp_float && !lh.null_literal && st == ST_I64 && ch.has_minmax) {
+    mode = chunk_leaf_mode(lh.lo_i, lh.hi_i, lh.neg, true, ch.min_bits, ch.max_bits, ch.null_count, int64_t(v.rg->n_rows));
+  } else if (st == ST_DICT && lh.op == FGPU_OP_EQ && lh.lit->lit_type == FGPU_SCALAR_STRING && ch.has_minmax_str) {
+    // string equality against the chunk's bounding strings (binaryscalarexpr.go:98-104; bounds may be
+    // truncated by the writer, they still bound): outside them no value can be equal
+    const std::string& lit = lh.lit->lit_bytes;
+    if (lit < ch.min_str || lit > ch.max_str) mode = LM_NONE;
+  }
+  // equality with a value the chunk's bloom filter rules out: the leaf is false on every row of the row group
+  // (also under a disjunction, where the row group itself stays)
+  if (mode == LM_EVAL && lh.op == FGPU_OP_EQ && !lh.null_literal && !v.part->arrow && !bloom_may_contain(ch, *lh.lit)) mode = LM_NONE;
+  return mode;
+}
+
+// Row-group pruning by chunk statistics.  LSM.Scan asks the filter's TrueNegativeFilter whether a row group may
+// hold matching rows before it hands the row group to the plan (index/lsm.go:401-454; expr/binaryscalarexpr.go:41-190
+// compares the literal with the chunk's min/max).  Same decision here, from the footer statistics, before anything
+// is uploaded: an int64 range leaf whose chunk bounds miss the range selects nothing in that row group (under a
+// conjunction the row group is dropped: never uploaded, never scanned); bounds inside the range of a chunk without
+// NULLs select every row, and the leaf's column is then not read there.  `base`: the slots needed regardless of the
+// filter.
+void prune_row_groups(const QueryPlan& q, const Switches& w, const std::vector<uint8_t>& base, Compiled* c) {
+  const bool conj = c->qd.n_filter_prog > 0 && c->qd.filter_kind == FK_AND;
+  const bool prune_on = !w.no_prune;
+  MaxPushDown max_agg;
+  if (prune_on && q.kind == FGPU_PLAN_AGGREGATE && q.group_by.empty() && q.aggs.size() == 1 && q.aggs[0].func == FGPU_AGG_MAX &&
+      q.filter < 0 && q.exprs[size_t(q.aggs[0].expr)].kind == FGPU_EXPR_COLUMN)
+    max_agg.column = &q.exprs[size_t(q.aggs[0].expr)].name;
+  std::vector<VisibleRG> kept;
+  for (VisibleRG& v : c->rgs) {
+    if (!max_agg.admit(v)) continue;
+    // Parquet parts: the reference's own row-group filter first (L0 Arrow records are never filtered, lsm.go:420-427)
+    if (prune_on && !v.part->arrow && q.filter >= 0 && !rg_may_match(q, q.filter, *v.rg)) continue;
+    bool drop = false;
+    for (size_t l = 0; l < c->leaves.size() && prune_on; l++) {
+      v.leaf_mode[l] = leaf_mode(*c, c->leaves[l], v);
+      if (conj && v.leaf_mode[l] == LM_NONE) drop = true;
+    }
+    if (drop) continue;
+    for (size_t s = 0; s < c->slot_names.size(); s++) {
+      bool needed = base[s] != 0;
+      for (size_t l = 0; l < c->leaves.size() && !needed; l++)
+        if (c->leaves[l].slot == int(s) && v.leaf_mode[l] == LM_EVAL) needed = true;
+      if (!needed || !c->slot_needed[s]) v.skip_slots |= 1ull << s;
+    }
+    kept.push_back(v);
+  }
+  c->pruned_row_groups = uint32_t(c->rgs.size() - kept.size());
+  c->rgs.swap(kept);
+  c->touched_rows = 0;
+  for (const VisibleRG& v : c->rgs) c->touched_rows += v.rg->n_rows;
+  // Every row group ruled out: nothing is scanned, but the plan keeps its full shape (keys, aggregates, table
+  // slots): a rank whose time range misses the filter must still produce a partial table its peers can merge.
+}
+
+// Lazy residency: the columns this query projects are built and uploaded now (parts put with
+// FGPU_PUT_BORROW_PINNED upload nothing until a query needs it; optimize.go:36-73 physical projection).
+int32_t make_resident(fgpu_ctx* ctx, Table& table, Compiled* c) {
+  PhaseClock pc;
+  double build_us = 0, upload_us = 0;
+  std::vector<std::pair<Part*, uint64_t>> reads;  // per part, in row-group order: bit s = some kept row group reads slot s
+  for (const VisibleRG& v : c->rgs) {
+    if (reads.empty() || reads.back().first != v.part) reads.push_back({v.part, 0});
+    reads.back().second |= ~v.skip_slots;
+  }
+  // numeric columns first: their bytes are the bulk of the transfer, which then runs while the host
+  // assembles the dictionary columns' run directories
+  for (int pass = 0; pass < 2; pass++) {
+    for (auto& [part, read] : reads) {
       for (size_t si = 0; si < c->slot_names.size(); si++) {
         const std::string& name = c->slot_names[si];
-        if ((c->slot_types[si] == ST_DICT) != (pass == 1)) continue;
-        bool read = false;
-        for (const VisibleRG& w : c->rgs)
-          if (w.part == v.part && !((w.skip_slots >> si) & 1)) { read = true; break; }
-        if (!read) continue;
-        if (std::find(v.part->columns.begin(), v.part->columns.end(), name) == v.part->columns.end()) continue;
-        int32_t rc = ensure_resident(ctx, &table, v.part, name, &c->h2d_bytes, pc.on ? &build_us : nullptr, pc.on ? &upload_us : nullptr);
+        if ((c->slot_types[si] == ST_DICT) != (pass == 1) || !((read >> si) & 1)) continue;
+        if (std::find(part->columns.begin(), part->columns.end(), name) == part->columns.end()) continue;
+        int32_t rc = ensure_resident(ctx, &table, part, name, &c->h2d_bytes, pc.on ? &build_us : nullptr, pc.on ? &upload_us : nullptr);
         if (rc) return rc;
-        const ColumnImage& img = v.part->images[name];
+        const ColumnImage& img = part->images[name];
         if (!img.error.empty()) return fail(FGPU_ERR_UNSUPPORTED, "column " + name + ": " + img.error);
       }
     }
-    }
-    if (pc.on && c->h2d_bytes) {
-      char buf[128];
-      snprintf(buf, sizeof buf, " build=%.0fus enqueue=%.0fus bytes=%llu", build_us, upload_us, (unsigned long long)c->h2d_bytes);
-      pc.line = buf;
-      pc.flush("residency");
-    }
   }
-  // shared-memory ring of the scan kernel: stage every numeric slot's PLAIN slice (up to kMaxStagePlain)
-  // and the chunk seeds of every hybrid stream (up to kMaxStageSeeds); the rest is read from HBM directly
+  if (pc.on && c->h2d_bytes) {
+    char buf[128];
+    snprintf(buf, sizeof buf, " build=%.0fus enqueue=%.0fus bytes=%llu", build_us, upload_us, (unsigned long long)c->h2d_bytes);
+    pc.line = buf;
+    pc.flush("residency");
+  }
+  return FGPU_OK;
+}
+
+// shared-memory ring of the scan kernel: stage every numeric slot's PLAIN slice (up to kMaxStagePlain)
+// and the chunk seeds of every hybrid stream (up to kMaxStageSeeds); the rest is read from HBM directly
+void stage_slots(Compiled* c) {
+  QueryDesc& qd = c->qd;
   for (int s = 0; s < kMaxSlots; s++) {
     qd.slot_plain_stage[s] = -1;
     qd.slot_seed_stage[s][0] = qd.slot_seed_stage[s][1] = -1;
@@ -1442,21 +1431,44 @@ int32_t compile(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, const Switches& 
       qd.slot_plain_stage[s] = int8_t(qd.n_stage_plain);
       qd.stage_plain_slot[qd.n_stage_plain++] = uint8_t(s);
     }
-    if (any_vals && qd.n_stage_seeds < kMaxStageSeeds) {
-      qd.slot_seed_stage[s][0] = int8_t(qd.n_stage_seeds);
+    for (int is_def = 0; is_def < 2; is_def++) {  // the values' stream, then the definition levels'
+      if (!(is_def ? any_def : any_vals) || qd.n_stage_seeds >= kMaxStageSeeds) continue;
+      qd.slot_seed_stage[s][is_def] = int8_t(qd.n_stage_seeds);
       qd.stage_seed_slot[qd.n_stage_seeds] = uint8_t(s);
-      qd.stage_seed_is_def[qd.n_stage_seeds++] = 0;
-    }
-    if (any_def && qd.n_stage_seeds < kMaxStageSeeds) {
-      qd.slot_seed_stage[s][1] = int8_t(qd.n_stage_seeds);
-      qd.stage_seed_slot[qd.n_stage_seeds] = uint8_t(s);
-      qd.stage_seed_is_def[qd.n_stage_seeds++] = 1;
+      qd.stage_seed_is_def[qd.n_stage_seeds++] = uint8_t(is_def);
     }
   }
-  // aggregates
+}
+
+// Operand-stack depth of prog[off, off + len): the kernel evaluates aggregate and group-by expressions on a stack of
+// three shared-memory vectors.
+int prog_depth(const std::vector<ProgOp>& prog, size_t off, size_t len) {
+  int depth = 0, maxd = 0;
+  for (size_t p = off; p < off + len; p++) {
+    depth += (prog[p].op == PO_LOAD || prog[p].op == PO_CONST) ? 1 : -1;
+    maxd = std::max(maxd, depth);
+  }
+  return maxd;
+}
+
+// Whether every kept row group has every column of expression `node`; if not, *missing is the first one lacking.
+bool in_every_row_group(const QueryPlan& q, int node, const std::vector<VisibleRG>& rgs, std::string* missing) {
+  std::vector<std::string> cols;
+  collect_columns(q, node, &cols);
+  for (const VisibleRG& v : rgs)
+    for (auto& n : cols)
+      if (!v.rg->cols.count(n)) {
+        *missing = n;
+        return false;
+      }
+  return true;
+}
+
+// Aggregate programs, in qd.prog in aggregate order.
+int32_t compile_aggregates(const QueryPlan& q, const std::map<std::string, int>& slot_of, Compiled* c, std::vector<ProgOp>* prog) {
+  QueryDesc& qd = c->qd;
   if (q.aggs.size() > size_t(kMaxAggs)) return fail(FGPU_ERR_UNSUPPORTED, "too many aggregates");
   qd.n_aggs = int32_t(q.aggs.size());
-  std::vector<ProgOp> prog;
   for (size_t a = 0; a < q.aggs.size(); a++) {
     AggDesc& ad = qd.aggs[a];
     int f = q.aggs[a].func;
@@ -1464,115 +1476,92 @@ int32_t compile(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, const Switches& 
       return fail(FGPU_ERR_UNSUPPORTED, std::string("aggregate function not supported on the GPU path: ") + agg_string(f));
     ad.func = uint8_t(f);
     bool any_float = false, any_int_col = false;
-    size_t off = prog.size();
-    int32_t rc = compile_agg_expr(q, q.aggs[a].expr, slot_of, *c, &prog, &any_float, &any_int_col);
+    size_t off = prog->size();
+    int32_t rc = compile_agg_expr(q, q.aggs[a].expr, slot_of, *c, prog, &any_float, &any_int_col);
     if (rc) return rc;
     if (any_float && any_int_col) return fail(FGPU_ERR_UNSUPPORTED, "arithmetic mixes int64 and float64 columns");
     if (any_float) {  // integer literals take part as doubles
-      for (size_t p = off; p < prog.size(); p++)
-        if (prog[p].op == PO_CONST && prog[p].slot == 0) {
-          double d = double(prog[p].imm);
-          std::memcpy(&prog[p].imm, &d, 8);
+      for (size_t p = off; p < prog->size(); p++)
+        if ((*prog)[p].op == PO_CONST && (*prog)[p].slot == 0) {
+          double d = double((*prog)[p].imm);
+          std::memcpy(&(*prog)[p].imm, &d, 8);
         }
     }
     ad.is_float = any_float;
     ad.prog_off = uint8_t(off);
-    ad.prog_len = uint8_t(prog.size() - off);
+    ad.prog_len = uint8_t(prog->size() - off);
     // the aggregated column must exist in every record (aggregate.go:367-380)
-    std::vector<std::string> acols;
-    collect_columns(q, q.aggs[a].expr, &acols);
-    for (const VisibleRG& v : c->rgs)
-      for (auto& n : acols)
-        if (!v.rg->cols.count(n))
-          return fail(FGPU_ERR_NOT_FOUND, "aggregate field(s) not found [\"" + n + "\"], aggregations are not possible without it");
+    std::string missing;
+    if (!in_every_row_group(q, q.aggs[a].expr, c->rgs, &missing))
+      return fail(FGPU_ERR_NOT_FOUND, "aggregate field(s) not found [\"" + missing + "\"], aggregations are not possible without it");
   }
-  if (prog.size() > size_t(kMaxProg)) return fail(FGPU_ERR_UNSUPPORTED, "aggregate expressions too large");
-  for (size_t p = 0; p < prog.size(); p++) qd.prog[p] = prog[p];
-  // the kernel evaluates aggregate expressions on an operand stack of three shared-memory vectors
-  for (size_t a = 0; a < q.aggs.size(); a++) {
-    int depth = 0, maxd = 0;
-    for (int p = qd.aggs[a].prog_off; p < qd.aggs[a].prog_off + qd.aggs[a].prog_len; p++) {
-      depth += (prog[size_t(p)].op == PO_LOAD || prog[size_t(p)].op == PO_CONST) ? 1 : -1;
-      maxd = std::max(maxd, depth);
-    }
-    if (maxd > 3) return fail(FGPU_ERR_UNSUPPORTED, "aggregate expression nests too deeply for the GPU path");
+  // every aggregate's columns are looked up before any program is sized or its depth checked
+  if (prog->size() > size_t(kMaxProg)) return fail(FGPU_ERR_UNSUPPORTED, "aggregate expressions too large");
+  for (size_t p = 0; p < prog->size(); p++) qd.prog[p] = (*prog)[p];
+  for (size_t a = 0; a < q.aggs.size(); a++)
+    if (prog_depth(*prog, qd.aggs[a].prog_off, qd.aggs[a].prog_len) > 3)
+      return fail(FGPU_ERR_UNSUPPORTED, "aggregate expression nests too deeply for the GPU path");
+  return FGPU_OK;
+}
+
+// One result key column of the plan (slot -1: a computed key).
+void add_key(Compiled* c, Table& table, const std::string& name, uint8_t type, int slot) {
+  KeyOut ko;
+  ko.name = name;
+  ko.is_int64 = type != ST_DICT;
+  ko.is_float = type == ST_F64;
+  if (!ko.is_int64) ko.dict = &table.dicts[name];  // (a column whose every row group was pruned was never built: empty dictionary)
+  c->keys.push_back(std::move(ko));
+  c->key_slots.push_back(slot);
+}
+
+// Filter -> Projection(columns): the resolved columns are the output of a rows plan, no table.
+int32_t project_rows(const Columns& k, Table& table, Compiled* c) {
+  if (k.key_names.size() > size_t(kMaxOut)) return fail(FGPU_ERR_UNSUPPORTED, "too many projected columns");
+  c->qd.n_out = int32_t(k.key_names.size());
+  for (size_t i = 0; i < k.key_names.size(); i++) {
+    const int slot = k.slot_of.at(k.key_names[i]);
+    c->qd.out_slot[i] = uint8_t(slot);
+    add_key(c, table, k.key_names[i], c->slot_types[size_t(slot)], slot);
   }
-  qd.tile_rows = ctx->tile_rows;
-  qd.n_rg = int32_t(c->rgs.size());
-  if (q.kind == FGPU_PLAN_FILTER) {
-    // Filter -> Projection(columns): the resolved columns are the output, no table
-    if (key_names.size() > size_t(kMaxOut)) return fail(FGPU_ERR_UNSUPPORTED, "too many projected columns");
-    qd.n_out = int32_t(key_names.size());
-    for (size_t k = 0; k < key_names.size(); k++) {
-      int slot = slot_of.at(key_names[k]);
-      qd.out_slot[k] = uint8_t(slot);
-      KeyOut ko;
-      ko.name = key_names[k];
-      ko.is_int64 = c->slot_types[size_t(slot)] != ST_DICT;
-      ko.is_float = c->slot_types[size_t(slot)] == ST_F64;
-      if (!ko.is_int64) ko.dict = &table.dicts[key_names[k]];  // (a column whose every row group was pruned was never built: empty dictionary)
-      c->keys.push_back(std::move(ko));
-      c->key_slots.push_back(slot);
-    }
-    return FGPU_OK;
-  }
-  // keys and table shape
-  qd.n_keys = int32_t(key_names.size());
+  return FGPU_OK;
+}
+
+// Group keys (dictionary and int64 columns, and computed int64 keys, whose programs follow the aggregates' in qd.prog)
+// and the aggregate table: dense over the dictionary ids when every key is a dictionary column and the product of
+// their radices is at most kDenseMax, a hash table of packed keys otherwise.
+int32_t table_shape(const QueryPlan& q, const Columns& k, Table& table, std::vector<ProgOp>* prog, Compiled* c) {
+  QueryDesc& qd = c->qd;
+  qd.n_keys = int32_t(k.key_names.size());
+  c->dense_radix.assign(k.key_names.size(), 0);
   bool all_dict = true;
   long double product = 1;
-  c->dense_radix.assign(key_names.size(), 0);
-  for (size_t k = 0; k < key_names.size(); k++) {
-    const auto kx = key_expr.find(key_names[k]);
-    if (kx != key_expr.end()) {  // computed int64 key: its program sits behind the aggregates' in qd.prog
+  for (size_t i = 0; i < k.key_names.size(); i++) {
+    const std::string& name = k.key_names[i];
+    const auto kx = k.key_expr.find(name);
+    if (kx != k.key_expr.end()) {  // computed int64 key
       bool any_float = false, any_int_col = false;
-      const size_t off = prog.size();
-      int32_t rc = compile_agg_expr(q, kx->second, slot_of, *c, &prog, &any_float, &any_int_col);
+      const size_t off = prog->size();
+      int32_t rc = compile_agg_expr(q, kx->second, k.slot_of, *c, prog, &any_float, &any_int_col);
       if (rc) return rc;
       if (any_float) return fail(FGPU_ERR_UNSUPPORTED, "float64 group-by expressions are not supported");
-      if (prog.size() > size_t(kMaxProg) || prog.size() - off > 255) return fail(FGPU_ERR_UNSUPPORTED, "group-by expression too large");
-      int depth = 0, maxd = 0;
-      for (size_t p = off; p < prog.size(); p++) {
-        depth += (prog[p].op == PO_LOAD || prog[p].op == PO_CONST) ? 1 : -1;
-        maxd = std::max(maxd, depth);
-      }
-      if (maxd > 3) return fail(FGPU_ERR_UNSUPPORTED, "group-by expression nests too deeply for the GPU path");
-      for (size_t p = off; p < prog.size(); p++) qd.prog[p] = prog[p];
-      std::vector<std::string> kcols;
-      collect_columns(q, kx->second, &kcols);
-      for (const VisibleRG& v : c->rgs)
-        for (auto& n : kcols)
-          if (!v.rg->cols.count(n)) return fail(FGPU_ERR_NOT_FOUND, "group-by expression column not found: " + n);
-      KeyOut ko;
-      ko.name = key_names[k];
-      ko.is_int64 = true;
-      all_dict = false;
-      product *= 1e18L;
-      c->keys.push_back(std::move(ko));
-      c->key_slots.push_back(-1);
-      qd.keys[k].slot = 0xff;
-      qd.keys[k].is_int64 = 1;
-      qd.keys[k].prog_off = uint8_t(off);
-      qd.keys[k].prog_len = uint8_t(prog.size() - off);
-      continue;
+      if (prog->size() > size_t(kMaxProg) || prog->size() - off > 255) return fail(FGPU_ERR_UNSUPPORTED, "group-by expression too large");
+      if (prog_depth(*prog, off, prog->size() - off) > 3) return fail(FGPU_ERR_UNSUPPORTED, "group-by expression nests too deeply for the GPU path");
+      for (size_t p = off; p < prog->size(); p++) qd.prog[p] = (*prog)[p];
+      std::string missing;
+      if (!in_every_row_group(q, kx->second, c->rgs, &missing)) return fail(FGPU_ERR_NOT_FOUND, "group-by expression column not found: " + missing);
+      qd.keys[i].prog_off = uint8_t(off);
+      qd.keys[i].prog_len = uint8_t(prog->size() - off);
     }
-    int slot = slot_of.at(key_names[k]);
-    KeyOut ko;
-    ko.name = key_names[k];
-    ko.is_int64 = c->slot_types[size_t(slot)] != ST_DICT;
-    if (c->slot_types[size_t(slot)] == ST_F64) return fail(FGPU_ERR_UNSUPPORTED, "float64 group-by columns are not supported");
-    if (ko.is_int64) {
-      all_dict = false;
-      product *= 1e18L;
-    } else {
-      ko.dict = &table.dicts[key_names[k]];
-      uint32_t card = ko.dict->cardinality();
-      c->dense_radix[k] = card + 1;
-      product *= (long double)(card + 1);
-    }
-    c->keys.push_back(std::move(ko));
-    c->key_slots.push_back(slot);
-    qd.keys[k].slot = uint8_t(slot);
-    qd.keys[k].is_int64 = c->keys.back().is_int64;
+    const int slot = kx != k.key_expr.end() ? -1 : k.slot_of.at(name);
+    const uint8_t type = slot < 0 ? uint8_t(ST_I64) : c->slot_types[size_t(slot)];
+    if (type == ST_F64) return fail(FGPU_ERR_UNSUPPORTED, "float64 group-by columns are not supported");
+    add_key(c, table, name, type, slot);
+    if (type == ST_DICT) c->dense_radix[i] = c->keys.back().dict->cardinality() + 1;
+    if (type != ST_DICT) all_dict = false;
+    product *= type == ST_DICT ? (long double)c->dense_radix[i] : 1e18L;
+    qd.keys[i].slot = uint8_t(slot < 0 ? 0xff : slot);
+    qd.keys[i].is_int64 = type != ST_DICT;
   }
   long double bound = std::min<long double>(product, (long double)std::max<uint64_t>(c->total_rows, 1));
   c->group_bound = uint64_t(bound);
@@ -1581,85 +1570,132 @@ int32_t compile(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, const Switches& 
     qd.table_mode = TM_DENSE;
     qd.key_words = 1;
     uint64_t stride = 1;
-    for (size_t k = key_names.size(); k-- > 0;) {
+    for (size_t k = c->keys.size(); k-- > 0;) {
       qd.keys[k].dense_stride = uint32_t(stride);
       stride *= c->dense_radix[k];
     }
     qd.table_slots = uint32_t(std::max<uint64_t>(stride, 1));
-  } else {
-    qd.table_mode = TM_HASH;
-    int word = 0, used = 0;
-    for (size_t k = 0; k < key_names.size(); k++) {
-      if (c->keys[k].is_int64) continue;
-      int bits = std::max(1, bit_width_u32(c->dense_radix[k] - 1));
-      if (used + bits > 64) { word++; used = 0; }
-      qd.keys[k].word = uint8_t(word);
-      qd.keys[k].shift = uint8_t(used);
-      qd.keys[k].bits = uint32_t(bits);
-      used += bits;
-    }
-    int words = (used > 0 || word > 0) ? word + 1 : 0;
-    for (size_t k = 0; k < key_names.size(); k++) {
-      if (!c->keys[k].is_int64) continue;
-      qd.keys[k].word = uint8_t(words++);
-      qd.keys[k].shift = 0;
-      qd.keys[k].bits = 64;
-    }
-    if (words > kMaxKeyWords) return fail(FGPU_ERR_UNSUPPORTED, "group key wider than the packed-key limit");
-    qd.key_words = std::max(words, 1);
-    uint64_t cap = 1024;
-    while (cap < 2 * c->group_bound && cap < (1ull << 28)) cap <<= 1;
-    qd.table_slots = uint32_t(cap);
+    return FGPU_OK;
   }
-  // ---- scan kernel: vector length, ring depth and the per-warp shared-memory layout ----------------
-  {
-    int vl = w.vl, ring = w.ring;
-    bool any_expr = false;
-    for (int k = 0; k < qd.n_keys; k++)
-      if (qd.keys[k].prog_len) any_expr = true;
-    for (int a = 0; a < qd.n_aggs; a++)
-      if (qd.aggs[a].func != FGPU_AGG_COUNT && !(qd.aggs[a].prog_len == 1 && qd.prog[qd.aggs[a].prog_off].op == PO_LOAD)) any_expr = true;
-    auto r128 = [](size_t x) { return (x + 127) & ~size_t(127); };
-    for (;;) {
-      size_t off = r128(size_t(ring) * 8);
-      size_t slot = r128(size_t(qd.n_stage_plain) * vl * 8 + size_t(qd.n_stage_seeds) * sizeof(Seed));
-      if (slot == 0) slot = 128;
-      qd.slot_bytes = uint32_t(slot);
-      qd.wr_ring = uint32_t(off); off += size_t(ring) * slot;
-      qd.wr_act = uint32_t(off); off = r128(off + size_t(vl / 32) * 4);
-      qd.wr_leaf = uint32_t(off); off = r128(off + ((qd.n_filter_prog > 0 && qd.filter_kind != FK_AND) ? size_t(vl) * 4 : 0));
-      qd.wr_slot = uint32_t(off); off = r128(off + size_t(vl) * 4);
-      qd.wr_keyw = uint32_t(off); off = r128(off + (qd.table_mode == TM_HASH ? size_t(qd.key_words) * vl * 8 : 0));
-      qd.wr_tmp1 = uint32_t(off); off = r128(off + (any_expr ? size_t(vl) * 8 : 0));
-      qd.wr_tmp2 = uint32_t(off); off = r128(off + (any_expr ? size_t(vl) * 16 : 0));
-      qd.wr_acc = uint32_t(off); off = r128(off + size_t(qd.n_aggs) * 32 * 8 + 16 + 32 * 4 + 32 * 4 + (qd.table_mode == TM_HASH ? size_t(qd.key_words) * 32 * 8 : 0));
-      qd.wr_cdesc = uint32_t(off); off = r128(off + size_t(std::max(qd.n_slots, 1)) * sizeof(ChunkDesc));
-      qd.wr_clrt = uint32_t(off); off = r128(off + size_t(std::max(qd.n_leaves, 1)) * sizeof(LeafRt));
-      qd.wr_fplan = uint32_t(off); off = r128(off + 512);
-      qd.wr_iplan = uint32_t(off); off = r128(off + 8 + 16 * size_t(kMaxStagePlain + kMaxStageSeeds));
-      qd.wr_bytes = uint32_t(off);
-      if (size_t(qd.wr_bytes) * (kVecThreads / 32) <= 200 * 1024 || vl == 128) break;
-      vl /= 2;  // many staged columns / wide keys: shorter vectors
-    }
-    qd.vl = vl;
-    qd.n_ring = ring;
-    // fused fast path: conjunction of numeric leaves, dense dictionary keys, simple aggregates
-    bool fast = qd.table_mode == TM_DENSE && (qd.n_filter_prog == 0 || qd.filter_kind == FK_AND) && qd.n_leaves <= 2 && qd.n_keys <= 3 &&
-                !w.no_fast;
-    for (int l = 0; l < qd.n_leaves && fast; l++) {
-      const LeafHost& lh = c->leaves[size_t(l)];
-      if (lh.slot >= 0 && c->slot_types[size_t(lh.slot)] == ST_DICT) fast = false;
-      if (lh.slot >= 0 && lh.null_literal) fast = false;
-    }
-    int stored = 0;
-    for (int a = 0; a < qd.n_aggs && fast; a++) {
-      if (qd.aggs[a].func == FGPU_AGG_COUNT) continue;
-      stored++;
-      if (!(qd.aggs[a].prog_len == 1 && qd.prog[qd.aggs[a].prog_off].op == PO_LOAD)) fast = false;
-    }
-    if (stored > 2) fast = false;
-    qd.fast_ok = fast ? 1 : 0;
+  qd.table_mode = TM_HASH;
+  int word = 0, used = 0;
+  for (size_t k = 0; k < c->keys.size(); k++) {
+    if (c->keys[k].is_int64) continue;
+    int bits = std::max(1, bit_width_u32(c->dense_radix[k] - 1));
+    if (used + bits > 64) { word++; used = 0; }
+    qd.keys[k].word = uint8_t(word);
+    qd.keys[k].shift = uint8_t(used);
+    qd.keys[k].bits = uint32_t(bits);
+    used += bits;
   }
+  int words = (used > 0 || word > 0) ? word + 1 : 0;
+  for (size_t k = 0; k < c->keys.size(); k++) {
+    if (!c->keys[k].is_int64) continue;
+    qd.keys[k].word = uint8_t(words++);
+    qd.keys[k].shift = 0;
+    qd.keys[k].bits = 64;
+  }
+  if (words > kMaxKeyWords) return fail(FGPU_ERR_UNSUPPORTED, "group key wider than the packed-key limit");
+  qd.key_words = std::max(words, 1);
+  uint64_t cap = 1024;
+  while (cap < 2 * c->group_bound && cap < (1ull << 28)) cap <<= 1;
+  qd.table_slots = uint32_t(cap);
+  return FGPU_OK;
+}
+
+// An aggregate that loads one column as it is (no arithmetic).
+bool plain_load(const QueryDesc& qd, int a) { return qd.aggs[a].prog_len == 1 && qd.prog[qd.aggs[a].prog_off].op == PO_LOAD; }
+
+// fused fast path of k_scan: conjunction of numeric leaves, dense dictionary keys, simple aggregates
+bool fast_path_ok(const Compiled& c, const Switches& w) {
+  const QueryDesc& qd = c.qd;
+  if (w.no_fast || qd.table_mode != TM_DENSE || (qd.n_filter_prog != 0 && qd.filter_kind != FK_AND) || qd.n_leaves > 2 || qd.n_keys > 3)
+    return false;
+  for (int l = 0; l < qd.n_leaves; l++) {
+    const LeafHost& lh = c.leaves[size_t(l)];
+    if (lh.slot >= 0 && (c.slot_types[size_t(lh.slot)] == ST_DICT || lh.null_literal)) return false;
+  }
+  int stored = 0;
+  for (int a = 0; a < qd.n_aggs; a++) {
+    if (qd.aggs[a].func == FGPU_AGG_COUNT) continue;
+    stored++;
+    if (!plain_load(qd, a)) return false;
+  }
+  return stored <= 2;
+}
+
+// k_scan: vector length, ring depth and the per-warp shared-memory layout
+void scan_layout(const Switches& w, Compiled* c) {
+  QueryDesc& qd = c->qd;
+  int vl = w.vl, ring = w.ring;
+  bool any_expr = false;
+  for (int k = 0; k < qd.n_keys; k++)
+    if (qd.keys[k].prog_len) any_expr = true;
+  for (int a = 0; a < qd.n_aggs; a++)
+    if (qd.aggs[a].func != FGPU_AGG_COUNT && !plain_load(qd, a)) any_expr = true;
+  auto r128 = [](size_t x) { return (x + 127) & ~size_t(127); };
+  for (;;) {
+    size_t off = r128(size_t(ring) * 8);
+    size_t slot = r128(size_t(qd.n_stage_plain) * vl * 8 + size_t(qd.n_stage_seeds) * sizeof(Seed));
+    if (slot == 0) slot = 128;
+    qd.slot_bytes = uint32_t(slot);
+    qd.wr_ring = uint32_t(off); off += size_t(ring) * slot;
+    qd.wr_act = uint32_t(off); off = r128(off + size_t(vl / 32) * 4);
+    qd.wr_leaf = uint32_t(off); off = r128(off + ((qd.n_filter_prog > 0 && qd.filter_kind != FK_AND) ? size_t(vl) * 4 : 0));
+    qd.wr_slot = uint32_t(off); off = r128(off + size_t(vl) * 4);
+    qd.wr_keyw = uint32_t(off); off = r128(off + (qd.table_mode == TM_HASH ? size_t(qd.key_words) * vl * 8 : 0));
+    qd.wr_tmp1 = uint32_t(off); off = r128(off + (any_expr ? size_t(vl) * 8 : 0));
+    qd.wr_tmp2 = uint32_t(off); off = r128(off + (any_expr ? size_t(vl) * 16 : 0));
+    qd.wr_acc = uint32_t(off); off = r128(off + size_t(qd.n_aggs) * 32 * 8 + 16 + 32 * 4 + 32 * 4 + (qd.table_mode == TM_HASH ? size_t(qd.key_words) * 32 * 8 : 0));
+    qd.wr_cdesc = uint32_t(off); off = r128(off + size_t(std::max(qd.n_slots, 1)) * sizeof(ChunkDesc));
+    qd.wr_clrt = uint32_t(off); off = r128(off + size_t(std::max(qd.n_leaves, 1)) * sizeof(LeafRt));
+    qd.wr_fplan = uint32_t(off); off = r128(off + 512);
+    qd.wr_iplan = uint32_t(off); off = r128(off + 8 + 16 * size_t(kMaxStagePlain + kMaxStageSeeds));
+    qd.wr_bytes = uint32_t(off);
+    if (size_t(qd.wr_bytes) * (kVecThreads / 32) <= 200 * 1024 || vl == 128) break;
+    vl /= 2;  // many staged columns / wide keys: shorter vectors
+  }
+  qd.vl = vl;
+  qd.n_ring = ring;
+  qd.fast_ok = fast_path_ok(*c, w) ? 1 : 0;
+}
+
+// Resolves the plan against the visible row groups and fills everything of QueryDesc that does
+// not need device memory.  The phases run in this order, and so do their refusals.
+int32_t compile(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, const Switches& w, Compiled* c) {
+  Table& table = ctx->tables[q.table];  // a table without parts scans nothing (empty LSM)
+  for (auto& p : table.parts) {
+    if (p->tx > tx) continue;  // index/lsm.go:416
+    for (auto& rg : p->rgs) {
+      c->rgs.push_back({p.get(), &rg});
+      c->total_rows += rg.n_rows;
+    }
+  }
+  QueryDesc& qd = c->qd;
+  qd.tile_rows = ctx->tile_rows;
+  if (c->rgs.empty()) {  // nothing to scan: no records, exactly like an Iterator over an empty LSM
+    qd.table_mode = TM_DENSE;
+    qd.key_words = 1;
+    qd.table_slots = 1;
+    return FGPU_OK;
+  }
+  Columns k;
+  int32_t rc = resolve_columns(q, table, c, &k);
+  if (rc) return rc;
+  rc = compile_predicate(q, w, k.slot_of, c);
+  if (rc) return rc;
+  prune_row_groups(q, w, q.kind == FGPU_PLAN_FILTER ? std::vector<uint8_t>(c->slot_names.size(), 1) : k.value_slots(q, false), c);
+  rc = make_resident(ctx, table, c);
+  if (rc) return rc;
+  stage_slots(c);
+  std::vector<ProgOp> prog;
+  rc = compile_aggregates(q, k.slot_of, c, &prog);
+  if (rc) return rc;
+  qd.n_rg = int32_t(c->rgs.size());
+  if (q.kind == FGPU_PLAN_FILTER) return project_rows(k, table, c);
+  rc = table_shape(q, k, table, &prog, c);
+  if (rc) return rc;
+  scan_layout(w, c);
   return FGPU_OK;
 }
 
