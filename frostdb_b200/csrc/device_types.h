@@ -205,6 +205,30 @@ struct SeedJob {
   uint32_t n_runs, total, n_chunks, is_def;
 };
 
+// ---- PLAIN string pages interned at upload (intern_strings.cu) ------------------------------------------
+// One column chunk of an intern batch: its PLAIN string values (validated by the host's page walk) and its
+// open-addressing table, power-of-two capacity of at least twice its values.
+struct StrChunk {
+  const uint8_t* bytes;      // the chunk's PLAIN value regions (a copy of the file bytes)
+  const uint32_t* off;       // per value: offset of its 4-byte length prefix in `bytes`
+  unsigned long long* keys;  // per slot: (hash >> 32) << 32 | representative value index; ~0: empty
+  uint32_t* first;           // per slot: smallest value index; after k_str_compact: the slot's rank among the used slots
+  uint32_t* slot;            // per value: its slot
+  uint32_t* out_first;       // k_str_compact: first value index per rank (page-locked host memory)
+  uint32_t n, mask;          // values; capacity - 1
+  uint32_t v0, s0;           // values / slots of the batch's chunks before this one
+};
+
+// One PLAIN string page whose chunk-local indices k_str_codes packs, LSB first, into the hole its page owns.
+struct StrCodeJob {
+  uint8_t* dst;           // the hole: ceil(n / 8) * w bytes (an image offset until the image is resident)
+  const uint32_t* slot;   // per value of the page: its slot
+  const uint32_t* rank;   // per slot of its chunk: rank
+  const uint32_t* code;   // per rank of its chunk: chunk-local index
+  uint32_t n, w;          // values; bits per index (1 .. 24)
+  uint32_t g0, _pad;      // 8-value groups of the launch's jobs before this one
+};
+
 // ---- sorted-run scan (k_runs_tma): the plan shape of compacted parts -----------------------------------
 // Row groups whose filter columns and aggregate inputs are PLAIN non-null int64 and whose group-key
 // columns are run-length only (sorted parts) are scanned by a dedicated kernel that walks the key run

@@ -392,13 +392,211 @@ struct fgpu_result {
 
 namespace {
 
+// Device scratch of one intern batch (intern_plain_strings): the images of the columns it finished hold StrCodeJobs
+// into it until ensure_resident launches them.  Freed in stream order when the batch goes; a finished column whose
+// jobs were never launched (its upload did not happen) is reset to unbuilt, so that it is interned again when needed.
+struct StrBatch {
+  DevBuf scratch;
+  std::vector<std::pair<Part*, std::string>> cols;
+  StrBatch() = default;
+  StrBatch(const StrBatch&) = delete;
+  StrBatch& operator=(const StrBatch&) = delete;
+  ~StrBatch() {
+    for (auto& [part, col] : cols) {
+      ColumnImage& img = part->images[col];
+      if (!img.str_jobs.empty() && !img.resident) img = ColumnImage{};
+    }
+  }
+};
+
+// PLAIN string pages of every listed column that walk_column left walked but not built, interned on the device in one
+// batch (intern_strings.cu): the chunks' PLAIN value regions and offsets go up with one transfer per contiguous span,
+// k_str_hash and k_str_compact leave every distinct value's first occurrence in page-locked memory, and after the one
+// synchronisation the host interns the new strings in order of first occurrence (finish_column), uploads the
+// chunk-local index of every distinct value and queues one StrCodeJob per PLAIN page on the column's image.
+int32_t intern_plain_strings(fgpu_ctx* ctx, Table* table, const std::vector<std::pair<Part*, std::string>>& cols, StrBatch* batch) {
+  struct Item {
+    ChunkWalk* wk;
+    uint64_t v0, s0, cap, byte_off;
+  };
+  std::vector<Item> items;
+  std::vector<std::pair<Part*, std::string>> todo;
+  uint64_t nv = 0, ns = 0;
+  for (const auto& pc : cols) {
+    ColumnImage& img = pc.first->images[pc.second];
+    if (!img.walked || img.built) continue;
+    todo.push_back(pc);
+    for (ChunkWalk& wk : img.walks) {
+      if (!wk.host.error.empty() || wk.str_off.empty()) continue;
+      uint64_t cap = 16;
+      while (cap < 2 * uint64_t(wk.str_off.size())) cap <<= 1;
+      items.push_back({&wk, nv, ns, cap, 0});
+      nv += wk.str_off.size();
+      ns += cap;
+    }
+  }
+  if (todo.empty()) return FGPU_OK;
+  batch->cols.insert(batch->cols.end(), todo.begin(), todo.end());
+  if (ns > 0xffffffffull) return fail(FGPU_ERR_UNSUPPORTED, "PLAIN string values of one upload exceed 2^31");
+  // PLAIN value regions: neighbouring chunks' regions (a few page headers apart) travel as one transfer
+  struct Span { const uint8_t* src; uint64_t len, stage_off; };
+  std::vector<Span> spans;
+  constexpr uint64_t kGap = 4096;
+  uint64_t payload = 0;
+  for (Item& it : items) {
+    const uint8_t* src = it.wk->str_base;
+    const uint64_t len = it.wk->str_span;
+    if (!spans.empty() && src >= spans.back().src + spans.back().len && uint64_t(src - (spans.back().src + spans.back().len)) <= kGap) {
+      spans.back().len = uint64_t(src - spans.back().src) + len;
+    } else {
+      if (!spans.empty()) payload += (spans.back().len + 15) & ~uint64_t(15);
+      spans.push_back({src, len, payload});
+    }
+    it.byte_off = spans.back().stage_off + uint64_t(src - spans.back().src);
+  }
+  if (!spans.empty()) payload += (spans.back().len + 15) & ~uint64_t(15);
+  // scratch: [chunks][counts][offsets][slots][codes][first / rank][keys][payload], 16-byte aligned pieces
+  auto al = [](uint64_t n) { return (n + 15) & ~uint64_t(15); };
+  const uint64_t n = items.size();
+  const uint64_t o_cnt = al(n * sizeof(StrChunk)), o_off = o_cnt + al(n * 4), o_slot = o_off + al(nv * 4), o_code = o_slot + al(nv * 4),
+                 o_first = o_code + al(nv * 4), o_keys = o_first + al(ns * 4), o_pay = o_keys + ns * 8;
+  CUDA_TRY(batch->scratch.alloc(o_pay + payload, ctx->stream));
+  uint8_t* d = static_cast<uint8_t*>(batch->scratch.p);
+  size_t pin_cap = 0;
+  uint8_t* pin = ctx->pinned_take(size_t(nv * 4 + n * 4), &pin_cap);  // first occurrences (written by k_str_compact), counts
+  if (!pin) return fail(FGPU_ERR_OOM, "PLAIN string interning: page-locked result buffer");
+  struct Give { fgpu_ctx* ctx; uint8_t* p; size_t cap; ~Give() { ctx->pinned_give(p, cap); } } give{ctx, pin, pin_cap};
+  uint32_t* h_first = reinterpret_cast<uint32_t*>(pin);
+  uint32_t* h_count = h_first + nv;
+  std::vector<uint8_t> head(o_slot, 0);  // chunk table, zero counts, offsets
+  for (size_t i = 0; i < items.size(); i++) {
+    const Item& it = items[i];
+    StrChunk c{};
+    c.bytes = d + o_pay + it.byte_off;
+    c.off = reinterpret_cast<const uint32_t*>(d + o_off) + it.v0;
+    c.keys = reinterpret_cast<unsigned long long*>(d + o_keys) + it.s0;
+    c.first = reinterpret_cast<uint32_t*>(d + o_first) + it.s0;
+    c.slot = reinterpret_cast<uint32_t*>(d + o_slot) + it.v0;
+    c.out_first = h_first + it.v0;
+    c.n = uint32_t(it.wk->str_off.size());
+    c.mask = uint32_t(it.cap - 1);
+    c.v0 = uint32_t(it.v0);
+    c.s0 = uint32_t(it.s0);
+    std::memcpy(head.data() + i * sizeof(StrChunk), &c, sizeof c);
+    std::memcpy(head.data() + o_off + it.v0 * 4, it.wk->str_off.data(), it.wk->str_off.size() * 4);
+  }
+  auto upload = [&](void* dst, const void* src, size_t bytes) {
+    if (void* p = ctx->arena_take(bytes)) {
+      std::memcpy(p, src, bytes);
+      src = p;
+    }
+    return cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, ctx->stream);
+  };
+  cudaError_t e = upload(d, head.data(), head.size());
+  if (e == cudaSuccess) e = cudaMemsetAsync(d + o_first, 0xff, size_t(o_pay - o_first), ctx->stream);  // first = ~0, keys empty
+  for (const Span& sp : spans) {
+    if (e != cudaSuccess) break;
+    e = cudaMemcpyAsync(d + o_pay + sp.stage_off, sp.src, sp.len, cudaMemcpyHostToDevice, ctx->stream);
+  }
+  const StrChunk* d_chunks = reinterpret_cast<const StrChunk*>(d);
+  uint32_t* d_count = reinterpret_cast<uint32_t*>(d + o_cnt);
+  if (e == cudaSuccess) e = launch_str_hash(d_chunks, uint32_t(n), uint32_t(nv), ctx->stream);
+  if (e == cudaSuccess) e = launch_str_compact(d_chunks, uint32_t(n), uint32_t(ns), d_count, ctx->stream);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(h_count, d_count, n * 4, cudaMemcpyDeviceToHost, ctx->stream);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    return fail(FGPU_ERR_CUDA, std::string("PLAIN string interning: ") + cudaGetErrorString(e));
+  }
+  // first occurrences in ascending order (they name the distinct values), remembering each one's rank
+  std::vector<std::vector<uint32_t>> rank_of(items.size());
+  for (size_t i = 0; i < items.size(); i++) {
+    const uint32_t cnt = h_count[i];
+    std::vector<std::pair<uint32_t, uint32_t>> fr(cnt);
+    for (uint32_t r = 0; r < cnt; r++) fr[r] = {h_first[items[i].v0 + r], r};
+    std::sort(fr.begin(), fr.end());
+    items[i].wk->str_firsts.resize(cnt);
+    rank_of[i].resize(cnt);
+    for (uint32_t k = 0; k < cnt; k++) {
+      items[i].wk->str_firsts[k] = fr[k].first;
+      rank_of[i][k] = fr[k].second;
+    }
+  }
+  // the sections: interning of the new strings, holes for the indices; then the chunk-local index per rank
+  std::vector<uint32_t> codes;
+  std::vector<uint64_t> code0(items.size());
+  for (const auto& [part, col] : todo) finish_column(kIndexRows, table, part, col, /*host_intern=*/false);
+  for (size_t i = 0; i < items.size(); i++) {
+    code0[i] = codes.size();
+    codes.resize(codes.size() + rank_of[i].size());
+    const ChunkWalk& wk = *items[i].wk;
+    if (wk.str_codes.size() != rank_of[i].size()) continue;  // the chunk was refused while its sections were written
+    for (size_t k = 0; k < rank_of[i].size(); k++) codes[code0[i] + rank_of[i][k]] = wk.str_codes[k];
+  }
+  if (!codes.empty()) e = upload(d + o_code, codes.data(), codes.size() * 4);
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    return fail(FGPU_ERR_CUDA, std::string("PLAIN string interning: ") + cudaGetErrorString(e));
+  }
+  size_t i = 0;
+  for (const auto& [part, col] : todo) {
+    ColumnImage& img = part->images[col];
+    for (size_t g = 0; g < img.walks.size(); g++) {
+      const ChunkWalk& wk = img.walks[g];
+      if (i >= items.size() || items[i].wk != &wk) continue;
+      const Item& it = items[i];
+      const uint64_t c0 = code0[i++];
+      if (!img.error.empty()) continue;  // a refused chunk makes the column unreadable: it is never uploaded
+      for (const StrPage& pg : wk.str_pages) {
+        StrCodeJob j{};
+        j.dst = reinterpret_cast<uint8_t*>(uintptr_t(pg.hole));  // image offset: rebased at upload
+        j.slot = reinterpret_cast<const uint32_t*>(d + o_slot) + it.v0 + pg.first;
+        j.rank = reinterpret_cast<const uint32_t*>(d + o_first) + it.s0;
+        j.code = reinterpret_cast<const uint32_t*>(d + o_code) + c0;
+        j.n = pg.n;
+        j.w = wk.str_w;
+        img.str_jobs.push_back(j);
+      }
+    }
+    img.walks.clear();
+  }
+  return FGPU_OK;
+}
+
+// The PLAIN string pages' indices of a column whose image is now at `dev` (queued by intern_plain_strings).
+cudaError_t launch_str_jobs(fgpu_ctx* ctx, ColumnImage& img, void* dev) {
+  if (img.str_jobs.empty()) return cudaSuccess;
+  uint32_t groups = 0;
+  for (StrCodeJob& j : img.str_jobs) {
+    j.dst = static_cast<uint8_t*>(dev) + reinterpret_cast<uintptr_t>(j.dst);
+    j.g0 = groups;
+    groups += (j.n + 7) / 8;
+  }
+  const size_t bytes = img.str_jobs.size() * sizeof(StrCodeJob);
+  DevBuf d_jobs;  // released in stream order
+  cudaError_t e = d_jobs.alloc(bytes, ctx->stream);
+  const void* src = img.str_jobs.data();
+  if (void* pin = ctx->arena_take(bytes)) {
+    std::memcpy(pin, src, bytes);
+    src = pin;
+  }
+  if (e == cudaSuccess) e = cudaMemcpyAsync(d_jobs.p, src, bytes, cudaMemcpyHostToDevice, ctx->stream);
+  if (e == cudaSuccess) e = launch_str_codes(static_cast<const StrCodeJob*>(d_jobs.p), uint32_t(img.str_jobs.size()), groups, ctx->stream);
+  std::vector<StrCodeJob>().swap(img.str_jobs);
+  return e;
+}
+
 // Uploads one column of one part if it is not resident yet: the host-assembled meta region with one
 // copy, the PLAIN value regions straight from the source file (one async copy per contiguous extent),
 // all on the engine stream so that kernels queued behind need no extra synchronisation.
+// A column with PLAIN string values that no caller's intern batch has finished is interned here on its own.
 int32_t ensure_resident(fgpu_ctx* ctx, Table* table, Part* part, const std::string& column, uint64_t* h2d_bytes,
                         double* build_us = nullptr, double* upload_us = nullptr) {
   auto t0 = std::chrono::steady_clock::now();
-  build_column(kIndexRows, table, part, column, /*device_seeds=*/true);
+  walk_column(kIndexRows, table, part, column, /*device_seeds=*/true);
+  StrBatch own;
+  if (!part->images[column].built)
+    if (int32_t rc = intern_plain_strings(ctx, table, {{part, column}}, &own)) return rc;
   auto t1 = std::chrono::steady_clock::now();
   if (build_us) *build_us += std::chrono::duration<double, std::micro>(t1 - t0).count();
   struct Tail {
@@ -465,6 +663,7 @@ int32_t ensure_resident(fgpu_ctx* ctx, Table* table, Part* part, const std::stri
       e = launch_gather_pages(stage.p, dev, reinterpret_cast<const PageCopy*>(static_cast<uint8_t*>(stage.p) + table_off), uint32_t(copies.size()), ctx->stream);
     // `stage` is released in stream order when it goes out of scope
   }
+  if (e == cudaSuccess) e = launch_str_jobs(ctx, img, dev);
   if (e == cudaSuccess) e = launch_make_seeds(dev, img.seed_jobs_off, img.n_seed_jobs, img.max_seed_chunks, ctx->stream);
   if (e != cudaSuccess) {
     cudaFreeAsync(dev, ctx->stream);
@@ -507,7 +706,7 @@ void prebuild_columns(Table* table, Part* part, const std::vector<std::string>& 
       for (;;) {
         const size_t i = next.fetch_add(1);
         if (i >= todo.size()) break;
-        build_column(kIndexRows, table, part, *todo[i], /*device_seeds=*/true);
+        walk_column(kIndexRows, table, part, *todo[i], /*device_seeds=*/true);  // (PLAIN strings: finished after the intern batch)
       }
     });
   for (std::thread& w : workers) w.join();
@@ -1386,18 +1585,38 @@ int32_t make_resident(fgpu_ctx* ctx, Table& table, Compiled* c) {
   }
   // numeric columns first: their bytes are the bulk of the transfer, which then runs while the host
   // assembles the dictionary columns' run directories
+  auto upload = [&](Part* part, const std::string& name) -> int32_t {
+    int32_t rc = ensure_resident(ctx, &table, part, name, &c->h2d_bytes, pc.on ? &build_us : nullptr, pc.on ? &upload_us : nullptr);
+    if (rc) return rc;
+    const ColumnImage& img = part->images[name];
+    if (!img.error.empty()) return fail(FGPU_ERR_UNSUPPORTED, "column " + name + ": " + img.error);
+    return FGPU_OK;
+  };
+  std::vector<std::pair<Part*, std::string>> plain_strings;  // walked, waiting for the intern batch
   for (int pass = 0; pass < 2; pass++) {
     for (auto& [part, read] : reads) {
       for (size_t si = 0; si < c->slot_names.size(); si++) {
         const std::string& name = c->slot_names[si];
         if ((c->slot_types[si] == ST_DICT) != (pass == 1) || !((read >> si) & 1)) continue;
         if (std::find(part->columns.begin(), part->columns.end(), name) == part->columns.end()) continue;
-        int32_t rc = ensure_resident(ctx, &table, part, name, &c->h2d_bytes, pc.on ? &build_us : nullptr, pc.on ? &upload_us : nullptr);
-        if (rc) return rc;
-        const ColumnImage& img = part->images[name];
-        if (!img.error.empty()) return fail(FGPU_ERR_UNSUPPORTED, "column " + name + ": " + img.error);
+        if (pass == 1 && !part->images[name].resident) {
+          const auto tw = std::chrono::steady_clock::now();
+          walk_column(kIndexRows, &table, part, name, /*device_seeds=*/true);
+          if (pc.on) build_us += std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - tw).count();
+          if (!part->images[name].built) {
+            plain_strings.push_back({part, name});
+            continue;
+          }
+        }
+        if (int32_t rc = upload(part, name)) return rc;
       }
     }
+  }
+  if (!plain_strings.empty()) {
+    StrBatch batch;
+    if (int32_t rc = intern_plain_strings(ctx, &table, plain_strings, &batch)) return rc;
+    for (auto& [part, name] : plain_strings)
+      if (int32_t rc = upload(part, name)) return rc;
   }
   if (pc.on && c->h2d_bytes) {
     char buf[128];
@@ -3391,8 +3610,17 @@ int32_t fgpu_part_put_parquet(fgpu_ctx* ctx, const char* table, uint64_t part_id
   if (!open_part(file, len, part.get(), &err)) return fail(FGPU_ERR_PARQUET, err);
   if (!part->borrowed) {
     // The caller may reuse the buffer on return: every column goes to the device now (host images built in
-    // parallel, one worker per column).
+    // parallel, one worker per column; PLAIN string pages interned in one batch).
     prebuild_columns(&t, part.get(), part->columns);
+    StrBatch batch;
+    {
+      std::vector<std::pair<Part*, std::string>> cols;
+      for (const std::string& col : part->columns) cols.push_back({part.get(), col});
+      if (int32_t rc = intern_plain_strings(ctx, &t, cols, &batch)) {
+        free_part(ctx, part.get());
+        return rc;
+      }
+    }
     for (const std::string& col : part->columns) {
       int32_t rc = ensure_resident(ctx, &t, part.get(), col, nullptr);
       if (rc) {
@@ -3994,24 +4222,7 @@ int32_t fgpu_parquet_dict_values(const uint8_t* file, uint64_t len, const char* 
   std::string err;
   if (!parse_parquet(file, len, &pf, &err)) return fail(FGPU_ERR_PARQUET, err);
   GlobalDict d;  // first-seen order over the file's row groups
-  for (size_t c = 0; c < pf.leaves.size(); c++) {
-    if (pf.leaves[c].name != column) continue;
-    for (const RowGroupMeta& rg : pf.row_groups) {
-      const ChunkMeta& cm = rg.chunks[c];
-      if (!cm.error.empty()) return fail(FGPU_ERR_PARQUET, std::string(column) + ": " + cm.error);
-      const uint8_t* p = cm.dict;
-      const uint8_t* end = cm.dict + cm.dict_len;
-      for (uint32_t i = 0; i < cm.dict_num_values; i++) {
-        if (end - p < 4) return fail(FGPU_ERR_PARQUET, "dictionary page truncated");
-        uint32_t l;
-        std::memcpy(&l, p, 4);
-        p += 4;
-        if (l > uint64_t(end - p)) return fail(FGPU_ERR_PARQUET, "dictionary entry overruns page");
-        d.intern(reinterpret_cast<const char*>(p), l);
-        p += l;
-      }
-    }
-  }
+  if (!column_dict_values(pf, column, &d, &err)) return fail(FGPU_ERR_PARQUET, err);
   uint64_t need = 0;
   for (auto& v : d.values) need += 4 + v.size();
   *out_len = need;

@@ -94,9 +94,30 @@ inline uint64_t popcount_range(const std::vector<uint64_t>& bm, uint64_t pos, ui
 
 bool is_dict_encoding(int32_t e) { return e == ENC_RLE_DICTIONARY || e == ENC_PLAIN_DICTIONARY; }
 
-// Builds every section of one column chunk into the image.
-void build_chunk(const ChunkMeta& cm, const SchemaLeaf& leaf, uint32_t n_rows, int tile_rows, GlobalDict* dict,
-                 ImageWriter& w, ChunkHost* out) {
+// Length prefixes of one PLAIN BYTE_ARRAY page holding `n` values: one offset per value, from the chunk's first PLAIN
+// value region.  Every value must lie inside the page and the values must fill it.
+bool walk_plain_strings(const PageInfo& pg, uint32_t n, ChunkWalk* wk, std::string* err) {
+  if (!wk->str_base) wk->str_base = pg.values;
+  const uint64_t base = uint64_t(pg.values - wk->str_base);  // pages are walked in file order
+  if (base + pg.values_len > 0xffffffffull) { *err = "PLAIN string pages of one chunk span more than 4 GiB"; return false; }
+  const uint8_t* q = pg.values;
+  const uint8_t* end = pg.values + pg.values_len;
+  for (uint32_t i = 0; i < n; i++) {
+    if (end - q < 4) { *err = "PLAIN string page shorter than its value count"; return false; }
+    uint32_t l;
+    std::memcpy(&l, q, 4);
+    if (l > uint64_t(end - q) - 4) { *err = "PLAIN string length prefix overruns its page"; return false; }
+    wk->str_off.push_back(uint32_t(base + uint64_t(q - pg.values)));
+    q += 4 + uint64_t(l);
+  }
+  if (q != end) { *err = "PLAIN string page holds more values than its definition levels"; return false; }
+  wk->str_span = uint32_t(base + pg.values_len);
+  return true;
+}
+
+// Walks and validates every page of one column chunk (first half of building it).
+void walk_chunk(const ChunkMeta& cm, const SchemaLeaf& leaf, uint32_t n_rows, ChunkWalk* wk) {
+  ChunkHost* out = &wk->host;
   out->phys = leaf.phys;
   out->stored_bytes = uint64_t(cm.total_compressed_size);
   out->has_minmax = cm.has_minmax;
@@ -120,16 +141,14 @@ void build_chunk(const ChunkMeta& cm, const SchemaLeaf& leaf, uint32_t n_rows, i
     else if (pg.encoding == ENC_PLAIN) any_plain = true;
     else { out->error = "unsupported page encoding " + std::to_string(pg.encoding); return; }
   }
-  if (any_dict && any_plain) { out->error = "column chunk mixes dictionary and PLAIN pages"; return; }
-  if (leaf.phys == PT_BYTE_ARRAY && any_plain) { out->error = "PLAIN byte-array pages are not supported"; return; }
-  const uint32_t T = uint32_t(tile_rows);
-  const uint32_t n_tiles = (n_rows + T - 1) / T;
+  // (a string chunk may hold both: a dictionary whose writer fell back to PLAIN part of the way through)
+  if (any_dict && any_plain && leaf.phys != PT_BYTE_ARRAY) { out->error = "column chunk mixes dictionary and PLAIN pages"; return; }
 
   // ---- definition levels --------------------------------------------------------------------
   std::string err;
-  std::vector<uint8_t> defstream;
-  std::vector<HostRun> defruns;
-  std::vector<uint64_t> valid;  // bitset, only when max_def == 1
+  std::vector<uint8_t>& defstream = wk->defstream;
+  std::vector<HostRun>& defruns = wk->defruns;
+  std::vector<uint64_t>& valid = wk->valid;  // bitset, only when max_def == 1
   std::vector<uint32_t> page_nn(cm.pages.size());
   uint32_t n_values = n_rows;
   bool all_present = false;  // optional column whose definition levels are one run of 1s per page: no bitset needed
@@ -191,16 +210,24 @@ void build_chunk(const ChunkMeta& cm, const SchemaLeaf& leaf, uint32_t n_rows, i
   } else {
     for (size_t p = 0; p < cm.pages.size(); p++) page_nn[p] = cm.pages[p].num_values;
   }
-  const bool has_nulls = (n_values != n_rows);
+  wk->n_values = n_values;
 
   // ---- values -------------------------------------------------------------------------------
-  std::vector<uint8_t> vstream;
-  std::vector<HostRun> vruns;
-  if (any_dict || (!any_plain && leaf.phys == PT_BYTE_ARRAY)) {
+  std::vector<uint8_t>& vstream = wk->vstream;
+  std::vector<HostRun>& vruns = wk->vruns;
+  if (any_dict || leaf.phys == PT_BYTE_ARRAY) {
     uint32_t vo = 0;
     for (size_t p = 0; p < cm.pages.size(); p++) {
       const PageInfo& pg = cm.pages[p];
       if (page_nn[p] == 0) continue;
+      if (pg.encoding == ENC_PLAIN) {  // strings: one bit-packed run whose hole the section writing places here
+        const uint32_t first = uint32_t(wk->str_off.size());
+        if (!walk_plain_strings(pg, page_nn[p], wk, &err)) { out->error = err; return; }
+        wk->str_pages.push_back(StrPage{uint32_t(vruns.size()), first, page_nn[p]});
+        vruns.push_back(HostRun{vo, uint32_t(vstream.size()), 0, 1u});
+        vo += page_nn[p];
+        continue;
+      }
       if (pg.values_len < 1) { out->error = "dictionary-index page without bit width"; return; }
       int bw = pg.values[0];
       if (bw > 32) { out->error = "dictionary index bit width > 32"; return; }
@@ -217,37 +244,121 @@ void build_chunk(const ChunkMeta& cm, const SchemaLeaf& leaf, uint32_t n_rows, i
       const PageInfo& pg = cm.pages[p];
       uint64_t need = uint64_t(page_nn[p]) * 8;
       if (need > pg.values_len) { out->error = "PLAIN page shorter than its value count"; return; }
+      wk->plain64.push_back({pg.values, page_nn[p]});
     }
     out->desc.kind = CK_PLAIN64;
   }
 
   // ---- dictionary ---------------------------------------------------------------------------
-  std::vector<int64_t> dict64;
   uint32_t dict_size = 0;
   if (out->desc.kind == CK_DICT_STR) {
     const uint8_t* p = cm.dict;
     const uint8_t* end = cm.dict + cm.dict_len;
-    out->lut_host.reserve(cm.dict_num_values);
+    wk->dict_entries.reserve(cm.dict_num_values);
     for (uint32_t i = 0; i < cm.dict_num_values; i++) {
       if (end - p < 4) { out->error = "dictionary page truncated"; return; }
       uint32_t l;
       std::memcpy(&l, p, 4);
       p += 4;
       if (l > uint64_t(end - p)) { out->error = "dictionary entry overruns page"; return; }
-      out->lut_host.push_back(dict->intern(reinterpret_cast<const char*>(p), l));
+      wk->dict_entries.push_back({p, l});
       p += l;
     }
     dict_size = cm.dict_num_values;
   } else if (out->desc.kind == CK_DICT64) {
     if (uint64_t(cm.dict_num_values) * 8 > cm.dict_len) { out->error = "numeric dictionary page truncated"; return; }
-    dict64.resize(cm.dict_num_values);
-    std::memcpy(dict64.data(), cm.dict, size_t(cm.dict_num_values) * 8);
+    wk->dict64.resize(cm.dict_num_values);
+    std::memcpy(wk->dict64.data(), cm.dict, size_t(cm.dict_num_values) * 8);
     dict_size = cm.dict_num_values;
   }
   if (out->desc.kind != CK_PLAIN64) {
     for (const HostRun& r : vruns)
       if ((r.meta & 1u) == 0 && r.val >= dict_size) { out->error = "dictionary index out of range"; return; }
-    if (n_values > 0 && dict_size == 0) { out->error = "dictionary-encoded values without a dictionary page"; return; }
+    if (n_values > wk->str_off.size() && dict_size == 0) { out->error = "dictionary-encoded values without a dictionary page"; return; }
+  }
+}
+
+// Packs `n` indices LSB first at `w` bits into `dst` (whole bytes of 8-value groups: ceil(n / 8) * w bytes).
+void pack_bits(const uint32_t* v, uint32_t n, uint32_t w, uint8_t* dst) {
+  uint64_t acc = 0;
+  uint32_t bits = 0;
+  for (uint32_t i = 0; i < (n + 7) / 8 * 8; i++) {
+    acc |= uint64_t(i < n ? v[i] : 0u) << bits;
+    bits += w;
+    while (bits >= 8) {
+      *dst++ = uint8_t(acc);
+      acc >>= 8;
+      bits -= 8;
+    }
+  }
+}
+
+// Writes every section of one walked column chunk into the image (second half of building it).
+void write_chunk(ChunkWalk& wk, uint32_t n_rows, int tile_rows, GlobalDict* dict, bool host_intern, ImageWriter& w, ChunkHost* out) {
+  *out = std::move(wk.host);
+  if (!out->error.empty()) return;
+  const uint32_t T = uint32_t(tile_rows);
+  const uint32_t n_tiles = (n_rows + T - 1) / T;
+  const uint32_t n_values = wk.n_values;
+  const bool has_nulls = (n_values != n_rows);
+  const std::vector<uint64_t>& valid = wk.valid;
+  std::vector<uint8_t>& defstream = wk.defstream;
+  std::vector<HostRun>& defruns = wk.defruns;
+  std::vector<uint8_t>& vstream = wk.vstream;
+  std::vector<HostRun>& vruns = wk.vruns;
+  std::vector<int64_t>& dict64 = wk.dict64;
+
+  // ---- chunk-local string dictionary: the dictionary page, then the PLAIN values not in it, in order of first occurrence ----
+  uint32_t dict_size = uint32_t(dict64.size());
+  if (out->desc.kind == CK_DICT_STR) {
+    ChunkInterner in(dict, &out->lut_host);
+    out->lut_host.reserve(wk.dict_entries.size());
+    for (const auto& e : wk.dict_entries) in.entry(reinterpret_cast<const char*>(e.first), e.second);
+    std::vector<uint32_t> codes;  // host: per PLAIN value; device: per distinct PLAIN value (str_firsts)
+    if (host_intern) {
+      codes.reserve(wk.str_off.size());
+      for (uint32_t i = 0; i < uint32_t(wk.str_off.size()); i++) {
+        const std::string_view s = plain_string(wk, i);
+        codes.push_back(in.add(s.data(), s.size()));
+      }
+    } else {
+      codes.reserve(wk.str_firsts.size());
+      for (uint32_t f : wk.str_firsts) {
+        const std::string_view s = plain_string(wk, f);
+        codes.push_back(in.add(s.data(), s.size()));
+      }
+    }
+    dict_size = uint32_t(out->lut_host.size());
+    if (dict_size > (1u << 24)) { out->error = "PLAIN string values need a chunk dictionary of more than 2^24 entries"; return; }
+    // holes for the PLAIN pages' indices, at the stream positions their pages held
+    if (!wk.str_pages.empty()) {
+      uint32_t bw = 1;
+      while ((uint64_t(1) << bw) < dict_size) bw++;
+      wk.str_w = bw;
+      std::vector<uint8_t> vs;
+      uint32_t src = 0, shift = 0;
+      size_t sp = 0;
+      for (size_t k = 0; k < vruns.size(); k++) {
+        HostRun& r = vruns[k];
+        if (sp < wk.str_pages.size() && wk.str_pages[sp].run == k) {
+          StrPage& pg = wk.str_pages[sp++];
+          vs.insert(vs.end(), vstream.begin() + src, vstream.begin() + r.off);
+          src = r.off;
+          r.off = uint32_t(vs.size());
+          r.meta = 1u | (bw << 8);
+          pg.hole = r.off;  // relative to the section until it is written
+          const uint32_t bytes = (pg.n + 7) / 8 * bw;
+          vs.resize(vs.size() + bytes, 0);
+          if (host_intern) pack_bits(codes.data() + pg.first, pg.n, bw, vs.data() + r.off);
+          shift += bytes;
+        } else if (r.meta & 1u) {
+          r.off += shift;
+        }
+      }
+      vs.insert(vs.end(), vstream.begin() + src, vstream.end());
+      vstream.swap(vs);
+    }
+    if (!host_intern) wk.str_codes = std::move(codes);
   }
 
   // ---- RLE run values of string dictionaries become global ids (no LUT hop for run-length data) ----
@@ -305,14 +416,15 @@ void build_chunk(const ChunkMeta& cm, const SchemaLeaf& leaf, uint32_t n_rows, i
   if (out->desc.kind == CK_PLAIN64) {
     // value regions go to the device straight from the file: negative offsets mark "extent region"
     const uint64_t eoff = w.begin_extent();
-    for (size_t p = 0; p < cm.pages.size(); p++) {
-      w.add_extent(cm.pages[p].values, uint64_t(page_nn[p]) * 8);
-      plain_bytes += uint64_t(page_nn[p]) * 8;
+    for (const auto& pg : wk.plain64) {
+      w.add_extent(pg.first, uint64_t(pg.second) * 8);
+      plain_bytes += uint64_t(pg.second) * 8;
     }
     w.end_extent();
     out->off_values = -int64_t(eoff) - 1;
   } else {
     out->off_values = w.section(vstream.data(), vstream.size());
+    for (StrPage& pg : wk.str_pages) pg.hole += uint64_t(out->off_values);
   }
   uint64_t val0_off = ~0ull;
   if (w.device_seeds && has_nulls) val0_off = uint64_t(w.section(chunk_val0.data(), chunk_val0.size() * 4));
@@ -485,30 +597,64 @@ bool open_part(const uint8_t* file, uint64_t len, Part* part, std::string* err) 
   return true;
 }
 
-void build_column(int index_rows, Table* table, Part* part, const std::string& column, bool device_seeds) {
+void walk_column(int index_rows, Table* table, Part* part, const std::string& column, bool device_seeds) {
   ColumnImage& img = part->images[column];
-  if (img.built) return;
-  img.built = true;
+  if (img.built || img.walked) return;
+  img.walked = true;
+  img.device_seeds = device_seeds;
   size_t leaf = part->pf.leaves.size();
   for (size_t c = 0; c < part->pf.leaves.size(); c++)
     if (part->pf.leaves[c].name == column) leaf = c;
-  if (leaf == part->pf.leaves.size()) { img.error = "column not in part"; return; }
+  if (leaf == part->pf.leaves.size()) {
+    img.error = "column not in part";
+    img.built = true;
+    return;
+  }
   const SchemaLeaf& sl = part->pf.leaves[leaf];
-  GlobalDict* dict = (sl.phys == PT_BYTE_ARRAY) ? &table->dicts[column] : nullptr;
-  ImageWriter w(img.meta, img.extents);
-  w.device_seeds = device_seeds;
+  img.walks.resize(part->rgs.size());
+  bool plain_strings = false;
   size_t g = 0;
   for (RowGroupMeta& rg : part->pf.row_groups) {
     if (rg.num_rows == 0) continue;
-    RowGroupHost& h = part->rgs[g++];
-    ChunkHost ch;
+    ChunkWalk& wk = img.walks[g];
     walk_chunk_pages(part->file, part->file_bytes, sl, rg.num_rows, &rg.chunks[leaf]);  // first touch of this chunk
-    build_chunk(rg.chunks[leaf], sl, h.n_rows, index_rows, dict, w, &ch);
+    walk_chunk(rg.chunks[leaf], sl, part->rgs[g].n_rows, &wk);
+    if (!wk.host.error.empty() && img.error.empty()) img.error = wk.host.error;
+    plain_strings = plain_strings || (wk.host.error.empty() && !wk.str_off.empty());
+    g++;
+  }
+  if (!plain_strings || !img.error.empty()) {
+    finish_column(index_rows, table, part, column, /*host_intern=*/true);
+    img.walks.clear();
+  }
+}
+
+void finish_column(int index_rows, Table* table, Part* part, const std::string& column, bool host_intern) {
+  ColumnImage& img = part->images[column];
+  if (img.built) return;
+  img.built = true;
+  GlobalDict* dict = nullptr;
+  for (const SchemaLeaf& l : part->pf.leaves)
+    if (l.name == column && l.phys == PT_BYTE_ARRAY) dict = &table->dicts[column];
+  ImageWriter w(img.meta, img.extents);
+  w.device_seeds = img.device_seeds;
+  for (size_t g = 0; g < part->rgs.size(); g++) {
+    RowGroupHost& h = part->rgs[g];
+    ChunkHost ch;
+    write_chunk(img.walks[g], h.n_rows, index_rows, dict, host_intern, w, &ch);
     if (!ch.error.empty() && img.error.empty()) img.error = ch.error;
     ch.bloom = std::move(h.cols[column].bloom);  // (footer-level fact of the skeleton the built chunk replaces)
     h.cols[column] = std::move(ch);
   }
   finish_image(w, img, part, column);
+}
+
+void build_column(int index_rows, Table* table, Part* part, const std::string& column, bool device_seeds) {
+  walk_column(index_rows, table, part, column, device_seeds);
+  ColumnImage& img = part->images[column];
+  if (img.built) return;
+  finish_column(index_rows, table, part, column, /*host_intern=*/true);
+  img.walks.clear();
 }
 
 namespace {
@@ -631,16 +777,10 @@ bool build_arrow_column(Table* table, Part* part, const std::string& name, const
     } else {
       const int32_t* soff = static_cast<const int32_t*>(ca->buffers[1]) + off;
       const char* sbytes = static_cast<const char*>(ca->buffers[2]);
-      std::unordered_map<std::string, uint32_t> local;
+      ChunkInterner in(gd, &ch.lut_host);
       for (uint32_t i = 0; i < n_rows; i++) {
         if (!valid_at(i)) continue;
-        std::string v(sbytes ? sbytes + soff[i] : "", size_t(soff[i + 1] - soff[i]));
-        auto it = local.find(v);
-        if (it == local.end()) {
-          it = local.emplace(v, uint32_t(ch.lut_host.size())).first;
-          ch.lut_host.push_back(gd->intern(v.data(), v.size()));
-        }
-        idx.push_back(it->second);
+        idx.push_back(in.add(sbytes ? sbytes + soff[i] : "", size_t(soff[i + 1] - soff[i])));
       }
     }
     ch.desc.dict_size = uint32_t(ch.lut_host.size());
@@ -722,6 +862,43 @@ void patch_column_pointers(Part* part, const std::string& column, const uint8_t*
       c.desc.row_seeds = nullptr;
     }
   }
+}
+
+bool column_dict_values(const ParsedFile& pf, const std::string& column, GlobalDict* d, std::string* err) {
+  for (size_t c = 0; c < pf.leaves.size(); c++) {
+    if (pf.leaves[c].name != column) continue;
+    for (const RowGroupMeta& rg : pf.row_groups) {
+      const ChunkMeta& cm = rg.chunks[c];
+      if (!cm.error.empty()) { *err = column + ": " + cm.error; return false; }
+      bool plain_strings = false;
+      for (const PageInfo& pg : cm.pages) plain_strings = plain_strings || (pf.leaves[c].phys == PT_BYTE_ARRAY && pg.encoding == ENC_PLAIN);
+      if (plain_strings) {  // the page walk validates the dictionary page and the PLAIN values
+        ChunkWalk wk;
+        walk_chunk(cm, pf.leaves[c], uint32_t(rg.num_rows), &wk);
+        if (!wk.host.error.empty()) { *err = column + ": " + wk.host.error; return false; }
+        std::vector<uint32_t> lut;
+        ChunkInterner in(d, &lut);
+        for (const auto& e : wk.dict_entries) in.entry(reinterpret_cast<const char*>(e.first), e.second);
+        for (uint32_t i = 0; i < uint32_t(wk.str_off.size()); i++) {
+          const std::string_view s = plain_string(wk, i);
+          in.add(s.data(), s.size());
+        }
+        continue;
+      }
+      const uint8_t* p = cm.dict;
+      const uint8_t* end = cm.dict + cm.dict_len;
+      for (uint32_t i = 0; i < cm.dict_num_values; i++) {
+        if (end - p < 4) { *err = "dictionary page truncated"; return false; }
+        uint32_t l;
+        std::memcpy(&l, p, 4);
+        p += 4;
+        if (l > uint64_t(end - p)) { *err = "dictionary entry overruns page"; return false; }
+        d->intern(reinterpret_cast<const char*>(p), l);
+        p += l;
+      }
+    }
+  }
+  return true;
 }
 
 // ---- host-only description (tests without a GPU) ---------------------------------------------------

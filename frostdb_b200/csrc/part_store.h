@@ -3,9 +3,11 @@
 // already laid out in HBM for the scan kernel.
 #pragma once
 #include <cstdint>
+#include <cstring>
 #include <map>
 #include <memory>
 #include <string>
+#include <string_view>
 #include <unordered_map>
 #include <vector>
 
@@ -32,6 +34,35 @@ struct GlobalDict {
   }
   uint32_t cardinality() const { return uint32_t(values.size()); }
   const std::string& value(uint32_t id) const { return values[id]; }
+};
+
+// Chunk-local dictionary of one string chunk, in order of first occurrence, each new entry interned into the table's
+// GlobalDict.  The host's one reference interner: Arrow string arrays, PLAIN string pages built without a device, and
+// the distinct PLAIN values the device's intern batch found (fed in order of first occurrence, so the result is the
+// same).  Keys alias the source bytes, which outlive the interner.
+struct ChunkInterner {
+  GlobalDict* gd;
+  std::vector<uint32_t>* lut;  // chunk-local index -> global id
+  std::vector<std::pair<std::string_view, uint32_t>> entries;  // dictionary page entries, hashed on the first add() only
+  std::unordered_map<std::string_view, uint32_t> local;
+  ChunkInterner(GlobalDict* g, std::vector<uint32_t>* l) : gd(g), lut(l) {}
+  // a dictionary page entry: its own chunk-local index, numbered as the page numbers it
+  void entry(const char* p, size_t n) {
+    entries.push_back({std::string_view(p, n), uint32_t(lut->size())});
+    lut->push_back(gd->intern(p, n));
+  }
+  // a value: its chunk-local index; a value not seen before is appended
+  uint32_t add(const char* p, size_t n) {
+    for (const auto& e : entries) local.emplace(e.first, e.second);  // (a repeated entry keeps its first index)
+    entries.clear();
+    const std::string_view s(p, n);
+    auto it = local.find(s);
+    if (it != local.end()) return it->second;
+    const uint32_t idx = uint32_t(lut->size());
+    local.emplace(s, idx);
+    lut->push_back(gd->intern(p, n));
+    return idx;
+  }
 };
 
 struct ChunkHost {
@@ -78,8 +109,51 @@ struct Extent {
   uint64_t dst_off;  // offset inside the column image
 };
 
+// One PLAIN BYTE_ARRAY page of a chunk: its values become one bit-packed run of chunk-local indices, whose payload
+// is a hole in the value-stream section (zero until the indices are written into it).
+struct StrPage {
+  uint32_t run;       // its entry in the chunk's value directory
+  uint32_t first, n;  // its non-null values: ordinals [first, first + n) among the chunk's PLAIN values
+  uint64_t hole = 0;  // once the sections are written: image offset of its ceil(n / 8) * w index bytes
+};
+
+// What the page walk of one chunk leaves for the section writing (the two halves of building a column).
+struct ChunkWalk {
+  ChunkHost host;                 // footer facts, kind, error
+  std::vector<uint8_t> defstream;
+  std::vector<HostRun> defruns;
+  std::vector<uint64_t> valid;    // bitset of the non-null rows (nullable chunks that are not all present)
+  uint32_t n_values = 0;
+  std::vector<uint8_t> vstream;   // dictionary-index pages, without the PLAIN pages' holes
+  std::vector<HostRun> vruns;     // a PLAIN page's entry holds its hole's position in `vstream` until the holes exist
+  std::vector<std::pair<const uint8_t*, uint32_t>> dict_entries;  // string dictionary page, validated
+  std::vector<int64_t> dict64;
+  std::vector<std::pair<const uint8_t*, uint32_t>> plain64;  // PLAIN int64 / double pages: value region, values
+  // PLAIN string values, validated: every length prefix and its bytes lie inside their page
+  const uint8_t* str_base = nullptr;  // value region of the first PLAIN page
+  uint32_t str_span = 0;              // bytes from str_base to the end of the last PLAIN page's value region
+  std::vector<uint32_t> str_off;      // per PLAIN value: offset of its length prefix from str_base
+  std::vector<StrPage> str_pages;
+  // intern result: the first ordinal of every distinct PLAIN value, ascending (left by the device's intern batch;
+  // empty: the host interns row by row), and after the section writing the chunk-local index of each of them
+  std::vector<uint32_t> str_firsts, str_codes;
+  uint32_t str_w = 0;  // bit width of the PLAIN pages' indices
+};
+
+// PLAIN string value `i` of a walked chunk.
+inline std::string_view plain_string(const ChunkWalk& wk, uint32_t i) {
+  const uint8_t* p = wk.str_base + wk.str_off[i];
+  uint32_t l;
+  std::memcpy(&l, p, 4);
+  return std::string_view(reinterpret_cast<const char*>(p + 4), l);
+}
+
 // Device residency of one column of one part (all its row groups in one allocation).
 struct ColumnImage {
+  bool walked = false;     // page walk done (`walks` holds it until the sections are written)
+  bool device_seeds = false;
+  std::vector<ChunkWalk> walks;  // per row group, between the walk and the section writing
+  std::vector<StrCodeJob> str_jobs;  // PLAIN string pages whose indices the device writes at upload (dst: image offset)
   bool built = false;      // host side done (ChunkHosts filled, dictionary interned)
   bool resident = false;   // bytes are on the device
   void* dev = nullptr;
@@ -122,7 +196,23 @@ bool open_part(const uint8_t* file, uint64_t len, Part* part, std::string* err);
 // LUTs into `image.meta`, PLAIN value regions as extents.  Interns dictionary entries into `table`.
 // ChunkDesc pointers are offsets until patch_column_pointers() is called.
 // device_seeds: leave the cursor seeds to k_make_seeds (ColumnImage::seed_jobs_*) instead of building them here.
+// PLAIN string pages are interned here on the host, row by row (ChunkInterner), and their indices packed by the host.
 void build_column(int index_rows, Table* table, Part* part, const std::string& column, bool device_seeds = false);
+
+// build_column in two halves, with the device's intern batch between them:
+// walk_column walks every chunk's pages and validates them.  A column without PLAIN string values, or with an
+// unreadable chunk, is finished at once (the host interns whatever PLAIN strings it has); otherwise it stays walked
+// but not built, its ChunkWalks waiting for str_firsts.
+void walk_column(int index_rows, Table* table, Part* part, const std::string& column, bool device_seeds);
+// finish_column writes every chunk's sections.  host_intern == false: every chunk with PLAIN string values carries its
+// str_firsts; their chunk-local indices come back in str_codes and the holes are left for the device (StrPage::hole).
+// The walks are kept until the caller clears them.
+void finish_column(int index_rows, Table* table, Part* part, const std::string& column, bool host_intern);
+
+// The distinct strings of one column of a parsed Parquet file (pages walked), in the order a put of the file interns
+// them: per row group the dictionary page, then the PLAIN pages' values not in it, in order of first occurrence.
+// Returns false on a chunk whose dictionary page or PLAIN string pages cannot be read.
+bool column_dict_values(const ParsedFile& pf, const std::string& column, GlobalDict* out, std::string* err);
 
 // L0 Arrow-record part (parts/arrow.go:14-55): one row group holding the record's rows.  Every column image
 // is built here (the record is released by the caller afterwards): int64 / float64 arrays become PLAIN
