@@ -14,7 +14,9 @@
 //                  counters), then compacts the FOLD of the n mailbox slots into the result columns: wait, merge and
 //                  finalize are one launch;
 //   k_comm_wait + k_merge_dense  the same in two launches for the plans without an execution cache (the final table is
-//                  written back; hash tables go through k_merge per rank, kernels.cu).
+//                  written back; hash tables go through k_merge per rank, kernels.cu).  Dense tables have the same
+//                  shape on every rank, which k_comm_wait checks; a hash table is sized from its rank's own rows, so
+//                  the host reads the pushed byte counts behind the wait and sizes the merge table from them.
 // Double buffering by sequence parity is enough: a rank can only push sequence k + 2 after it merged k + 1, which
 // needed every peer's push k + 1, which every peer enqueued behind its own merge of k.
 #include <cuda_runtime.h>
@@ -78,7 +80,7 @@ __global__ void k_comm_wait(CommWait w) {
       __nanosleep(200);
       if (global_timer_ns() - t0 > w.timeout_ns) { timeout = true; break; }
     }
-    if (!timeout && w.flags[2 * r + 1] != w.bytes) mismatch = true;
+    if (!timeout && w.bytes != 0 && w.flags[2 * r + 1] != w.bytes) mismatch = true;
   }
   if (timeout) atomicExch(w.counters + 3, 1ull);
   else if (mismatch) atomicExch(w.counters + 3, 2ull);

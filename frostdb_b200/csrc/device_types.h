@@ -457,7 +457,7 @@ struct CommPush {
 };
 struct CommWait {
   const unsigned long long* flags;     // this rank's flags of the current set: {seq, bytes} per rank
-  unsigned long long seq, bytes, timeout_ns;
+  unsigned long long seq, bytes, timeout_ns;  // bytes: what every rank must have pushed (dense tables); 0: no check
   unsigned long long* counters;        // the query's counters: [3] = 1 timeout, 2 table shapes differ
   int32_t n, _pad;
 };

@@ -1746,6 +1746,15 @@ int32_t project_rows(const Columns& k, Table& table, Compiled* c) {
   return FGPU_OK;
 }
 
+// Hash-table slots for `groups` groups: the smallest power of two >= groups, from kMinHashSlots up to kMaxHashSlots
+// (beyond that a scan or a merge reports an overflow).
+constexpr uint64_t kMinHashSlots = 1024, kMaxHashSlots = 1ull << 28;
+uint32_t hash_slots(uint64_t groups) {
+  uint64_t cap = kMinHashSlots;
+  while (cap < groups && cap < kMaxHashSlots) cap <<= 1;
+  return uint32_t(cap);
+}
+
 // Group keys (dictionary and int64 columns, and computed int64 keys, whose programs follow the aggregates' in qd.prog)
 // and the aggregate table: dense over the dictionary ids when every key is a dictionary column and the product of
 // their radices is at most kDenseMax, a hash table of packed keys otherwise.
@@ -1816,9 +1825,7 @@ int32_t table_shape(const QueryPlan& q, const Columns& k, Table& table, std::vec
   }
   if (words > kMaxKeyWords) return fail(FGPU_ERR_UNSUPPORTED, "group key wider than the packed-key limit");
   qd.key_words = std::max(words, 1);
-  uint64_t cap = 1024;
-  while (cap < 2 * c->group_bound && cap < (1ull << 28)) cap <<= 1;
-  qd.table_slots = uint32_t(cap);
+  qd.table_slots = hash_slots(2 * c->group_bound);
   return FGPU_OK;
 }
 
@@ -1995,7 +2002,7 @@ int32_t comm_wait_merge(fgpu_ctx* ctx, const QueryDesc& qd, void* table, uint64_
   CommWait w{};
   w.flags = reinterpret_cast<const unsigned long long*>(cm.mailbox + cm.flag_off(set, 0));
   w.seq = seq;
-  w.bytes = bytes;
+  w.bytes = qd.table_mode == TM_DENSE ? bytes : 0;  // hash tables: sized per rank, checked by hash_partial_slots
   w.timeout_ns = comm_timeout_ns();
   w.counters = qd.counters;
   w.n = cm.n;
@@ -2014,6 +2021,29 @@ int32_t comm_wait_merge(fgpu_ctx* ctx, const QueryDesc& qd, void* table, uint64_
 int32_t comm_check(unsigned long long code) {
   if (code == 1) return fail(FGPU_ERR_CUDA, "collective Execute: a peer did not deliver its partial table within the timeout");
   if (code == 2) return fail(FGPU_ERR_UNSUPPORTED, "collective Execute: partial table shapes differ between ranks (dictionaries not preloaded identically?)");
+  return FGPU_OK;
+}
+
+// Hash mode: a rank sizes its partial table from its own visible rows, so the ranks' tables differ in size.  Behind
+// the wait, each rank's pushed byte count is read from the flags of this set (one copy, one synchronisation); it must
+// be this plan's table_layout at a power-of-two slot count, whose slot count goes to src_slots[r].
+int32_t hash_partial_slots(fgpu_ctx* ctx, const QueryDesc& qd, uint64_t seq, uint32_t* src_slots) {
+  Comm& cm = ctx->comm;
+  CUDA_TRY(ctx->ensure_scratch(size_t(kMaxRanks) * 16));
+  unsigned long long* flags = reinterpret_cast<unsigned long long*>(ctx->scratch);
+  CUDA_TRY(cudaMemcpyAsync(flags, cm.mailbox + cm.flag_off(seq & 1u, 0), size_t(cm.n) * 16, cudaMemcpyDeviceToHost, ctx->stream));
+  CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+  for (int r = 0; r < cm.n; r++) {
+    if (flags[2 * r] < seq) return comm_check(1);  // k_comm_wait gave up on this peer
+    src_slots[r] = 0;
+    for (uint64_t S = kMinHashSlots; S <= kMaxHashSlots && !src_slots[r]; S <<= 1) {
+      QueryDesc q = qd;
+      q.table_slots = uint32_t(S);
+      size_t off_aggs, off_tags, off_keys;
+      if (((table_layout(q, &off_aggs, &off_tags, &off_keys) + 15) & ~size_t(15)) == flags[2 * r + 1]) src_slots[r] = uint32_t(S);
+    }
+    if (!src_slots[r]) return comm_check(2);
+  }
   return FGPU_OK;
 }
 
@@ -3486,16 +3516,26 @@ int32_t collective_end(fgpu_ctx* ctx, fgpu_result* res) {
   int32_t rc = comm_wait_merge(ctx, qd, res->table.p, res->pending_seq, res->pending_bytes);
   if (rc) return rc;
   FinalizeDesc& fd = res->fd;
-  if (qd.table_mode != TM_DENSE) {  // hash tables: fold every rank's slot into a fresh table
-    DevBuf merged;
-    CUDA_TRY(merged.alloc(res->table_bytes + 128, s));
+  if (qd.table_mode != TM_DENSE) {  // hash tables: fold every rank's slot, at its own size, into a fresh table
+    uint32_t src_slots[kMaxRanks];
+    if (int32_t rcs = hash_partial_slots(ctx, qd, res->pending_seq, src_slots)) return rcs;
+    uint64_t total = 0;
+    for (int r = 0; r < ctx->comm.n; r++) total += src_slots[r];
     QueryDesc q2 = qd;
+    q2.table_slots = hash_slots(total);
+    size_t off_aggs, off_tags, off_keys;
+    const size_t tbytes = table_layout(q2, &off_aggs, &off_tags, &off_keys);
+    DevBuf merged;
+    CUDA_TRY(merged.alloc(tbytes + 128, s));
     bind_table(&q2, static_cast<uint8_t*>(merged.p));
     CUDA_TRY(launch_table_init(q2, s, /*zero_counters=*/false));
-    for (int r = 0; r < ctx->comm.n; r++) CUDA_TRY(launch_merge(q2, ctx->comm.mailbox + ctx->comm.data_off(res->pending_seq & 1u, r), s));
+    for (int r = 0; r < ctx->comm.n; r++)
+      CUDA_TRY(launch_merge(q2, ctx->comm.mailbox + ctx->comm.data_off(res->pending_seq & 1u, r), src_slots[r], s));
     std::swap(res->table.p, merged.p);
     std::swap(res->table.n, merged.n);
+    res->table_bytes = tbytes;
     qd = q2;
+    fd.table_slots = qd.table_slots;
     bind_finalize(&fd, qd);
   }
   if (res->cnt_ptr) {  // count the groups of the final table behind the merge
@@ -3868,19 +3908,25 @@ int32_t fgpu_result_merge_partials(fgpu_ctx* ctx, fgpu_result* r, const void* ga
   if (n > 0) {
     if (!gathered) return fail(FGPU_ERR_INVALID, "null gathered buffer");
     if (nbytes != r->table_bytes) return fail(FGPU_ERR_INVALID, "partial table size differs between ranks (dictionaries not preloaded identically?)");
-    // Start from an empty table and fold every rank's partial in, this rank's own included.
-    DevBuf merged;
-    CUDA_TRY(merged.alloc(r->table_bytes, ctx->stream));
+    // Start from an empty table and fold every rank's partial in, this rank's own included.  A hash table takes the
+    // groups of n partials: it is sized for n times this rank's slots.
     QueryDesc qd = r->qd;
+    const uint32_t src_slots = qd.table_slots;
+    if (qd.table_mode != TM_DENSE) qd.table_slots = hash_slots(uint64_t(n) * src_slots);
+    size_t off_aggs, off_tags, off_keys;
+    const size_t tbytes = table_layout(qd, &off_aggs, &off_tags, &off_keys);
+    DevBuf merged;
+    CUDA_TRY(merged.alloc(tbytes, ctx->stream));
     bind_table(&qd, static_cast<uint8_t*>(merged.p));
     CUDA_TRY(launch_table_init(qd, ctx->stream));
     for (int32_t i = 0; i < n; i++) {
-      CUDA_TRY(launch_merge(qd, static_cast<const uint8_t*>(gathered) + size_t(i) * nbytes, ctx->stream));
+      CUDA_TRY(launch_merge(qd, static_cast<const uint8_t*>(gathered) + size_t(i) * nbytes, src_slots, ctx->stream));
       r->stats.kernel_launches++;
     }
     // the result now lives in the merged table; its groups are counted right behind the merges so that
     // finalisation needs one host round trip less
     FinalizeDesc& fd = r->fd;
+    fd.table_slots = qd.table_slots;
     bind_finalize(&fd, qd);
     if (r->cnt_ptr) {
       CUDA_TRY(cudaMemsetAsync(r->cnt_ptr, 0, 16, ctx->stream));
@@ -3898,6 +3944,7 @@ int32_t fgpu_result_merge_partials(fgpu_ctx* ctx, fgpu_result* r, const void* ga
     }
     std::swap(r->table.p, merged.p);
     std::swap(r->table.n, merged.n);
+    r->table_bytes = tbytes;
     r->qd = qd;
   }
   return finalize_result(ctx, r);

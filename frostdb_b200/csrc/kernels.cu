@@ -1830,11 +1830,12 @@ __global__ void k_finalize(FinalizeDesc f) {
 }
 
 // ======================================================================================================
-// k_merge: fold one remote partial table (same QueryDesc shape) into the local one.
+// k_merge: fold one remote partial table (same QueryDesc shape, S source slots) into the local one.  Hash-mode
+// tables of different ranks may differ in S (each rank sizes its table from its own rows); a dense table has the
+// local table's S.
 // Partial layout (position independent): [rows u64 x S][stored agg i64 x S]...[tags u32 x S (8-aligned)][keys u64 x S*W]
 // ======================================================================================================
-__global__ void k_merge(QueryDesc q, const uint8_t* __restrict__ partial) {
-  const size_t S = q.table_slots;
+__global__ void k_merge(QueryDesc q, const uint8_t* __restrict__ partial, size_t S) {
   const unsigned long long* p_rows = reinterpret_cast<const unsigned long long*>(partial);
   const long long* p_agg = reinterpret_cast<const long long*>(partial + S * 8);
   int n_stored = 0;
@@ -2063,8 +2064,8 @@ cudaError_t launch_finalize_dense(const DenseOut& f, cudaStream_t st) {
   return cudaGetLastError();
 }
 
-cudaError_t launch_merge(const QueryDesc& q, const void* partial, cudaStream_t st) {
-  k_merge<<<grid_for(q.table_slots), 256, 0, st>>>(q, static_cast<const uint8_t*>(partial));
+cudaError_t launch_merge(const QueryDesc& q, const void* partial, size_t src_slots, cudaStream_t st) {
+  k_merge<<<grid_for(src_slots), 256, 0, st>>>(q, static_cast<const uint8_t*>(partial), src_slots);
   return cudaGetLastError();
 }
 

@@ -53,7 +53,7 @@ cudaError_t launch_comm_wait(const CommWait& w, cudaStream_t st);
 cudaError_t launch_merge_dense(const QueryDesc& q, const CommMerge& m, cudaStream_t st);
 cudaError_t launch_rows(const QueryDesc* d_q, const QueryDesc& q, int sm_count, cudaStream_t st);
 cudaError_t launch_finalize(const FinalizeDesc& f, cudaStream_t st);
-cudaError_t launch_merge(const QueryDesc& q, const void* partial, cudaStream_t st);
+cudaError_t launch_merge(const QueryDesc& q, const void* partial, size_t src_slots, cudaStream_t st);
 cudaError_t launch_finalize_dense(const DenseOut& f, cudaStream_t st);
 cudaError_t launch_gather_pages(const void* stage, void* image, const PageCopy* table, uint32_t n, cudaStream_t st);
 cudaError_t launch_make_seeds(void* image, uint64_t jobs_off, uint32_t n_jobs, uint32_t max_chunks, cudaStream_t st);

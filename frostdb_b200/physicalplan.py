@@ -230,9 +230,12 @@ def _eval_post(e: lp.Expr, r: pa.RecordBatch):
                 if is_float:
                     out = np.where(mask, 0.0, a / np.where(mask, 1.0, b))
                 else:
-                    bb = np.where(mask, 1, b)
-                    qv = np.abs(a) // np.abs(bb)
-                    out = np.where((a < 0) != (bb < 0), -qv, qv).astype(np.int64)
+                    # floor division corrected toward zero; a divisor of -1 negates (INT64_MIN / -1 wraps to
+                    # INT64_MIN), so no quotient leaves int64 on the way (abs(INT64_MIN) would)
+                    bb = np.where(mask | (b == -1), 1, b)
+                    qv = a // bb
+                    qv = qv + (((a % bb) != 0) & ((a < 0) != (bb < 0)))
+                    out = np.where(b == -1, np.int64(0) - a, qv).astype(np.int64)
         return e.Name(), pa.array(out, mask=mask if mask is not None and mask.any() else None)
     name = e.Name()
     idx = r.schema.get_field_index(name)

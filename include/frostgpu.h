@@ -260,11 +260,15 @@ int32_t fgpu_parquet_dict_values(const uint8_t* file, uint64_t len, const char* 
                                  uint8_t* buf, uint64_t cap, uint64_t* out_len, uint32_t* out_count);
 
 /* Scan only.  `*dev_ptr` is a DEVICE pointer to a position-independent partial table of
- * `*nbytes` bytes (same size on every rank for the same query + unified dictionaries). */
+ * `*nbytes` bytes.  A dense table (dictionary keys with a small product of cardinalities) has the
+ * same size on every rank for the same query + unified dictionaries; a hash table is sized from
+ * the rank's own visible rows, so its size can differ between ranks. */
 int32_t fgpu_query_execute_partial(fgpu_ctx* ctx, fgpu_query* q, uint64_t tx_watermark,
                                    fgpu_result** out, void** dev_ptr, uint64_t* nbytes);
 /* Merges `n` partial tables laid out back to back at DEVICE pointer `gathered` (each `nbytes`
- * long, e.g. the output of an all-gather) into `r` and finalises it. */
+ * long, e.g. the output of an all-gather) into `r` and finalises it.  Every partial must have the
+ * size of `r`'s own (FGPU_ERR_INVALID otherwise); a hash-mode merge table is sized for the groups of
+ * all `n`.  The collective Execute has no such restriction: it merges hash tables of any size. */
 int32_t fgpu_result_merge_partials(fgpu_ctx* ctx, fgpu_result* r, const void* gathered,
                                    uint64_t nbytes, int32_t n);
 /* `*out` = 1 when the partial table of `r` merges by element-wise int64 addition (dense table, every
