@@ -205,18 +205,35 @@ struct SeedJob {
   uint32_t n_runs, total, n_chunks, is_def;
 };
 
-// ---- PLAIN string pages interned at upload (intern_strings.cu) ------------------------------------------
-// One column chunk of an intern batch: its PLAIN string values (validated by the host's page walk) and its
-// open-addressing table, power-of-two capacity of at least twice its values.
+// ---- non-dictionary string pages interned at upload (intern_strings.cu) ------------------------------------
+// One column chunk of an intern batch: its PLAIN / DELTA_LENGTH_BYTE_ARRAY / DELTA_BYTE_ARRAY string values
+// (validated by the host's page walk) and its open-addressing table, power-of-two capacity of at least twice its values.
+// A value is addressed in one of two ways: `len` null (PLAIN pages only): `off` is the offset of its 4-byte length
+// prefix; else `off` is its start and `len` its length.  DELTA_BYTE_ARRAY values start at `rb0` or above: k_str_unfront
+// rebuilds them there, behind the file bytes.
 struct StrChunk {
-  const uint8_t* bytes;      // the chunk's PLAIN value regions (a copy of the file bytes)
-  const uint32_t* off;       // per value: offset of its 4-byte length prefix in `bytes`
+  uint8_t* bytes;            // the chunk's value regions (a copy of the file bytes), then its rebuilt values
+  const uint32_t* off;       // per value: offset of its length prefix, or its start, in `bytes`
+  const uint32_t* len;       // per value: its length; null: a length prefix precedes it
   unsigned long long* keys;  // per slot: (hash >> 32) << 32 | representative value index; ~0: empty
   uint32_t* first;           // per slot: smallest value index; after k_str_compact: the slot's rank among the used slots
   uint32_t* slot;            // per value: its slot
   uint32_t* out_first;       // k_str_compact: first value index per rank (page-locked host memory)
+  const uint32_t* pre;       // DELTA_BYTE_ARRAY values: prefix length, in page order (null: the chunk has none)
+  const uint32_t* suf;       //   start of the suffix in `bytes`
+  const uint32_t* wmin;      //   least prefix length of each window of 32 values of a page
+  uint8_t* out_rebuilt;      // k_str_gather: the rebuilt region, as `bytes` + rb0 holds it, where distinct values go
+                             //   (page-locked host memory; null: the chunk has no DELTA_BYTE_ARRAY values)
   uint32_t n, mask;          // values; capacity - 1
   uint32_t v0, s0;           // values / slots of the batch's chunks before this one
+  uint32_t rb0, _pad;        // start of the rebuilt values in `bytes` (~0: none)
+};
+
+// A run of at most kFrontSeg values of one DELTA_BYTE_ARRAY page, which one warp of k_str_unfront rebuilds.
+struct StrFrontJob {
+  uint32_t chunk;       // in the batch
+  uint32_t v0, d0, w0;  // the page's first value, its index in pre / suf, its first window in wmin
+  uint32_t seg, n;      // the run's first value, relative to the page; its values
 };
 
 // One PLAIN string page whose chunk-local indices k_str_codes packs, LSB first, into the hole its page owns.

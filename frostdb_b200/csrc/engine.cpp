@@ -409,19 +409,22 @@ struct StrBatch {
   }
 };
 
-// PLAIN string pages of every listed column that walk_column left walked but not built, interned on the device in one
-// batch (intern_strings.cu): the chunks' PLAIN value regions and offsets go up with one transfer per contiguous span,
-// k_str_hash and k_str_compact leave every distinct value's first occurrence in page-locked memory, and after the one
-// synchronisation the host interns the new strings in order of first occurrence (finish_column), uploads the
-// chunk-local index of every distinct value and queues one StrCodeJob per PLAIN page on the column's image.
+// Non-dictionary string pages of every listed column that walk_column left walked but not built, interned on the device
+// in one batch (intern_strings.cu): the chunks' value regions and value addresses go up with one transfer per contiguous
+// span, k_str_unfront rebuilds the DELTA_BYTE_ARRAY values behind their chunk's file bytes, k_str_hash and k_str_compact
+// leave every distinct value's first occurrence in page-locked memory, k_str_gather (batches with DELTA_BYTE_ARRAY
+// values only) copies the distinct rebuilt values there too, and after the one synchronisation the host interns the
+// new strings in order of first occurrence (finish_column), uploads the chunk-local index of every distinct value and
+// queues one StrCodeJob per page on the column's image.
 int32_t intern_plain_strings(fgpu_ctx* ctx, Table* table, const std::vector<std::pair<Part*, std::string>>& cols, StrBatch* batch) {
   struct Item {
     ChunkWalk* wk;
     uint64_t v0, s0, cap, byte_off;
+    uint64_t l0, d0, w0, r0;  // in the batch's lengths, prefix / suffix, window and rebuilt-value arrays
   };
   std::vector<Item> items;
   std::vector<std::pair<Part*, std::string>> todo;
-  uint64_t nv = 0, ns = 0;
+  uint64_t nv = 0, ns = 0, nl = 0, nd = 0, nw = 0, nr = 0, n_fronts = 0;
   for (const auto& pc : cols) {
     ColumnImage& img = pc.first->images[pc.second];
     if (!img.walked || img.built) continue;
@@ -430,60 +433,93 @@ int32_t intern_plain_strings(fgpu_ctx* ctx, Table* table, const std::vector<std:
       if (!wk.host.error.empty() || wk.str_off.empty()) continue;
       uint64_t cap = 16;
       while (cap < 2 * uint64_t(wk.str_off.size())) cap <<= 1;
-      items.push_back({&wk, nv, ns, cap, 0});
+      items.push_back({&wk, nv, ns, cap, 0, nl, nd, nw, nr});
       nv += wk.str_off.size();
       ns += cap;
+      nl += wk.str_len.size();
+      nd += wk.str_pre.size();
+      nw += wk.str_wmin.size();
+      if (!wk.str_fronts.empty()) nr += (wk.str_rebuilt_len + 15) & ~uint64_t(15);
+      for (const StrFront& f : wk.str_fronts) n_fronts += (f.n + kFrontSeg - 1) / kFrontSeg;
     }
   }
   if (todo.empty()) return FGPU_OK;
   batch->cols.insert(batch->cols.end(), todo.begin(), todo.end());
   if (ns > 0xffffffffull) return fail(FGPU_ERR_UNSUPPORTED, "PLAIN string values of one upload exceed 2^31");
-  // PLAIN value regions: neighbouring chunks' regions (a few page headers apart) travel as one transfer
+  // value regions: neighbouring chunks' regions (a few page headers apart) travel as one transfer; a chunk with
+  // DELTA_BYTE_ARRAY values ends its span, and its rebuilt values follow at str_rb0 from its first byte
   struct Span { const uint8_t* src; uint64_t len, stage_off; };
   std::vector<Span> spans;
   constexpr uint64_t kGap = 4096;
   uint64_t payload = 0;
+  bool closed = false;  // the last span ends with a chunk's rebuilt values (payload is past them)
   for (Item& it : items) {
     const uint8_t* src = it.wk->str_base;
     const uint64_t len = it.wk->str_span;
-    if (!spans.empty() && src >= spans.back().src + spans.back().len && uint64_t(src - (spans.back().src + spans.back().len)) <= kGap) {
+    if (!closed && !spans.empty() && src >= spans.back().src + spans.back().len && uint64_t(src - (spans.back().src + spans.back().len)) <= kGap) {
       spans.back().len = uint64_t(src - spans.back().src) + len;
     } else {
-      if (!spans.empty()) payload += (spans.back().len + 15) & ~uint64_t(15);
+      if (!spans.empty() && !closed) payload += (spans.back().len + 15) & ~uint64_t(15);
       spans.push_back({src, len, payload});
     }
     it.byte_off = spans.back().stage_off + uint64_t(src - spans.back().src);
+    closed = !it.wk->str_fronts.empty();
+    if (closed) payload = (it.byte_off + it.wk->str_rb0 + it.wk->str_rebuilt_len + 15) & ~uint64_t(15);
   }
-  if (!spans.empty()) payload += (spans.back().len + 15) & ~uint64_t(15);
-  // scratch: [chunks][counts][offsets][slots][codes][first / rank][keys][payload], 16-byte aligned pieces
+  if (!spans.empty() && !closed) payload += (spans.back().len + 15) & ~uint64_t(15);
+  // scratch: [chunks][counts][offsets][lengths][prefixes][suffixes][windows][front jobs][slots][codes][first / rank][keys]
+  // [payload], 16-byte aligned pieces (the pieces of delta pages are empty in a batch of PLAIN pages)
   auto al = [](uint64_t n) { return (n + 15) & ~uint64_t(15); };
   const uint64_t n = items.size();
-  const uint64_t o_cnt = al(n * sizeof(StrChunk)), o_off = o_cnt + al(n * 4), o_slot = o_off + al(nv * 4), o_code = o_slot + al(nv * 4),
-                 o_first = o_code + al(nv * 4), o_keys = o_first + al(ns * 4), o_pay = o_keys + ns * 8;
+  const uint64_t o_cnt = al(n * sizeof(StrChunk)), o_off = o_cnt + al(n * 4), o_len = o_off + al(nv * 4), o_pre = o_len + al(nl * 4),
+                 o_suf = o_pre + al(nd * 4), o_wmin = o_suf + al(nd * 4), o_jobs = o_wmin + al(nw * 4),
+                 o_slot = o_jobs + al(n_fronts * sizeof(StrFrontJob)), o_code = o_slot + al(nv * 4), o_first = o_code + al(nv * 4),
+                 o_keys = o_first + al(ns * 4), o_pay = o_keys + ns * 8;
   CUDA_TRY(batch->scratch.alloc(o_pay + payload, ctx->stream));
   uint8_t* d = static_cast<uint8_t*>(batch->scratch.p);
   size_t pin_cap = 0;
-  uint8_t* pin = ctx->pinned_take(size_t(nv * 4 + n * 4), &pin_cap);  // first occurrences (written by k_str_compact), counts
+  // first occurrences (written by k_str_compact), counts, rebuilt regions (the distinct values written by k_str_gather)
+  const uint64_t pin_rebuilt = al(nv * 4 + n * 4);
+  uint8_t* pin = ctx->pinned_take(size_t(pin_rebuilt + nr), &pin_cap);
   if (!pin) return fail(FGPU_ERR_OOM, "PLAIN string interning: page-locked result buffer");
   struct Give { fgpu_ctx* ctx; uint8_t* p; size_t cap; ~Give() { ctx->pinned_give(p, cap); } } give{ctx, pin, pin_cap};
   uint32_t* h_first = reinterpret_cast<uint32_t*>(pin);
   uint32_t* h_count = h_first + nv;
-  std::vector<uint8_t> head(o_slot, 0);  // chunk table, zero counts, offsets
+  std::vector<uint8_t> head(o_slot, 0);  // chunk table, zero counts, value addresses, front jobs
+  uint64_t job = 0;
   for (size_t i = 0; i < items.size(); i++) {
     const Item& it = items[i];
+    const ChunkWalk& wk = *it.wk;
     StrChunk c{};
     c.bytes = d + o_pay + it.byte_off;
     c.off = reinterpret_cast<const uint32_t*>(d + o_off) + it.v0;
+    c.len = wk.str_len.empty() ? nullptr : reinterpret_cast<const uint32_t*>(d + o_len) + it.l0;
     c.keys = reinterpret_cast<unsigned long long*>(d + o_keys) + it.s0;
     c.first = reinterpret_cast<uint32_t*>(d + o_first) + it.s0;
     c.slot = reinterpret_cast<uint32_t*>(d + o_slot) + it.v0;
     c.out_first = h_first + it.v0;
-    c.n = uint32_t(it.wk->str_off.size());
+    c.n = uint32_t(wk.str_off.size());
     c.mask = uint32_t(it.cap - 1);
     c.v0 = uint32_t(it.v0);
     c.s0 = uint32_t(it.s0);
+    c.rb0 = wk.str_rb0;
+    if (!wk.str_fronts.empty()) {
+      c.pre = reinterpret_cast<const uint32_t*>(d + o_pre) + it.d0;
+      c.suf = reinterpret_cast<const uint32_t*>(d + o_suf) + it.d0;
+      c.wmin = reinterpret_cast<const uint32_t*>(d + o_wmin) + it.w0;
+      c.out_rebuilt = pin + pin_rebuilt + it.r0;
+      std::memcpy(head.data() + o_pre + it.d0 * 4, wk.str_pre.data(), wk.str_pre.size() * 4);
+      std::memcpy(head.data() + o_suf + it.d0 * 4, wk.str_suf.data(), wk.str_suf.size() * 4);
+      std::memcpy(head.data() + o_wmin + it.w0 * 4, wk.str_wmin.data(), wk.str_wmin.size() * 4);
+      for (const StrFront& f : wk.str_fronts)
+        for (uint32_t seg = 0; seg < f.n; seg += kFrontSeg) {
+          const StrFrontJob fj{uint32_t(i), f.v0, f.d0, f.w0, seg, std::min(kFrontSeg, f.n - seg)};
+          std::memcpy(head.data() + o_jobs + job++ * sizeof(StrFrontJob), &fj, sizeof fj);
+        }
+    }
     std::memcpy(head.data() + i * sizeof(StrChunk), &c, sizeof c);
-    std::memcpy(head.data() + o_off + it.v0 * 4, it.wk->str_off.data(), it.wk->str_off.size() * 4);
+    std::memcpy(head.data() + o_off + it.v0 * 4, wk.str_off.data(), wk.str_off.size() * 4);
+    if (!wk.str_len.empty()) std::memcpy(head.data() + o_len + it.l0 * 4, wk.str_len.data(), wk.str_len.size() * 4);
   }
   auto upload = [&](void* dst, const void* src, size_t bytes) {
     if (void* p = ctx->arena_take(bytes)) {
@@ -500,8 +536,10 @@ int32_t intern_plain_strings(fgpu_ctx* ctx, Table* table, const std::vector<std:
   }
   const StrChunk* d_chunks = reinterpret_cast<const StrChunk*>(d);
   uint32_t* d_count = reinterpret_cast<uint32_t*>(d + o_cnt);
+  if (e == cudaSuccess) e = launch_str_unfront(d_chunks, reinterpret_cast<const StrFrontJob*>(d + o_jobs), uint32_t(n_fronts), ctx->stream);
   if (e == cudaSuccess) e = launch_str_hash(d_chunks, uint32_t(n), uint32_t(nv), ctx->stream);
   if (e == cudaSuccess) e = launch_str_compact(d_chunks, uint32_t(n), uint32_t(ns), d_count, ctx->stream);
+  if (e == cudaSuccess && nr > 0) e = launch_str_gather(d_chunks, uint32_t(n), uint32_t(ns), ctx->stream);
   if (e == cudaSuccess) e = cudaMemcpyAsync(h_count, d_count, n * 4, cudaMemcpyDeviceToHost, ctx->stream);
   if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
   if (e != cudaSuccess) {
@@ -521,6 +559,7 @@ int32_t intern_plain_strings(fgpu_ctx* ctx, Table* table, const std::vector<std:
       items[i].wk->str_firsts[k] = fr[k].first;
       rank_of[i][k] = fr[k].second;
     }
+    if (!items[i].wk->str_fronts.empty()) items[i].wk->str_rebuilt = pin + pin_rebuilt + items[i].r0;
   }
   // the sections: interning of the new strings, holes for the indices; then the chunk-local index per rank
   std::vector<uint32_t> codes;

@@ -41,11 +41,14 @@ cudaError_t launch_flatten(const FlatJob* d_jobs, uint32_t n_jobs, uint32_t tota
 cudaError_t launch_chunk_minmax(const NarrowJob* d_jobs, uint32_t n_jobs, uint32_t total_blocks, long long* d_mm, unsigned long long* d_bsum,
                                 cudaStream_t st);
 cudaError_t launch_narrow(const NarrowJob* d_jobs, uint32_t n_jobs, uint32_t total_blocks, const unsigned long long* d_bsum, cudaStream_t st);
-// PLAIN string pages -> chunk-local dictionary indices (intern_strings.cu): hash and insert every value into its
-// chunk's table, rank each chunk's used slots (first occurrences to the host, counts per chunk), then pack every
-// page's indices into its hole
+// Non-dictionary string pages -> chunk-local dictionary indices (intern_strings.cu): rebuild the DELTA_BYTE_ARRAY
+// values, hash and insert every value into its chunk's table, rank each chunk's used slots (first occurrences to the
+// host, counts per chunk), copy the distinct rebuilt values to the host, then pack every page's indices into its hole
+constexpr uint32_t kFrontSeg = 1024;  // values of one StrFrontJob
+cudaError_t launch_str_unfront(const StrChunk* d_chunks, const StrFrontJob* d_jobs, uint32_t n_jobs, cudaStream_t st);
 cudaError_t launch_str_hash(const StrChunk* d_chunks, uint32_t n_chunks, uint32_t total_values, cudaStream_t st);
 cudaError_t launch_str_compact(const StrChunk* d_chunks, uint32_t n_chunks, uint32_t total_slots, uint32_t* d_counts, cudaStream_t st);
+cudaError_t launch_str_gather(const StrChunk* d_chunks, uint32_t n_chunks, uint32_t total_slots, cudaStream_t st);
 cudaError_t launch_str_codes(const StrCodeJob* d_jobs, uint32_t n_jobs, uint32_t total_groups, cudaStream_t st);
 // partial-table exchange over peer-mapped mailboxes (comm.cu)
 cudaError_t launch_comm_push(const CommPush& p, int sm_count, cudaStream_t st);

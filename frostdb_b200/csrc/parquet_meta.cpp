@@ -2,7 +2,9 @@
 // public format specification (field ids in comments are parquet.thrift's).
 #include "parquet_meta.h"
 
+#include <algorithm>
 #include <cstring>
+#include <type_traits>
 
 namespace fgpu {
 namespace {
@@ -658,6 +660,80 @@ uint32_t hybrid_value_at(const uint8_t* stream, const std::vector<HostRun>& runs
   for (int i = 0; i < 5; i++) window |= uint64_t(p[i]) << (8 * i);  // callers pad streams by 8 bytes
   return uint32_t((window >> (bit & 7)) & ((w == 32) ? 0xffffffffull : ((1ull << w) - 1)));
 }
+
+// ---- DELTA_BINARY_PACKED -------------------------------------------------------------------------------------
+namespace {
+bool read_uleb(const uint8_t*& p, const uint8_t* end, uint64_t* v) {
+  uint64_t x = 0;
+  for (int shift = 0; shift < 70; shift += 7) {
+    if (p >= end) return false;
+    const uint8_t b = *p++;
+    if (shift < 64) x |= uint64_t(b & 0x7f) << shift;
+    if ((b & 0x80) == 0) {
+      *v = x;
+      return true;
+    }
+  }
+  return false;
+}
+}  // namespace
+
+template <typename T>
+bool decode_delta_binary_packed(const uint8_t* data, uint64_t len, uint32_t count, std::vector<T>* out, uint64_t* used, std::string* err) {
+  using U = typename std::make_unsigned<T>::type;
+  constexpr uint32_t kBits = 8 * sizeof(T);
+  const uint8_t* p = data;
+  const uint8_t* const end = data + len;
+  const std::string overrun = "DELTA_BINARY_PACKED stream overruns its page";
+  uint64_t block = 0, n_mb = 0, total = 0, first = 0;
+  if (!read_uleb(p, end, &block) || !read_uleb(p, end, &n_mb) || !read_uleb(p, end, &total) || !read_uleb(p, end, &first)) {
+    *err = overrun;
+    return false;
+  }
+  if (block == 0 || block % 128 != 0) { *err = "DELTA_BINARY_PACKED block size is not a multiple of 128"; return false; }
+  if (n_mb == 0 || block % n_mb != 0 || (block / n_mb) % 32 != 0) { *err = "DELTA_BINARY_PACKED miniblock size is not a multiple of 32"; return false; }
+  if (total != count) { *err = "DELTA_BINARY_PACKED value count differs from the page's values"; return false; }
+  const uint64_t per_mb = block / n_mb;
+  if (per_mb > (uint64_t(1) << 40) && count > 1) { *err = overrun; return false; }  // (a miniblock larger than any page)
+  out->clear();
+  out->reserve(count);
+  U v = U((first >> 1) ^ (~(first & 1) + 1));  // zigzag, wrapped to the value width
+  if (count > 0) out->push_back(T(v));
+  while (out->size() < count) {
+    uint64_t zmin = 0;
+    if (!read_uleb(p, end, &zmin)) { *err = overrun; return false; }
+    const U min_delta = U((zmin >> 1) ^ (~(zmin & 1) + 1));
+    if (uint64_t(end - p) < n_mb) { *err = overrun; return false; }
+    const uint8_t* widths = p;
+    p += n_mb;
+    for (uint64_t m = 0; m < n_mb && out->size() < count; m++) {
+      const uint32_t w = widths[m];
+      if (w > kBits) { *err = "DELTA_BINARY_PACKED miniblock bit width > " + std::to_string(kBits); return false; }
+      const uint64_t bytes = per_mb * w / 8;  // a miniblock holding values is written whole (padding included)
+      if (uint64_t(end - p) < bytes) { *err = overrun; return false; }
+      const uint64_t take = std::min<uint64_t>(per_mb, count - out->size());
+      for (uint64_t i = 0; i < take; i++) {
+        uint64_t d = 0;
+        if (w) {  // LSB first; a 64-bit value at an odd bit position spans 9 bytes
+          const uint64_t b0 = (i * w) >> 3, avail = bytes - b0;
+          const unsigned sh = unsigned((i * w) & 7);
+          uint64_t window = 0;
+          for (uint64_t k = 0; k < std::min<uint64_t>(8, avail); k++) window |= uint64_t(p[b0 + k]) << (8 * k);
+          d = window >> sh;
+          if (sh && avail > 8) d |= uint64_t(p[b0 + 8]) << (64 - sh);
+          if (w < 64) d &= (uint64_t(1) << w) - 1;
+        }
+        v = U(v + min_delta + U(d));
+        out->push_back(T(v));
+      }
+      p += bytes;
+    }
+  }
+  *used = uint64_t(p - data);
+  return true;
+}
+
+template bool decode_delta_binary_packed<int32_t>(const uint8_t*, uint64_t, uint32_t, std::vector<int32_t>*, uint64_t*, std::string*);
 
 
 // ---- bloom filters ---------------------------------------------------------------------------------------------

@@ -111,4 +111,12 @@ bool walk_hybrid(const uint8_t* data, uint32_t len, int w, uint32_t count, uint3
 // Reads value i of a hybrid stream described by runs (host-side reference used by describe/tests).
 uint32_t hybrid_value_at(const uint8_t* stream, const std::vector<HostRun>& runs, uint32_t ordinal, bool* was_rle = nullptr);
 
+// Decodes one DELTA_BINARY_PACKED stream of `count` values of type T (int32_t: the length streams of
+// DELTA_LENGTH_BYTE_ARRAY / DELTA_BYTE_ARRAY pages), with the format's wrap-around arithmetic, from `data`.
+// Validates the header (block size a multiple of 128, values per miniblock a multiple of 32, total == count),
+// the bit width of every miniblock that holds values (<= the bits of T) and that nothing runs past `len`.
+// `used`: the stream's bytes (miniblocks holding values are whole; the unused ones of the last block are absent).
+template <typename T>
+bool decode_delta_binary_packed(const uint8_t* data, uint64_t len, uint32_t count, std::vector<T>* out, uint64_t* used, std::string* err);
+
 }  // namespace fgpu

@@ -93,6 +93,7 @@ inline uint64_t popcount_range(const std::vector<uint64_t>& bm, uint64_t pos, ui
 }
 
 bool is_dict_encoding(int32_t e) { return e == ENC_RLE_DICTIONARY || e == ENC_PLAIN_DICTIONARY; }
+bool is_delta_string(int32_t e) { return e == ENC_DELTA_LENGTH_BYTE_ARRAY || e == ENC_DELTA_BYTE_ARRAY; }
 
 // Length prefixes of one PLAIN BYTE_ARRAY page holding `n` values: one offset per value, from the chunk's first PLAIN
 // value region.  Every value must lie inside the page and the values must fill it.
@@ -102,18 +103,118 @@ bool walk_plain_strings(const PageInfo& pg, uint32_t n, ChunkWalk* wk, std::stri
   if (base + pg.values_len > 0xffffffffull) { *err = "PLAIN string pages of one chunk span more than 4 GiB"; return false; }
   const uint8_t* q = pg.values;
   const uint8_t* end = pg.values + pg.values_len;
+  const bool start_len = !wk->str_len.empty();  // the chunk holds delta pages too: values are addressed by start and length
   for (uint32_t i = 0; i < n; i++) {
     if (end - q < 4) { *err = "PLAIN string page shorter than its value count"; return false; }
     uint32_t l;
     std::memcpy(&l, q, 4);
     if (l > uint64_t(end - q) - 4) { *err = "PLAIN string length prefix overruns its page"; return false; }
-    wk->str_off.push_back(uint32_t(base + uint64_t(q - pg.values)));
+    wk->str_off.push_back(uint32_t(base + uint64_t(q - pg.values) + (start_len ? 4 : 0)));
+    if (start_len) wk->str_len.push_back(l);
     q += 4 + uint64_t(l);
   }
   if (q != end) { *err = "PLAIN string page holds more values than its definition levels"; return false; }
   wk->str_span = uint32_t(base + pg.values_len);
   return true;
 }
+
+// Values of one DELTA_LENGTH_BYTE_ARRAY (all lengths, then all bytes) or DELTA_BYTE_ARRAY (all prefix lengths, all
+// suffix lengths, then all suffix bytes) page holding `n` values.  The lengths must be non-negative and their bytes
+// must fill the page exactly; a prefix may not be longer than the value before it ("" at the start of the page).
+// DELTA_LENGTH_BYTE_ARRAY values are addressed in the file bytes, DELTA_BYTE_ARRAY values in the rebuilt region
+// (offsets relative to its start until the walk of the chunk ends).
+bool walk_delta_strings(const PageInfo& pg, uint32_t n, ChunkWalk* wk, std::string* err) {
+  const bool dba = pg.encoding == ENC_DELTA_BYTE_ARRAY;
+  const std::string what = dba ? "DELTA_BYTE_ARRAY" : "DELTA_LENGTH_BYTE_ARRAY";
+  if (!wk->str_base) wk->str_base = pg.values;
+  const uint64_t base = uint64_t(pg.values - wk->str_base);
+  if (base + pg.values_len > 0xffffffffull) { *err = what + " pages of one chunk span more than 4 GiB"; return false; }
+  if (wk->str_len.empty() && !wk->str_off.empty()) {  // PLAIN values walked so far: to start and length
+    for (uint32_t& o : wk->str_off) {
+      uint32_t l;
+      std::memcpy(&l, wk->str_base + o, 4);
+      wk->str_len.push_back(l);
+      o += 4;
+    }
+  }
+  const uint8_t* q = pg.values;
+  const uint8_t* const end = pg.values + pg.values_len;
+  std::vector<int32_t> a, b;
+  uint64_t used = 0;
+  std::string e;
+  if (!decode_delta_binary_packed(q, uint64_t(end - q), n, &a, &used, &e)) {
+    *err = what + (dba ? " prefix lengths: " : " lengths: ") + e;
+    return false;
+  }
+  q += used;
+  if (dba) {
+    if (!decode_delta_binary_packed(q, uint64_t(end - q), n, &b, &used, &e)) { *err = what + " suffix lengths: " + e; return false; }
+    q += used;
+  }
+  const std::vector<int32_t>& lens = dba ? b : a;
+  uint64_t total = 0, prev = 0;
+  for (uint32_t i = 0; i < n; i++) {
+    if (lens[i] < 0) { *err = what + (dba ? " suffix length is negative" : " length is negative"); return false; }
+    if (dba) {
+      if (a[i] < 0) { *err = what + " prefix length is negative"; return false; }
+      if (uint64_t(a[i]) > prev) { *err = what + " prefix is longer than the value before it"; return false; }
+      prev = uint64_t(a[i]) + uint64_t(b[i]);
+    }
+    total += uint64_t(lens[i]);
+  }
+  if (total != uint64_t(end - q)) {
+    *err = what + (dba ? " suffix lengths do not add up to the page's value bytes" : " lengths do not add up to the page's value bytes");
+    return false;
+  }
+  uint64_t pos = base + uint64_t(q - pg.values);  // file offset of the first value's (suffix) bytes
+  if (!dba) {
+    for (uint32_t i = 0; i < n; i++) {
+      wk->str_off.push_back(uint32_t(pos));
+      wk->str_len.push_back(uint32_t(a[i]));
+      pos += uint64_t(a[i]);
+    }
+  } else {
+    const StrFront f{uint32_t(wk->str_off.size()), uint32_t(wk->str_pre.size()), uint32_t(wk->str_wmin.size()), n};
+    uint64_t out = wk->str_rebuilt_len;
+    for (uint32_t i = 0; i < n; i++) {
+      const uint64_t len = uint64_t(a[i]) + uint64_t(b[i]);
+      if (out + len > 0xffffffffull) { *err = "DELTA_BYTE_ARRAY values of one chunk exceed 4 GiB"; return false; }
+      wk->str_off.push_back(uint32_t(out));
+      wk->str_len.push_back(uint32_t(len));
+      wk->str_pre.push_back(uint32_t(a[i]));
+      wk->str_suf.push_back(uint32_t(pos));
+      if (i % 32 == 0) wk->str_wmin.push_back(uint32_t(a[i]));
+      else wk->str_wmin.back() = std::min(wk->str_wmin.back(), uint32_t(a[i]));
+      out += len;
+      pos += uint64_t(b[i]);
+    }
+    wk->str_rebuilt_len = out;
+    wk->str_fronts.push_back(f);
+  }
+  wk->str_span = uint32_t(base + pg.values_len);
+  return true;
+}
+
+}  // namespace
+
+void unfront_strings(ChunkWalk* wk) {
+  if (wk->str_fronts.empty() || !wk->str_rebuilt_host.empty()) return;
+  wk->str_rebuilt_host.resize(size_t(wk->str_rebuilt_len) + 1);
+  uint8_t* const rb = wk->str_rebuilt_host.data();
+  for (const StrFront& f : wk->str_fronts) {
+    const uint8_t* prev = nullptr;
+    for (uint32_t i = 0; i < f.n; i++) {
+      uint8_t* dst = rb + (wk->str_off[f.v0 + i] - wk->str_rb0);
+      const uint32_t pre = wk->str_pre[f.d0 + i];
+      if (pre) std::memmove(dst, prev, pre);
+      std::memcpy(dst + pre, wk->str_base + wk->str_suf[f.d0 + i], wk->str_len[f.v0 + i] - pre);
+      prev = dst;
+    }
+  }
+  wk->str_rebuilt = rb;
+}
+
+namespace {
 
 // Walks and validates every page of one column chunk (first half of building it).
 void walk_chunk(const ChunkMeta& cm, const SchemaLeaf& leaf, uint32_t n_rows, ChunkWalk* wk) {
@@ -138,7 +239,7 @@ void walk_chunk(const ChunkMeta& cm, const SchemaLeaf& leaf, uint32_t n_rows, Ch
   bool any_dict = false, any_plain = false;
   for (const PageInfo& pg : cm.pages) {
     if (is_dict_encoding(pg.encoding)) any_dict = true;
-    else if (pg.encoding == ENC_PLAIN) any_plain = true;
+    else if (pg.encoding == ENC_PLAIN || (leaf.phys == PT_BYTE_ARRAY && is_delta_string(pg.encoding))) any_plain = true;
     else { out->error = "unsupported page encoding " + std::to_string(pg.encoding); return; }
   }
   // (a string chunk may hold both: a dictionary whose writer fell back to PLAIN part of the way through)
@@ -220,9 +321,10 @@ void walk_chunk(const ChunkMeta& cm, const SchemaLeaf& leaf, uint32_t n_rows, Ch
     for (size_t p = 0; p < cm.pages.size(); p++) {
       const PageInfo& pg = cm.pages[p];
       if (page_nn[p] == 0) continue;
-      if (pg.encoding == ENC_PLAIN) {  // strings: one bit-packed run whose hole the section writing places here
+      if (pg.encoding == ENC_PLAIN || is_delta_string(pg.encoding)) {  // strings: one bit-packed run whose hole the section writing places here
         const uint32_t first = uint32_t(wk->str_off.size());
-        if (!walk_plain_strings(pg, page_nn[p], wk, &err)) { out->error = err; return; }
+        const bool ok = pg.encoding == ENC_PLAIN ? walk_plain_strings(pg, page_nn[p], wk, &err) : walk_delta_strings(pg, page_nn[p], wk, &err);
+        if (!ok) { out->error = err; return; }
         wk->str_pages.push_back(StrPage{uint32_t(vruns.size()), first, page_nn[p]});
         vruns.push_back(HostRun{vo, uint32_t(vstream.size()), 0, 1u});
         vo += page_nn[p];
@@ -239,6 +341,14 @@ void walk_chunk(const ChunkMeta& cm, const SchemaLeaf& leaf, uint32_t n_rows, Ch
       vo += page_nn[p];
     }
     out->desc.kind = (leaf.phys == PT_BYTE_ARRAY) ? CK_DICT_STR : CK_DICT64;
+    // the rebuilt DELTA_BYTE_ARRAY values go behind the file bytes, in the same 32-bit address space
+    if (!wk->str_fronts.empty()) {
+      const uint64_t rb0 = (uint64_t(wk->str_span) + 15) & ~uint64_t(15);
+      if (rb0 + wk->str_rebuilt_len > 0xffffffffull) { out->error = "DELTA_BYTE_ARRAY values of one chunk exceed 4 GiB"; return; }
+      wk->str_rb0 = uint32_t(rb0);
+      for (const StrFront& f : wk->str_fronts)
+        for (uint32_t i = f.v0; i < f.v0 + f.n; i++) wk->str_off[i] += uint32_t(rb0);
+    }
   } else {
     for (size_t p = 0; p < cm.pages.size(); p++) {
       const PageInfo& pg = cm.pages[p];
@@ -314,17 +424,18 @@ void write_chunk(ChunkWalk& wk, uint32_t n_rows, int tile_rows, GlobalDict* dict
     ChunkInterner in(dict, &out->lut_host);
     out->lut_host.reserve(wk.dict_entries.size());
     for (const auto& e : wk.dict_entries) in.entry(reinterpret_cast<const char*>(e.first), e.second);
-    std::vector<uint32_t> codes;  // host: per PLAIN value; device: per distinct PLAIN value (str_firsts)
+    std::vector<uint32_t> codes;  // host: per non-dictionary value; device: per distinct one (str_firsts)
     if (host_intern) {
+      unfront_strings(&wk);
       codes.reserve(wk.str_off.size());
       for (uint32_t i = 0; i < uint32_t(wk.str_off.size()); i++) {
-        const std::string_view s = plain_string(wk, i);
+        const std::string_view s = chunk_string(wk, i);
         codes.push_back(in.add(s.data(), s.size()));
       }
-    } else {
+    } else {  // (the intern batch left the rebuilt bytes of the distinct DELTA_BYTE_ARRAY values in str_rebuilt)
       codes.reserve(wk.str_firsts.size());
       for (uint32_t f : wk.str_firsts) {
-        const std::string_view s = plain_string(wk, f);
+        const std::string_view s = chunk_string(wk, f);
         codes.push_back(in.add(s.data(), s.size()));
       }
     }
@@ -871,16 +982,18 @@ bool column_dict_values(const ParsedFile& pf, const std::string& column, GlobalD
       const ChunkMeta& cm = rg.chunks[c];
       if (!cm.error.empty()) { *err = column + ": " + cm.error; return false; }
       bool plain_strings = false;
-      for (const PageInfo& pg : cm.pages) plain_strings = plain_strings || (pf.leaves[c].phys == PT_BYTE_ARRAY && pg.encoding == ENC_PLAIN);
-      if (plain_strings) {  // the page walk validates the dictionary page and the PLAIN values
+      for (const PageInfo& pg : cm.pages)
+        plain_strings = plain_strings || (pf.leaves[c].phys == PT_BYTE_ARRAY && (pg.encoding == ENC_PLAIN || is_delta_string(pg.encoding)));
+      if (plain_strings) {  // the page walk validates the dictionary page and the non-dictionary values
         ChunkWalk wk;
         walk_chunk(cm, pf.leaves[c], uint32_t(rg.num_rows), &wk);
         if (!wk.host.error.empty()) { *err = column + ": " + wk.host.error; return false; }
+        unfront_strings(&wk);
         std::vector<uint32_t> lut;
         ChunkInterner in(d, &lut);
         for (const auto& e : wk.dict_entries) in.entry(reinterpret_cast<const char*>(e.first), e.second);
         for (uint32_t i = 0; i < uint32_t(wk.str_off.size()); i++) {
-          const std::string_view s = plain_string(wk, i);
+          const std::string_view s = chunk_string(wk, i);
           in.add(s.data(), s.size());
         }
         continue;

@@ -109,12 +109,18 @@ struct Extent {
   uint64_t dst_off;  // offset inside the column image
 };
 
-// One PLAIN BYTE_ARRAY page of a chunk: its values become one bit-packed run of chunk-local indices, whose payload
-// is a hole in the value-stream section (zero until the indices are written into it).
+// One PLAIN, DELTA_LENGTH_BYTE_ARRAY or DELTA_BYTE_ARRAY page of a chunk: its values become one bit-packed run of
+// chunk-local indices, whose payload is a hole in the value-stream section (zero until the indices are written into it).
 struct StrPage {
   uint32_t run;       // its entry in the chunk's value directory
-  uint32_t first, n;  // its non-null values: ordinals [first, first + n) among the chunk's PLAIN values
+  uint32_t first, n;  // its non-null values: ordinals [first, first + n) among the chunk's non-dictionary values
   uint64_t hole = 0;  // once the sections are written: image offset of its ceil(n / 8) * w index bytes
+};
+
+// One DELTA_BYTE_ARRAY page of a chunk: values [v0, v0 + n) of the chunk, front-coded.  Value i is the first
+// str_pre[d0 + i - v0] bytes of value i - 1 (of "" for the page's first value), then its suffix.
+struct StrFront {
+  uint32_t v0, d0, w0, n;  // first value; its index in str_pre / str_suf; the page's first window in str_wmin; values
 };
 
 // What the page walk of one chunk leaves for the section writing (the two halves of building a column).
@@ -129,24 +135,43 @@ struct ChunkWalk {
   std::vector<std::pair<const uint8_t*, uint32_t>> dict_entries;  // string dictionary page, validated
   std::vector<int64_t> dict64;
   std::vector<std::pair<const uint8_t*, uint32_t>> plain64;  // PLAIN int64 / double pages: value region, values
-  // PLAIN string values, validated: every length prefix and its bytes lie inside their page
-  const uint8_t* str_base = nullptr;  // value region of the first PLAIN page
-  uint32_t str_span = 0;              // bytes from str_base to the end of the last PLAIN page's value region
-  std::vector<uint32_t> str_off;      // per PLAIN value: offset of its length prefix from str_base
+  // Non-dictionary string values (PLAIN, DELTA_LENGTH_BYTE_ARRAY, DELTA_BYTE_ARRAY pages), validated: every value lies
+  // inside its page.  They are addressed in one 32-bit space per chunk: [0, str_span) the file bytes from str_base,
+  // [str_rb0, str_rb0 + str_rebuilt_len) the DELTA_BYTE_ARRAY values rebuilt from their prefixes and suffixes.
+  const uint8_t* str_base = nullptr;  // value region of the first non-dictionary page
+  uint32_t str_span = 0;              // bytes from str_base to the end of the last non-dictionary page's value region
+  std::vector<uint32_t> str_off;      // per value: str_len empty: offset of its 4-byte length prefix; else its start
+  std::vector<uint32_t> str_len;      // per value: its length (empty while the chunk holds PLAIN pages only)
   std::vector<StrPage> str_pages;
-  // intern result: the first ordinal of every distinct PLAIN value, ascending (left by the device's intern batch;
+  // DELTA_BYTE_ARRAY pages: per page, per value its prefix length and the start of its suffix (in the file bytes),
+  // per window of 32 values of a page the least prefix length in it
+  std::vector<StrFront> str_fronts;
+  std::vector<uint32_t> str_pre, str_suf, str_wmin;
+  uint32_t str_rb0 = 0xffffffffu;     // start of the rebuilt values (none: no value starts there)
+  uint64_t str_rebuilt_len = 0;
+  const uint8_t* str_rebuilt = nullptr;     // host bytes of the rebuilt region (all of it, or the values being interned)
+  std::vector<uint8_t> str_rebuilt_host;    // the host's own rebuild (unfront_strings)
+  // intern result: the first ordinal of every distinct value, ascending (left by the device's intern batch;
   // empty: the host interns row by row), and after the section writing the chunk-local index of each of them
   std::vector<uint32_t> str_firsts, str_codes;
-  uint32_t str_w = 0;  // bit width of the PLAIN pages' indices
+  uint32_t str_w = 0;  // bit width of the non-dictionary pages' indices
 };
 
-// PLAIN string value `i` of a walked chunk.
-inline std::string_view plain_string(const ChunkWalk& wk, uint32_t i) {
-  const uint8_t* p = wk.str_base + wk.str_off[i];
-  uint32_t l;
-  std::memcpy(&l, p, 4);
-  return std::string_view(reinterpret_cast<const char*>(p + 4), l);
+// Non-dictionary string value `i` of a walked chunk (a rebuilt DELTA_BYTE_ARRAY value needs str_rebuilt).
+inline std::string_view chunk_string(const ChunkWalk& wk, uint32_t i) {
+  const uint32_t off = wk.str_off[i];
+  if (wk.str_len.empty()) {
+    const uint8_t* p = wk.str_base + off;
+    uint32_t l;
+    std::memcpy(&l, p, 4);
+    return std::string_view(reinterpret_cast<const char*>(p + 4), l);
+  }
+  const uint8_t* p = off >= wk.str_rb0 ? wk.str_rebuilt + (off - wk.str_rb0) : wk.str_base + off;
+  return std::string_view(reinterpret_cast<const char*>(p), wk.str_len[i]);
 }
+
+// Rebuilds a walked chunk's DELTA_BYTE_ARRAY values on the host (str_rebuilt_host; no-op without such pages).
+void unfront_strings(ChunkWalk* wk);
 
 // Device residency of one column of one part (all its row groups in one allocation).
 struct ColumnImage {
@@ -210,8 +235,8 @@ void walk_column(int index_rows, Table* table, Part* part, const std::string& co
 void finish_column(int index_rows, Table* table, Part* part, const std::string& column, bool host_intern);
 
 // The distinct strings of one column of a parsed Parquet file (pages walked), in the order a put of the file interns
-// them: per row group the dictionary page, then the PLAIN pages' values not in it, in order of first occurrence.
-// Returns false on a chunk whose dictionary page or PLAIN string pages cannot be read.
+// them: per row group the dictionary page, then the non-dictionary (PLAIN, DELTA_LENGTH_BYTE_ARRAY, DELTA_BYTE_ARRAY)
+// pages' values not in it, in order of first occurrence.  Returns false on a chunk whose pages cannot be read.
 bool column_dict_values(const ParsedFile& pf, const std::string& column, GlobalDict* out, std::string* err);
 
 // L0 Arrow-record part (parts/arrow.go:14-55): one row group holding the record's rows.  Every column image

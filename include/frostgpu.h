@@ -253,8 +253,8 @@ int32_t fgpu_dict_export(fgpu_ctx* ctx, const char* table, const char* column, u
 int32_t fgpu_dict_preload(fgpu_ctx* ctx, const char* table, const char* column,
                           const uint8_t* blob, uint64_t len, uint32_t count);
 /* Host-only: the distinct strings of `column` in one Parquet file, in the blob format above, in the
- * order a put of the file interns them: per row group the dictionary page's entries, then the PLAIN
- * pages' values that are not among them, in order of first occurrence (first-seen order over the
+ * order a put of the file interns them: per row group the dictionary page's entries, then the
+ * non-dictionary pages' values that are not among them, in order of first occurrence (first-seen order over the
  * file).  Lets a rank contribute its strings to the union without uploading. */
 int32_t fgpu_parquet_dict_values(const uint8_t* file, uint64_t len, const char* column,
                                  uint8_t* buf, uint64_t cap, uint64_t* out_len, uint32_t* out_count);

@@ -1,5 +1,5 @@
-"""Upload cost of PLAIN string columns (interned on the device at put) against the same column as RLE_DICTIONARY and
-the same rows as an Arrow part (interned on the host, row by row).
+"""Upload cost of PLAIN, DELTA_LENGTH_BYTE_ARRAY and DELTA_BYTE_ARRAY string columns (interned on the device at put)
+against the same column as RLE_DICTIONARY and the same rows as an Arrow part (interned on the host, row by row).
 
 For 4 Mi-row parts whose string column `s` has 16, 64 Ki and 4 Mi distinct values, and each representation, it times
   put + first Execute   a fresh table: fgpu_part_put_* (the whole part goes to the device), then one Execute
@@ -7,6 +7,9 @@ For 4 Mi-row parts whose string column `s` has 16, 64 Ki and 4 Mi distinct value
 with a host clock around calls that end in a device synchronise.  The plan counts the rows whose `s` differs from a
 literal, so it reads every value of `s`.  Prints one JSON line per measurement, then one with all of them and the
 card's name and power limit, which --out also writes to a file.
+
+It also reports the device time of k_str_unfront (torch.profiler) in the put of a DELTA_BYTE_ARRAY part whose sorted
+values share long prefixes ("/usr/lib/python3/site-packages/module_0000123/frame_4").
 
     python scripts/plain_strings_upload.py [--rows N] [--reps K] [--out FILE]
 """
@@ -46,11 +49,38 @@ def make_table(n_rows: int, n_distinct: int, seed: int) -> pa.Table:
     return t.replace_schema_metadata({"dynamic_columns": ""})
 
 
-def parquet(t: pa.Table, dictionary: bool) -> bytes:
+def parquet(t: pa.Table, dictionary: bool, encoding: str = None) -> bytes:
     sink = io.BytesIO()
+    kwargs = {"column_encoding": {"s": encoding}} if encoding else {}
     pq.write_table(t, sink, compression="NONE", use_dictionary=["s"] if dictionary else False, dictionary_pagesize_limit=1 << 30,
-                   row_group_size=t.num_rows, store_schema=False)
+                   row_group_size=t.num_rows, store_schema=False, **kwargs)
     return sink.getvalue()
+
+
+def unfront_time(cs, db, n_rows: int) -> dict:
+    """k_str_unfront's device time in the put of a sorted DELTA_BYTE_ARRAY part with long shared prefixes."""
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+    s = pa.array([f"/usr/lib/python3/site-packages/module_{i // 5:07d}/frame_{i % 5}" for i in range(n_rows)], type=pa.string())
+    t = pa.table({"s": s, "timestamp": pa.array(np.arange(n_rows, dtype=np.int64)), "value": pa.array(np.zeros(n_rows, dtype=np.int64))})
+    buf = parquet(t.replace_schema_metadata({"dynamic_columns": ""}), False, "DELTA_BYTE_ARRAY")
+    torch.cuda.init()
+    out = {}
+    for rep in ("warm", "measured"):
+        name = f"unfront_{rep}"
+        db.Table(name, SCHEMA)
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            cs.engine.put_parquet(name, buf)
+        cs.engine.drop_table(name)
+        db.tables.pop(name, None)
+        us = {}
+        for e in prof.events():
+            if e.device_type.name == "CUDA" and "k_str_" in e.name:
+                k = e.name.split("k_str_")[1].split("(")[0].split("E")[0]
+                us["k_str_" + k] = us.get("k_str_" + k, 0.0) + e.device_time
+        out = {"rows": n_rows, "rebuilt_bytes": sum(len(v) for v in s.to_pylist()),
+               "kernel_us": {k: round(v, 1) for k, v in sorted(us.items())}}
+    return out
 
 
 def record(t: pa.Table) -> pa.RecordBatch:
@@ -87,7 +117,8 @@ def main() -> None:
     k = 0
     for n_distinct in (16, 64 << 10, args.rows):
         t = make_table(args.rows, n_distinct, 7)
-        inputs = {"plain": parquet(t, False), "dictionary": parquet(t, True), "arrow": record(t)}
+        inputs = {"plain": parquet(t, False), "dlba": parquet(t, False, "DELTA_LENGTH_BYTE_ARRAY"),
+                  "dba": parquet(t, False, "DELTA_BYTE_ARRAY"), "dictionary": parquet(t, True), "arrow": record(t)}
         for rep, src in inputs.items():
             k += 1
             name = f"u{k}"
@@ -112,8 +143,13 @@ def main() -> None:
             print(json.dumps(results[-1]), flush=True)
             cs.engine.drop_table(name)
             db.tables.pop(name, None)
+    try:
+        unfront = unfront_time(cs, db, args.rows)
+    except Exception as e:  # (the upload numbers are still reported)
+        unfront = {"error": repr(e)}
+    print(json.dumps({"unfront": unfront}), flush=True)
     cs.Close()
-    out = {"rows": args.rows, **card(), "results": results}
+    out = {"rows": args.rows, **card(), "results": results, "unfront": unfront}
     if args.out:
         with open(args.out, "w") as f:
             json.dump(out, f, indent=1)
