@@ -246,6 +246,26 @@ struct StrCodeJob {
   uint32_t g0, _pad;      // 8-value groups of the launch's jobs before this one
 };
 
+// ---- DELTA_BINARY_PACKED int64 pages decoded at upload (delta_int64.cu) --------------------------------------
+// One page of a column upload: its values are the page's first value, then one value per delta, written to `dst`.
+// The upload's pages are listed in order of g0, the ordinal of the page's first 32-value group among the upload's groups.
+struct DbpPage {
+  unsigned long long* dst;  // its n dense values (in the column image)
+  unsigned long long src;   // offset of its stream in the staging buffer
+  unsigned long long first; // its first value
+  uint32_t n, g0;           // values (>= 1); first group
+  uint32_t mb0, per_mb;     // its first miniblock in the upload's list; values per miniblock (clamped to 2^32 - 1)
+};
+
+// One miniblock of a page holding values: the deltas of the page's values 1 + k for k in [m * per_mb, (m + 1) * per_mb),
+// m its index within the page.
+struct DbpMini {
+  unsigned long long min_delta;
+  uint32_t off;    // byte offset of its packed deltas from the page's stream start
+  uint32_t width;  // 0 .. 64
+};
+constexpr int kDbpGroupsPerCta = 32;  // one warp per 32-value group: a CTA covers 1 024 values
+
 // ---- sorted-run scan (k_runs_tma): the plan shape of compacted parts -----------------------------------
 // Row groups whose filter columns and aggregate inputs are PLAIN non-null int64 and whose group-key
 // columns are run-length only (sorted parts) are scanned by a dedicated kernel that walks the key run

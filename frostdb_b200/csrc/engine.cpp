@@ -679,17 +679,55 @@ int32_t ensure_resident(fgpu_ctx* ctx, Table* table, Part* part, const std::stri
       for (size_t i = sp.first; i < sp.first + sp.n; i++)
         copies.push_back({sp.stage_off + uint64_t(img.extents[i].src - sp.src), img.extents[i].dst_off, img.extents[i].len});
     }
-    DevBuf stage;
     const uint64_t table_off = stage_bytes;
-    if (!copies.empty() && e == cudaSuccess) {
-      e = stage.alloc(stage_bytes + copies.size() * sizeof(PageCopy), ctx->stream);
-      if (e == cudaSuccess) {
-        const void* tsrc = copies.data();
-        if (void* pin = ctx->arena_take(copies.size() * sizeof(PageCopy))) {
-          std::memcpy(pin, copies.data(), copies.size() * sizeof(PageCopy));
-          tsrc = pin;
+    // DELTA_BINARY_PACKED pages: their streams (neighbours a page header apart as one transfer, each transfer followed
+    // by 16 pad bytes), then the page and miniblock tables, then the decode's scratch, behind the PLAIN staging
+    struct DSpan { const uint8_t* src; uint64_t len, stage_off; };
+    std::vector<DSpan> dspans;
+    std::vector<DbpPage> dpages;
+    std::vector<DbpMini> dmbs;
+    uint64_t dstream_off = (table_off + copies.size() * sizeof(PageCopy) + 15) & ~uint64_t(15), dbytes = 0, n_groups = 0;
+    for (const DeltaPage& d : img.delta_pages) {
+      if (!dspans.empty() && d.src >= dspans.back().src + dspans.back().len && uint64_t(d.src - (dspans.back().src + dspans.back().len)) <= kGap) {
+        dspans.back().len = uint64_t(d.src - dspans.back().src) + d.len;
+      } else {
+        if (!dspans.empty()) dbytes += ((dspans.back().len + 15) & ~uint64_t(15)) + 16;
+        dspans.push_back({d.src, d.len, dstream_off + dbytes});
+      }
+      DbpPage pg{};
+      pg.dst = reinterpret_cast<unsigned long long*>(static_cast<uint8_t*>(dev) + d.hole);
+      pg.src = dspans.back().stage_off + uint64_t(d.src - dspans.back().src);
+      pg.first = static_cast<unsigned long long>(d.first);
+      pg.n = d.n;
+      pg.g0 = uint32_t(n_groups);
+      pg.mb0 = uint32_t(dmbs.size());
+      pg.per_mb = uint32_t(std::min<uint64_t>(d.per_mb, 0xffffffffu));
+      n_groups += (d.n + 31) / 32;
+      for (uint32_t m = d.mb0; m < d.mb0 + d.n_mb; m++)
+        dmbs.push_back(DbpMini{img.delta_mbs[m].min_delta, uint32_t(img.delta_mbs[m].off), img.delta_mbs[m].width});
+      dpages.push_back(pg);
+    }
+    if (!dspans.empty()) dbytes += ((dspans.back().len + 15) & ~uint64_t(15)) + 16;
+    if (n_groups > 0xffffffffull) e = cudaErrorInvalidValue;  // (more than 2^37 values in one column of one part)
+    const uint64_t dtab_off = dstream_off + dbytes, dtab_bytes = dpages.size() * sizeof(DbpPage) + dmbs.size() * sizeof(DbpMini);
+    const uint64_t dscratch_off = (dtab_off + dtab_bytes + 15) & ~uint64_t(15);
+    DevBuf stage;
+    if ((!copies.empty() || !dpages.empty()) && e == cudaSuccess) {
+      e = stage.alloc(dpages.empty() ? table_off + copies.size() * sizeof(PageCopy) : dscratch_off + dbp_scratch_bytes(uint32_t(n_groups)), ctx->stream);
+      auto upload = [&](uint64_t off, const void* src, size_t bytes) {
+        if (void* pin = ctx->arena_take(bytes)) {
+          std::memcpy(pin, src, bytes);
+          src = pin;
         }
-        e = cudaMemcpyAsync(static_cast<uint8_t*>(stage.p) + table_off, tsrc, copies.size() * sizeof(PageCopy), cudaMemcpyHostToDevice, ctx->stream);
+        return cudaMemcpyAsync(static_cast<uint8_t*>(stage.p) + off, src, bytes, cudaMemcpyHostToDevice, ctx->stream);
+      };
+      if (e == cudaSuccess && !copies.empty()) e = upload(table_off, copies.data(), copies.size() * sizeof(PageCopy));
+      if (e == cudaSuccess && !dpages.empty()) {
+        std::vector<uint8_t> tab(dtab_bytes);
+        std::memcpy(tab.data(), dpages.data(), dpages.size() * sizeof(DbpPage));
+        std::memcpy(tab.data() + dpages.size() * sizeof(DbpPage), dmbs.data(), dmbs.size() * sizeof(DbpMini));
+        e = upload(dtab_off, tab.data(), tab.size());
+        copied += dtab_bytes;
       }
     }
     for (const Span& sp : spans) {
@@ -698,8 +736,19 @@ int32_t ensure_resident(fgpu_ctx* ctx, Table* table, Part* part, const std::stri
       if (sp.n == 1) e = cudaMemcpyAsync(static_cast<uint8_t*>(dev) + img.extents[sp.first].dst_off, sp.src, sp.len, cudaMemcpyHostToDevice, ctx->stream);
       else e = cudaMemcpyAsync(static_cast<uint8_t*>(stage.p) + sp.stage_off, sp.src, sp.len, cudaMemcpyHostToDevice, ctx->stream);
     }
+    for (const DSpan& sp : dspans) {
+      if (e != cudaSuccess) break;
+      copied += sp.len;
+      e = cudaMemcpyAsync(static_cast<uint8_t*>(stage.p) + sp.stage_off, sp.src, sp.len, cudaMemcpyHostToDevice, ctx->stream);
+    }
     if (e == cudaSuccess && !copies.empty())
       e = launch_gather_pages(stage.p, dev, reinterpret_cast<const PageCopy*>(static_cast<uint8_t*>(stage.p) + table_off), uint32_t(copies.size()), ctx->stream);
+    if (e == cudaSuccess && !dpages.empty()) {
+      const uint8_t* base = static_cast<const uint8_t*>(stage.p);
+      e = launch_dbp_decode(base, reinterpret_cast<const DbpPage*>(base + dtab_off), uint32_t(dpages.size()),
+                            reinterpret_cast<const DbpMini*>(base + dtab_off + dpages.size() * sizeof(DbpPage)), uint32_t(n_groups),
+                            static_cast<uint8_t*>(stage.p) + dscratch_off, ctx->stream);
+    }
     // `stage` is released in stream order when it goes out of scope
   }
   if (e == cudaSuccess) e = launch_str_jobs(ctx, img, dev);
@@ -947,6 +996,8 @@ void release_staging(fgpu_ctx* ctx) {
   for (ColumnImage* img : ctx->pending_uploads) {
     std::vector<uint8_t>().swap(img->meta);
     std::vector<Extent>().swap(img->extents);
+    std::vector<DeltaPage>().swap(img->delta_pages);
+    std::vector<DbpMiniblock>().swap(img->delta_mbs);
   }
   ctx->pending_uploads.clear();
 }

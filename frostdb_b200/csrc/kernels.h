@@ -50,6 +50,11 @@ cudaError_t launch_str_hash(const StrChunk* d_chunks, uint32_t n_chunks, uint32_
 cudaError_t launch_str_compact(const StrChunk* d_chunks, uint32_t n_chunks, uint32_t total_slots, uint32_t* d_counts, cudaStream_t st);
 cudaError_t launch_str_gather(const StrChunk* d_chunks, uint32_t n_chunks, uint32_t total_slots, cudaStream_t st);
 cudaError_t launch_str_codes(const StrCodeJob* d_jobs, uint32_t n_jobs, uint32_t total_groups, cudaStream_t st);
+// DELTA_BINARY_PACKED int64 pages -> dense values (delta_int64.cu): three launches per upload whatever its pages.
+// `scratch`: dbp_scratch_bytes(n_groups) bytes, 8-byte aligned
+size_t dbp_scratch_bytes(uint32_t n_groups);
+cudaError_t launch_dbp_decode(const uint8_t* stage, const DbpPage* d_pages, uint32_t n_pages, const DbpMini* d_mbs, uint32_t n_groups,
+                              void* scratch, cudaStream_t st);
 // partial-table exchange over peer-mapped mailboxes (comm.cu)
 cudaError_t launch_comm_push(const CommPush& p, int sm_count, cudaStream_t st);
 cudaError_t launch_comm_wait(const CommWait& w, cudaStream_t st);

@@ -679,7 +679,7 @@ bool read_uleb(const uint8_t*& p, const uint8_t* end, uint64_t* v) {
 }  // namespace
 
 template <typename T>
-bool decode_delta_binary_packed(const uint8_t* data, uint64_t len, uint32_t count, std::vector<T>* out, uint64_t* used, std::string* err) {
+bool parse_delta_binary_packed(const uint8_t* data, uint64_t len, uint32_t count, DbpStream* out, std::string* err) {
   using U = typename std::make_unsigned<T>::type;
   constexpr uint32_t kBits = 8 * sizeof(T);
   const uint8_t* p = data;
@@ -695,44 +695,73 @@ bool decode_delta_binary_packed(const uint8_t* data, uint64_t len, uint32_t coun
   if (total != count) { *err = "DELTA_BINARY_PACKED value count differs from the page's values"; return false; }
   const uint64_t per_mb = block / n_mb;
   if (per_mb > (uint64_t(1) << 40) && count > 1) { *err = overrun; return false; }  // (a miniblock larger than any page)
-  out->clear();
-  out->reserve(count);
-  U v = U((first >> 1) ^ (~(first & 1) + 1));  // zigzag, wrapped to the value width
-  if (count > 0) out->push_back(T(v));
-  while (out->size() < count) {
+  out->first = uint64_t(U((first >> 1) ^ (~(first & 1) + 1)));  // zigzag, wrapped to the value width
+  out->count = count;
+  out->per_mb = per_mb;
+  out->mbs.clear();
+  uint64_t produced = count > 0 ? 1 : 0;
+  while (produced < count) {
     uint64_t zmin = 0;
     if (!read_uleb(p, end, &zmin)) { *err = overrun; return false; }
-    const U min_delta = U((zmin >> 1) ^ (~(zmin & 1) + 1));
+    const uint64_t min_delta = uint64_t(U((zmin >> 1) ^ (~(zmin & 1) + 1)));
     if (uint64_t(end - p) < n_mb) { *err = overrun; return false; }
     const uint8_t* widths = p;
     p += n_mb;
-    for (uint64_t m = 0; m < n_mb && out->size() < count; m++) {
+    for (uint64_t m = 0; m < n_mb && produced < count; m++) {
       const uint32_t w = widths[m];
       if (w > kBits) { *err = "DELTA_BINARY_PACKED miniblock bit width > " + std::to_string(kBits); return false; }
       const uint64_t bytes = per_mb * w / 8;  // a miniblock holding values is written whole (padding included)
       if (uint64_t(end - p) < bytes) { *err = overrun; return false; }
-      const uint64_t take = std::min<uint64_t>(per_mb, count - out->size());
-      for (uint64_t i = 0; i < take; i++) {
-        uint64_t d = 0;
-        if (w) {  // LSB first; a 64-bit value at an odd bit position spans 9 bytes
-          const uint64_t b0 = (i * w) >> 3, avail = bytes - b0;
-          const unsigned sh = unsigned((i * w) & 7);
-          uint64_t window = 0;
-          for (uint64_t k = 0; k < std::min<uint64_t>(8, avail); k++) window |= uint64_t(p[b0 + k]) << (8 * k);
-          d = window >> sh;
-          if (sh && avail > 8) d |= uint64_t(p[b0 + 8]) << (64 - sh);
-          if (w < 64) d &= (uint64_t(1) << w) - 1;
-        }
-        v = U(v + min_delta + U(d));
-        out->push_back(T(v));
-      }
+      const uint64_t take = std::min<uint64_t>(per_mb, count - produced);
+      out->mbs.push_back(DbpMiniblock{uint64_t(p - data), min_delta, uint32_t(produced), uint32_t(take), w});
+      produced += take;
       p += bytes;
     }
   }
-  *used = uint64_t(p - data);
+  out->used = uint64_t(p - data);
   return true;
 }
 
+template <typename T>
+void unpack_delta_binary_packed(const uint8_t* data, T first, const DbpMiniblock* mbs, size_t n_mbs, uint32_t ord0, T* out) {
+  using U = typename std::make_unsigned<T>::type;
+  U v = U(first);
+  out[0] = first;
+  for (size_t m = 0; m < n_mbs; m++) {
+    const DbpMiniblock& mb = mbs[m];
+    const uint8_t* p = data + mb.off;
+    const uint32_t w = mb.width;
+    const uint64_t bytes = (uint64_t(mb.count) * w + 7) / 8;  // (the bytes its values need: the padding is not read)
+    T* dst = out + (mb.first - ord0);
+    for (uint64_t i = 0; i < mb.count; i++) {
+      uint64_t d = 0;
+      if (w) {  // LSB first; a 64-bit value at an odd bit position spans 9 bytes
+        const uint64_t b0 = (i * w) >> 3, avail = bytes - b0;
+        const unsigned sh = unsigned((i * w) & 7);
+        uint64_t window = 0;
+        for (uint64_t k = 0; k < std::min<uint64_t>(8, avail); k++) window |= uint64_t(p[b0 + k]) << (8 * k);
+        d = window >> sh;
+        if (sh && avail > 8) d |= uint64_t(p[b0 + 8]) << (64 - sh);
+        if (w < 64) d &= (uint64_t(1) << w) - 1;
+      }
+      v = U(v + U(mb.min_delta) + U(d));
+      dst[i] = T(v);
+    }
+  }
+}
+
+template <typename T>
+bool decode_delta_binary_packed(const uint8_t* data, uint64_t len, uint32_t count, std::vector<T>* out, uint64_t* used, std::string* err) {
+  DbpStream s;
+  if (!parse_delta_binary_packed<T>(data, len, count, &s, err)) return false;
+  out->assign(count, T(0));
+  if (count > 0) unpack_delta_binary_packed<T>(data, T(s.first), s.mbs.data(), s.mbs.size(), 0, out->data());
+  *used = s.used;
+  return true;
+}
+
+template bool parse_delta_binary_packed<int64_t>(const uint8_t*, uint64_t, uint32_t, DbpStream*, std::string*);
+template void unpack_delta_binary_packed<int64_t>(const uint8_t*, int64_t, const DbpMiniblock*, size_t, uint32_t, int64_t*);
 template bool decode_delta_binary_packed<int32_t>(const uint8_t*, uint64_t, uint32_t, std::vector<int32_t>*, uint64_t*, std::string*);
 
 

@@ -111,11 +111,39 @@ bool walk_hybrid(const uint8_t* data, uint32_t len, int w, uint32_t count, uint3
 // Reads value i of a hybrid stream described by runs (host-side reference used by describe/tests).
 uint32_t hybrid_value_at(const uint8_t* stream, const std::vector<HostRun>& runs, uint32_t ordinal, bool* was_rle = nullptr);
 
-// Decodes one DELTA_BINARY_PACKED stream of `count` values of type T (int32_t: the length streams of
-// DELTA_LENGTH_BYTE_ARRAY / DELTA_BYTE_ARRAY pages), with the format's wrap-around arithmetic, from `data`.
-// Validates the header (block size a multiple of 128, values per miniblock a multiple of 32, total == count),
-// the bit width of every miniblock that holds values (<= the bits of T) and that nothing runs past `len`.
-// `used`: the stream's bytes (miniblocks holding values are whole; the unused ones of the last block are absent).
+// One miniblock of a DELTA_BINARY_PACKED stream that holds values.
+struct DbpMiniblock {
+  uint64_t off;        // byte offset of its packed deltas from the stream's start
+  uint64_t min_delta;  // its block's min delta, wrapped to the value type
+  uint32_t first;      // ordinal of the value its first delta makes (>= 1: value 0 is the header's first value)
+  uint32_t count;      // values it makes
+  uint32_t width;      // bit width of its deltas
+};
+
+// What the parse step of a DELTA_BINARY_PACKED stream leaves: the header and the miniblocks holding values.
+struct DbpStream {
+  uint64_t first = 0;   // the first value, wrapped to the value type
+  uint32_t count = 0;   // values in the stream
+  uint64_t per_mb = 0;  // values per miniblock
+  uint64_t used = 0;    // the stream's bytes (miniblocks holding values are whole; the unused ones of the last block are absent)
+  std::vector<DbpMiniblock> mbs;
+};
+
+// Parse step of one DELTA_BINARY_PACKED stream of `count` values of type T, without unpacking a delta.  Validates the
+// header (block size a multiple of 128, values per miniblock a multiple of 32, total == count), the bit width of every
+// miniblock that holds values (<= the bits of T) and that no header, width list or miniblock (written whole) runs
+// past `len`.
+template <typename T>
+bool parse_delta_binary_packed(const uint8_t* data, uint64_t len, uint32_t count, DbpStream* out, std::string* err);
+
+// Unpack step: the values of the miniblocks `mbs[0, n_mbs)` of a parsed stream at `data`, with the format's wrap-around
+// arithmetic.  out[0] = first; the deltas of a miniblock make out[mb.first - ord0, + mb.count) (ord0: 0 for a parse
+// result, the page's first ordinal for miniblocks rebased onto a chunk's value ordinals).
+template <typename T>
+void unpack_delta_binary_packed(const uint8_t* data, T first, const DbpMiniblock* mbs, size_t n_mbs, uint32_t ord0, T* out);
+
+// Parse and unpack step of one stream (int32_t: the length streams of DELTA_LENGTH_BYTE_ARRAY / DELTA_BYTE_ARRAY pages).
+// `used`: DbpStream::used.
 template <typename T>
 bool decode_delta_binary_packed(const uint8_t* data, uint64_t len, uint32_t count, std::vector<T>* out, uint64_t* used, std::string* err);
 

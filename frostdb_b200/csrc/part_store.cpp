@@ -57,7 +57,16 @@ struct ImageWriter {
       extents.push_back({src, len, ext_size});
     ext_size += len;
   }
+  // reserves `len` bytes of the extent region without a copy (the device writes them); returns their offset in it
+  uint64_t add_hole(uint64_t len) {
+    const uint64_t off = ext_size;
+    ext_size += len;
+    return off;
+  }
   void end_extent() { ext_size += kTailPad; }
+  // DELTA_BINARY_PACKED pages whose holes the device fills (the image's lists; null: the image has none)
+  std::vector<DeltaPage>* delta_pages = nullptr;
+  std::vector<DbpMiniblock>* delta_mbs = nullptr;
 };
 
 inline void or_bits(std::vector<uint64_t>& bm, uint64_t pos, uint64_t bits8) {
@@ -195,6 +204,25 @@ bool walk_delta_strings(const PageInfo& pg, uint32_t n, ChunkWalk* wk, std::stri
   return true;
 }
 
+// One DELTA_BINARY_PACKED page of an INT64 chunk holding `n` non-null values, the chunk's values [v0, v0 + n): parsed
+// and validated, not unpacked (the host's work is per miniblock; the device unpacks at upload).
+bool walk_delta_int64(const PageInfo& pg, uint32_t n, uint32_t v0, ChunkWalk* wk, std::string* err) {
+  DbpStream s;
+  if (!parse_delta_binary_packed<int64_t>(pg.values, pg.values_len, n, &s, err)) {
+    *err = "int64 values: " + *err;
+    return false;
+  }
+  if (n == 0) return true;
+  const DeltaPage d{pg.values, s.used, int64_t(s.first), v0, n, s.per_mb, uint32_t(wk->delta_mbs.size()), uint32_t(s.mbs.size())};
+  for (DbpMiniblock& mb : s.mbs) {
+    mb.first += v0;
+    wk->delta_mbs.push_back(mb);
+  }
+  wk->plain64.push_back({pg.values, n, int32_t(wk->delta_pages.size())});
+  wk->delta_pages.push_back(d);
+  return true;
+}
+
 }  // namespace
 
 void unfront_strings(ChunkWalk* wk) {
@@ -239,7 +267,9 @@ void walk_chunk(const ChunkMeta& cm, const SchemaLeaf& leaf, uint32_t n_rows, Ch
   bool any_dict = false, any_plain = false;
   for (const PageInfo& pg : cm.pages) {
     if (is_dict_encoding(pg.encoding)) any_dict = true;
-    else if (pg.encoding == ENC_PLAIN || (leaf.phys == PT_BYTE_ARRAY && is_delta_string(pg.encoding))) any_plain = true;
+    else if (pg.encoding == ENC_PLAIN || (leaf.phys == PT_BYTE_ARRAY && is_delta_string(pg.encoding)) ||
+             (leaf.phys == PT_INT64 && pg.encoding == ENC_DELTA_BINARY_PACKED))
+      any_plain = true;
     else { out->error = "unsupported page encoding " + std::to_string(pg.encoding); return; }
   }
   // (a string chunk may hold both: a dictionary whose writer fell back to PLAIN part of the way through)
@@ -350,11 +380,18 @@ void walk_chunk(const ChunkMeta& cm, const SchemaLeaf& leaf, uint32_t n_rows, Ch
         for (uint32_t i = f.v0; i < f.v0 + f.n; i++) wk->str_off[i] += uint32_t(rb0);
     }
   } else {
+    uint32_t vo = 0;
     for (size_t p = 0; p < cm.pages.size(); p++) {
       const PageInfo& pg = cm.pages[p];
+      if (pg.encoding == ENC_DELTA_BINARY_PACKED) {  // (INT64 only: the encoding check above refuses it elsewhere)
+        if (!walk_delta_int64(pg, page_nn[p], vo, wk, &err)) { out->error = err; return; }
+        vo += page_nn[p];
+        continue;
+      }
       uint64_t need = uint64_t(page_nn[p]) * 8;
       if (need > pg.values_len) { out->error = "PLAIN page shorter than its value count"; return; }
-      wk->plain64.push_back({pg.values, page_nn[p]});
+      wk->plain64.push_back({pg.values, page_nn[p], -1});
+      vo += page_nn[p];
     }
     out->desc.kind = CK_PLAIN64;
   }
@@ -526,10 +563,19 @@ void write_chunk(ChunkWalk& wk, uint32_t n_rows, int tile_rows, GlobalDict* dict
   uint64_t plain_bytes = 0;
   if (out->desc.kind == CK_PLAIN64) {
     // value regions go to the device straight from the file: negative offsets mark "extent region"
+    // (a DELTA_BINARY_PACKED page's values are a hole where its PLAIN twin's would be copied to)
     const uint64_t eoff = w.begin_extent();
-    for (const auto& pg : wk.plain64) {
-      w.add_extent(pg.first, uint64_t(pg.second) * 8);
-      plain_bytes += uint64_t(pg.second) * 8;
+    for (const Page64& pg : wk.plain64) {
+      if (pg.delta < 0) {
+        w.add_extent(pg.values, uint64_t(pg.n) * 8);
+        plain_bytes += uint64_t(pg.n) * 8;
+        continue;
+      }
+      DeltaPage d = wk.delta_pages[size_t(pg.delta)];
+      d.hole = w.add_hole(uint64_t(pg.n) * 8);  // relative to the extent region until finish_image rebases it
+      w.delta_pages->push_back(d);
+      w.delta_pages->back().mb0 = uint32_t(w.delta_mbs->size());
+      w.delta_mbs->insert(w.delta_mbs->end(), wk.delta_mbs.begin() + d.mb0, wk.delta_mbs.begin() + d.mb0 + d.n_mb);
     }
     w.end_extent();
     out->off_values = -int64_t(eoff) - 1;
@@ -657,6 +703,7 @@ void finish_image(ImageWriter& w, ColumnImage& img, Part* part, const std::strin
   const uint64_t meta_size = (img.meta.size() + kAlign - 1) / kAlign * kAlign;
   const uint64_t dev_base = (meta_size + w.ext_size + kAlign - 1) / kAlign * kAlign;
   for (Extent& e : img.extents) e.dst_off += meta_size;
+  for (DeltaPage& d : img.delta_pages) d.hole += meta_size;
   for (RowGroupHost& h : part->rgs) {
     ChunkHost& ch = h.cols[column];
     if (ch.off_values < -0) ch.off_values = int64_t(meta_size) + (-ch.off_values - 1);
@@ -749,6 +796,8 @@ void finish_column(int index_rows, Table* table, Part* part, const std::string& 
     if (l.name == column && l.phys == PT_BYTE_ARRAY) dict = &table->dicts[column];
   ImageWriter w(img.meta, img.extents);
   w.device_seeds = img.device_seeds;
+  w.delta_pages = &img.delta_pages;
+  w.delta_mbs = &img.delta_mbs;
   for (size_t g = 0; g < part->rgs.size(); g++) {
     RowGroupHost& h = part->rgs[g];
     ChunkHost ch;
@@ -1042,6 +1091,9 @@ std::string describe_part_json(const uint8_t* file, uint64_t len, int tile_rows,
     std::vector<uint8_t> flat(size_t(img.dev_bytes), 0);
     std::memcpy(flat.data(), img.meta.data(), img.meta.size());
     for (const Extent& e : img.extents) std::memcpy(flat.data() + e.dst_off, e.src, size_t(e.len));
+    for (const DeltaPage& d : img.delta_pages)  // the holes the device fills at upload
+      unpack_delta_binary_packed<int64_t>(d.src, d.first, img.delta_mbs.data() + d.mb0, d.n_mb, d.v0,
+                                          reinterpret_cast<int64_t*>(flat.data() + d.hole));
     host_images.push_back(std::move(flat));
     patch_column_pointers(&part, name, host_images.back().data());  // pointers into the host image
     image_bytes += img.dev_bytes;

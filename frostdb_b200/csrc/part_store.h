@@ -86,12 +86,12 @@ struct ChunkHost {
   // flat code array of a CK_DICT_STR chunk (device pointer; derived on first use by k_flatten, see tile_agg.cu)
   const uint8_t* flat = nullptr;
   uint8_t flat_w = 0, flat_bias = 0;
-  // frame-of-reference image of a PLAIN non-null INT64 chunk whose range fits 32 bits (device pointer; derived on first
+  // frame-of-reference image of a dense (CK_PLAIN64) non-null INT64 chunk whose range fits 32 bits (device pointer; derived on first
   // use by the sorted-run kernel, see ensure_narrow): narrow_w bytes per row holding value - narrow_base
   const uint8_t* narrow = nullptr;
   uint8_t narrow_w = 0;
   int64_t narrow_base = 0;
-  // exclusive prefix sums of a PLAIN non-null INT64 chunk, n_rows + 1 entries modulo 2^64 (device pointer; derived on
+  // exclusive prefix sums of a dense (CK_PLAIN64) non-null INT64 chunk, n_rows + 1 entries modulo 2^64 (device pointer; derived on
   // first use by the prefix path of the sorted-run scan, see ensure_narrow)
   const long long* prefix = nullptr;
 };
@@ -123,6 +123,25 @@ struct StrFront {
   uint32_t v0, d0, w0, n;  // first value; its index in str_pre / str_suf; the page's first window in str_wmin; values
 };
 
+// One DELTA_BINARY_PACKED page of an INT64 chunk: its dense values [v0, v0 + n) are a hole of 8 * n bytes in the
+// chunk's value array, which the device fills at upload from the page's stream (delta_int64.cu).
+struct DeltaPage {
+  const uint8_t* src;   // its encoded stream (in the file)
+  uint64_t len;         // bytes of the stream (what follows it in the page is not read)
+  int64_t first;        // its first value
+  uint32_t v0, n;       // its non-null values: ordinals among the chunk's values
+  uint64_t per_mb;      // values per miniblock
+  uint32_t mb0, n_mb;   // its miniblocks holding values, in the walk's (then the image's) miniblock list
+  uint64_t hole = 0;    // once the sections are written: image offset of its values
+};
+
+// One page of a CK_PLAIN64 chunk: PLAIN (its value region in the file) or DELTA_BINARY_PACKED (an index into delta_pages).
+struct Page64 {
+  const uint8_t* values;
+  uint32_t n;
+  int32_t delta;  // -1: PLAIN
+};
+
 // What the page walk of one chunk leaves for the section writing (the two halves of building a column).
 struct ChunkWalk {
   ChunkHost host;                 // footer facts, kind, error
@@ -134,7 +153,9 @@ struct ChunkWalk {
   std::vector<HostRun> vruns;     // a PLAIN page's entry holds its hole's position in `vstream` until the holes exist
   std::vector<std::pair<const uint8_t*, uint32_t>> dict_entries;  // string dictionary page, validated
   std::vector<int64_t> dict64;
-  std::vector<std::pair<const uint8_t*, uint32_t>> plain64;  // PLAIN int64 / double pages: value region, values
+  std::vector<Page64> plain64;           // pages of an int64 / double chunk, in file order
+  std::vector<DeltaPage> delta_pages;    // its DELTA_BINARY_PACKED pages
+  std::vector<DbpMiniblock> delta_mbs;   // their miniblocks holding values, `first` rebased onto the chunk's value ordinals
   // Non-dictionary string values (PLAIN, DELTA_LENGTH_BYTE_ARRAY, DELTA_BYTE_ARRAY pages), validated: every value lies
   // inside its page.  They are addressed in one 32-bit space per chunk: [0, str_span) the file bytes from str_base,
   // [str_rb0, str_rb0 + str_rebuilt_len) the DELTA_BYTE_ARRAY values rebuilt from their prefixes and suffixes.
@@ -179,6 +200,10 @@ struct ColumnImage {
   bool device_seeds = false;
   std::vector<ChunkWalk> walks;  // per row group, between the walk and the section writing
   std::vector<StrCodeJob> str_jobs;  // PLAIN string pages whose indices the device writes at upload (dst: image offset)
+  // DELTA_BINARY_PACKED int64 pages of every chunk, whose values the device writes at upload (DeltaPage::hole: image
+  // offset), and their miniblocks (DeltaPage::mb0 indexes this list); kept until uploaded
+  std::vector<DeltaPage> delta_pages;
+  std::vector<DbpMiniblock> delta_mbs;
   bool built = false;      // host side done (ChunkHosts filled, dictionary interned)
   bool resident = false;   // bytes are on the device
   void* dev = nullptr;

@@ -31,6 +31,7 @@ class ColumnDefinition:
     nullable: bool = False
     dynamic: bool = False
     rle_dictionary: bool = False
+    delta_binary_packed: bool = False  # StorageLayout_ENCODING_DELTA_BINARY_PACKED (int64 columns only)
 
 
 @dataclasses.dataclass
@@ -201,10 +202,12 @@ def write_part(schema: Schema, columns: Dict[str, object], *, sort: bool = True,
         nullable = defn.nullable
         if not nullable and arr.null_count:
             raise ValueError(f"column {n} is not nullable but has NULLs")
+        if defn.delta_binary_packed and defn.type != TYPE_INT64:
+            raise ValueError(f"column {n}: DELTA_BINARY_PACKED needs an int64 column, not {defn.type}")
         if defn.type == TYPE_STRING and defn.rle_dictionary:
             dict_cols.append(n)
         else:
-            plain_cols[n] = "PLAIN"
+            plain_cols[n] = "DELTA_BINARY_PACKED" if defn.delta_binary_packed else "PLAIN"
         if defn.dynamic:
             dyn.setdefault(defn.name, []).append(n.split(".", 1)[1])
         fields.append(pa.field(n, arr.type, nullable=nullable))

@@ -200,6 +200,9 @@ enum {
  * directories, chunk seeds, global dictionary ids) and uploads it, and the caller may free the
  * buffer on return.  FGPU_PUT_BORROW_PINNED keeps the pointer instead: a column is built and
  * uploaded by the first query that projects it, its PLAIN pages DMA'd straight from `file`.
+ * DELTA_BINARY_PACKED int64 pages travel encoded and are decoded on the device into the same dense
+ * value array as PLAIN pages; a chunk the engine cannot read (compressed, a malformed page, an
+ * unsupported encoding) fails only the queries that project its column, with FGPU_ERR_UNSUPPORTED.
  * `tx` is the part's transaction id (parts.Part.TX()). */
 int32_t fgpu_part_put_parquet(fgpu_ctx* ctx, const char* table, uint64_t part_id, uint64_t tx,
                               const uint8_t* file, uint64_t len, int32_t flags);
