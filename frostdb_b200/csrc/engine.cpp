@@ -8,7 +8,6 @@
 
 #include <algorithm>
 #include <array>
-#include <atomic>
 #include <chrono>
 #include <cmath>
 #include <cstdio>
@@ -22,61 +21,19 @@
 #include <set>
 #include <sstream>
 #include <string>
-#include <thread>
 #include <vector>
 
 #include "../../include/frostgpu.h"
 #include "arrow_export.h"
+#include "context.h"
 #include "device_types.h"
 #include "kernels.h"
 #include "part_store.h"
+#include "residency.h"
 
 using namespace fgpu;
 
 namespace {
-
-thread_local std::string g_err;
-
-int32_t fail(int32_t code, const std::string& msg) {
-  g_err = msg;
-  return code;
-}
-
-#define CUDA_TRY(expr)                                                                         \
-  do {                                                                                         \
-    cudaError_t _e = (expr);                                                                   \
-    if (_e != cudaSuccess) {                                                                   \
-      cudaGetLastError();                                                                      \
-      return fail(_e == cudaErrorMemoryAllocation ? FGPU_ERR_OOM : FGPU_ERR_CUDA,              \
-                  std::string(#expr) + ": " + cudaGetErrorString(_e));                         \
-    }                                                                                          \
-  } while (0)
-
-// Stream-ordered device allocation (cudaMallocAsync on the engine stream, pool kept warm): a query's
-// scratch and a streamed part's columns cost microseconds to allocate instead of a cudaMalloc each.
-struct DevBuf {
-  void* p = nullptr;
-  size_t n = 0;
-  cudaStream_t st = nullptr;
-  DevBuf() = default;
-  DevBuf(const DevBuf&) = delete;
-  DevBuf& operator=(const DevBuf&) = delete;
-  ~DevBuf() { reset(); }
-  void reset() {
-    if (p) cudaFreeAsync(p, st);
-    p = nullptr;
-    n = 0;
-  }
-  cudaError_t alloc(size_t bytes, cudaStream_t stream) {
-    reset();
-    st = stream;
-    if (bytes == 0) bytes = 16;
-    cudaError_t e = cudaMallocAsync(&p, bytes, stream);
-    if (e == cudaSuccess) n = bytes;
-    else p = nullptr;
-    return e;
-  }
-};
 
 struct ExprNode {
   int32_t kind = 0, op = 0, left = -1, right = -1;
@@ -124,46 +81,6 @@ const char* agg_string(int f) {  // logicalplan.AggFunc.String(), expr.go:731-75
 
 }  // namespace
 
-// Page-locked host blocks, recycled: result images of cached plans and the columns of large results (which the
-// Arrow consumer holds until it releases the array, possibly after the context is gone: the pool is shared-owned).
-// Freeing page-locked memory synchronises the device, so blocks are only released when the pool itself dies.
-struct PinnedPool {
-  std::mutex mu;
-  std::multimap<size_t, uint8_t*> free_blocks;
-  size_t free_bytes = 0;
-  ~PinnedPool() {
-    for (auto& kv : free_blocks) cudaFreeHost(kv.second);
-  }
-  uint8_t* take(size_t bytes, size_t* cap) {
-    size_t want = 4096;
-    while (want < bytes) want <<= 1;
-    if (bytes > (size_t(1) << 24)) want = (bytes + (size_t(1) << 22) - 1) & ~((size_t(1) << 22) - 1);  // large blocks: 4 MiB granules
-    {
-      std::lock_guard<std::mutex> lk(mu);
-      auto it = free_blocks.lower_bound(want);
-      if (it != free_blocks.end() && it->first <= want * 2) {
-        uint8_t* p = it->second;
-        *cap = it->first;
-        free_bytes -= it->first;
-        free_blocks.erase(it);
-        return p;
-      }
-    }
-    uint8_t* p = nullptr;
-    if (cudaHostAlloc(reinterpret_cast<void**>(&p), want, cudaHostAllocDefault) != cudaSuccess) {
-      cudaGetLastError();
-      return nullptr;
-    }
-    *cap = want;
-    return p;
-  }
-  void give(uint8_t* p, size_t cap) {
-    std::lock_guard<std::mutex> lk(mu);
-    free_blocks.emplace(cap, p);
-    free_bytes += cap;
-  }
-};
-
 // Mailbox communicator of one rank (see comm.cu).
 struct CommHandle {  // what travels between the ranks (FGPU_COMM_HANDLE_BYTES)
   uint32_t magic;
@@ -174,67 +91,6 @@ struct CommHandle {  // what travels between the ranks (FGPU_COMM_HANDLE_BYTES)
 };
 static_assert(sizeof(CommHandle) <= FGPU_COMM_HANDLE_BYTES, "handle fits its blob");
 constexpr uint32_t kCommMagic = 0x46474d42u;  // "FGMB"
-constexpr size_t kCommDataOff = 4096;        // flags live in front of the slots
-
-struct Comm {
-  int rank = -1, n = 0;
-  uint64_t slot_bytes = 0, total = 0, seq = 0;
-  uint8_t* mailbox = nullptr;  // [flags: 2 sets x kMaxRanks x {seq, bytes}] ... [2 sets x n slots]
-  bool open = false;
-  uint8_t* peer[kMaxRanks] = {nullptr};
-  bool peer_ipc[kMaxRanks] = {false};
-  size_t flag_off(uint64_t set, int r) const { return (size_t(set) * kMaxRanks + size_t(r)) * 16; }
-  size_t data_off(uint64_t set, int r) const { return kCommDataOff + (size_t(set) * size_t(n) + size_t(r)) * slot_bytes; }
-};
-
-struct fgpu_ctx {
-  Comm comm;
-  int device = 0;
-  int sm_count = 132;
-  int tile_rows = kTileRows;
-  cudaStream_t stream = nullptr;
-  cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
-  std::mutex mu;
-  std::map<std::string, Table> tables;
-  std::vector<ColumnImage*> pending_uploads;  // staging to release after the next stream sync
-  uint64_t epoch_counter = 0;                 // source of Table::epoch stamps
-  std::map<std::string, std::shared_ptr<struct QueryPlan>> plans;  // by plan signature (bounded, see fgpu_query_prepare)
-  // page-locked arena for column metadata on its way to the device: a pageable source would make every
-  // cudaMemcpyAsync wait for the transfers queued before it.  Reset by release_staging() after a sync.
-  uint8_t* arena = nullptr;
-  size_t arena_cap = 0, arena_used = 0;
-  void* arena_take(size_t n) {
-    if (!arena) {
-      size_t want = size_t(64) << 20;
-      if (cudaHostAlloc(reinterpret_cast<void**>(&arena), want, cudaHostAllocDefault) != cudaSuccess) {
-        cudaGetLastError();
-        arena = nullptr;
-        return nullptr;
-      }
-      arena_cap = want;
-    }
-    size_t off = (arena_used + 63) & ~size_t(63);
-    if (off + n > arena_cap) return nullptr;  // caller falls back to the pageable source
-    arena_used = off + n;
-    return arena + off;
-  }
-  std::shared_ptr<PinnedPool> pinned = std::make_shared<PinnedPool>();
-  uint8_t* pinned_take(size_t bytes, size_t* cap) { return pinned->take(bytes, cap); }
-  void pinned_give(uint8_t* p, size_t cap) { pinned->give(p, cap); }
-  // page-locked scratch for the per-query descriptor upload and the counters read-back (guarded by mu)
-  uint8_t* scratch = nullptr;
-  size_t scratch_bytes = 0;
-  cudaError_t ensure_scratch(size_t bytes) {
-    if (bytes <= scratch_bytes) return cudaSuccess;
-    if (scratch) cudaFreeHost(scratch);
-    scratch = nullptr;
-    scratch_bytes = 0;
-    size_t want = std::max<size_t>(bytes * 2, 1 << 20);
-    cudaError_t e = cudaHostAlloc(reinterpret_cast<void**>(&scratch), want, cudaHostAllocDefault);
-    if (e == cudaSuccess) scratch_bytes = want;
-    return e;
-  }
-};
 
 // The FROSTGPU_* development switches (tests and measurements use them to force a kernel or a layout), parsed.  A
 // NO_* switch, TA_GLOBAL, TA_CARRY and PROFILE are on when they are set at all.  `key` lists every switch that is set
@@ -391,625 +247,6 @@ struct fgpu_result {
 };
 
 namespace {
-
-// Device scratch of one intern batch (intern_plain_strings): the images of the columns it finished hold StrCodeJobs
-// into it until ensure_resident launches them.  Freed in stream order when the batch goes; a finished column whose
-// jobs were never launched (its upload did not happen) is reset to unbuilt, so that it is interned again when needed.
-struct StrBatch {
-  DevBuf scratch;
-  std::vector<std::pair<Part*, std::string>> cols;
-  StrBatch() = default;
-  StrBatch(const StrBatch&) = delete;
-  StrBatch& operator=(const StrBatch&) = delete;
-  ~StrBatch() {
-    for (auto& [part, col] : cols) {
-      ColumnImage& img = part->images[col];
-      if (!img.str_jobs.empty() && !img.resident) img = ColumnImage{};
-    }
-  }
-};
-
-// Non-dictionary string pages of every listed column that walk_column left walked but not built, interned on the device
-// in one batch (intern_strings.cu): the chunks' value regions and value addresses go up with one transfer per contiguous
-// span, k_str_unfront rebuilds the DELTA_BYTE_ARRAY values behind their chunk's file bytes, k_str_hash and k_str_compact
-// leave every distinct value's first occurrence in page-locked memory, k_str_gather (batches with DELTA_BYTE_ARRAY
-// values only) copies the distinct rebuilt values there too, and after the one synchronisation the host interns the
-// new strings in order of first occurrence (finish_column), uploads the chunk-local index of every distinct value and
-// queues one StrCodeJob per page on the column's image.
-int32_t intern_plain_strings(fgpu_ctx* ctx, Table* table, const std::vector<std::pair<Part*, std::string>>& cols, StrBatch* batch) {
-  struct Item {
-    ChunkWalk* wk;
-    uint64_t v0, s0, cap, byte_off;
-    uint64_t l0, d0, w0, r0;  // in the batch's lengths, prefix / suffix, window and rebuilt-value arrays
-  };
-  std::vector<Item> items;
-  std::vector<std::pair<Part*, std::string>> todo;
-  uint64_t nv = 0, ns = 0, nl = 0, nd = 0, nw = 0, nr = 0, n_fronts = 0;
-  for (const auto& pc : cols) {
-    ColumnImage& img = pc.first->images[pc.second];
-    if (!img.walked || img.built) continue;
-    todo.push_back(pc);
-    for (ChunkWalk& wk : img.walks) {
-      if (!wk.host.error.empty() || wk.str_off.empty()) continue;
-      uint64_t cap = 16;
-      while (cap < 2 * uint64_t(wk.str_off.size())) cap <<= 1;
-      items.push_back({&wk, nv, ns, cap, 0, nl, nd, nw, nr});
-      nv += wk.str_off.size();
-      ns += cap;
-      nl += wk.str_len.size();
-      nd += wk.str_pre.size();
-      nw += wk.str_wmin.size();
-      if (!wk.str_fronts.empty()) nr += (wk.str_rebuilt_len + 15) & ~uint64_t(15);
-      for (const StrFront& f : wk.str_fronts) n_fronts += (f.n + kFrontSeg - 1) / kFrontSeg;
-    }
-  }
-  if (todo.empty()) return FGPU_OK;
-  batch->cols.insert(batch->cols.end(), todo.begin(), todo.end());
-  if (ns > 0xffffffffull) return fail(FGPU_ERR_UNSUPPORTED, "PLAIN string values of one upload exceed 2^31");
-  // value regions: neighbouring chunks' regions (a few page headers apart) travel as one transfer; a chunk with
-  // DELTA_BYTE_ARRAY values ends its span, and its rebuilt values follow at str_rb0 from its first byte
-  struct Span { const uint8_t* src; uint64_t len, stage_off; };
-  std::vector<Span> spans;
-  constexpr uint64_t kGap = 4096;
-  uint64_t payload = 0;
-  bool closed = false;  // the last span ends with a chunk's rebuilt values (payload is past them)
-  for (Item& it : items) {
-    const uint8_t* src = it.wk->str_base;
-    const uint64_t len = it.wk->str_span;
-    if (!closed && !spans.empty() && src >= spans.back().src + spans.back().len && uint64_t(src - (spans.back().src + spans.back().len)) <= kGap) {
-      spans.back().len = uint64_t(src - spans.back().src) + len;
-    } else {
-      if (!spans.empty() && !closed) payload += (spans.back().len + 15) & ~uint64_t(15);
-      spans.push_back({src, len, payload});
-    }
-    it.byte_off = spans.back().stage_off + uint64_t(src - spans.back().src);
-    closed = !it.wk->str_fronts.empty();
-    if (closed) payload = (it.byte_off + it.wk->str_rb0 + it.wk->str_rebuilt_len + 15) & ~uint64_t(15);
-  }
-  if (!spans.empty() && !closed) payload += (spans.back().len + 15) & ~uint64_t(15);
-  // scratch: [chunks][counts][offsets][lengths][prefixes][suffixes][windows][front jobs][slots][codes][first / rank][keys]
-  // [payload], 16-byte aligned pieces (the pieces of delta pages are empty in a batch of PLAIN pages)
-  auto al = [](uint64_t n) { return (n + 15) & ~uint64_t(15); };
-  const uint64_t n = items.size();
-  const uint64_t o_cnt = al(n * sizeof(StrChunk)), o_off = o_cnt + al(n * 4), o_len = o_off + al(nv * 4), o_pre = o_len + al(nl * 4),
-                 o_suf = o_pre + al(nd * 4), o_wmin = o_suf + al(nd * 4), o_jobs = o_wmin + al(nw * 4),
-                 o_slot = o_jobs + al(n_fronts * sizeof(StrFrontJob)), o_code = o_slot + al(nv * 4), o_first = o_code + al(nv * 4),
-                 o_keys = o_first + al(ns * 4), o_pay = o_keys + ns * 8;
-  CUDA_TRY(batch->scratch.alloc(o_pay + payload, ctx->stream));
-  uint8_t* d = static_cast<uint8_t*>(batch->scratch.p);
-  size_t pin_cap = 0;
-  // first occurrences (written by k_str_compact), counts, rebuilt regions (the distinct values written by k_str_gather)
-  const uint64_t pin_rebuilt = al(nv * 4 + n * 4);
-  uint8_t* pin = ctx->pinned_take(size_t(pin_rebuilt + nr), &pin_cap);
-  if (!pin) return fail(FGPU_ERR_OOM, "PLAIN string interning: page-locked result buffer");
-  struct Give { fgpu_ctx* ctx; uint8_t* p; size_t cap; ~Give() { ctx->pinned_give(p, cap); } } give{ctx, pin, pin_cap};
-  uint32_t* h_first = reinterpret_cast<uint32_t*>(pin);
-  uint32_t* h_count = h_first + nv;
-  std::vector<uint8_t> head(o_slot, 0);  // chunk table, zero counts, value addresses, front jobs
-  uint64_t job = 0;
-  for (size_t i = 0; i < items.size(); i++) {
-    const Item& it = items[i];
-    const ChunkWalk& wk = *it.wk;
-    StrChunk c{};
-    c.bytes = d + o_pay + it.byte_off;
-    c.off = reinterpret_cast<const uint32_t*>(d + o_off) + it.v0;
-    c.len = wk.str_len.empty() ? nullptr : reinterpret_cast<const uint32_t*>(d + o_len) + it.l0;
-    c.keys = reinterpret_cast<unsigned long long*>(d + o_keys) + it.s0;
-    c.first = reinterpret_cast<uint32_t*>(d + o_first) + it.s0;
-    c.slot = reinterpret_cast<uint32_t*>(d + o_slot) + it.v0;
-    c.out_first = h_first + it.v0;
-    c.n = uint32_t(wk.str_off.size());
-    c.mask = uint32_t(it.cap - 1);
-    c.v0 = uint32_t(it.v0);
-    c.s0 = uint32_t(it.s0);
-    c.rb0 = wk.str_rb0;
-    if (!wk.str_fronts.empty()) {
-      c.pre = reinterpret_cast<const uint32_t*>(d + o_pre) + it.d0;
-      c.suf = reinterpret_cast<const uint32_t*>(d + o_suf) + it.d0;
-      c.wmin = reinterpret_cast<const uint32_t*>(d + o_wmin) + it.w0;
-      c.out_rebuilt = pin + pin_rebuilt + it.r0;
-      std::memcpy(head.data() + o_pre + it.d0 * 4, wk.str_pre.data(), wk.str_pre.size() * 4);
-      std::memcpy(head.data() + o_suf + it.d0 * 4, wk.str_suf.data(), wk.str_suf.size() * 4);
-      std::memcpy(head.data() + o_wmin + it.w0 * 4, wk.str_wmin.data(), wk.str_wmin.size() * 4);
-      for (const StrFront& f : wk.str_fronts)
-        for (uint32_t seg = 0; seg < f.n; seg += kFrontSeg) {
-          const StrFrontJob fj{uint32_t(i), f.v0, f.d0, f.w0, seg, std::min(kFrontSeg, f.n - seg)};
-          std::memcpy(head.data() + o_jobs + job++ * sizeof(StrFrontJob), &fj, sizeof fj);
-        }
-    }
-    std::memcpy(head.data() + i * sizeof(StrChunk), &c, sizeof c);
-    std::memcpy(head.data() + o_off + it.v0 * 4, wk.str_off.data(), wk.str_off.size() * 4);
-    if (!wk.str_len.empty()) std::memcpy(head.data() + o_len + it.l0 * 4, wk.str_len.data(), wk.str_len.size() * 4);
-  }
-  auto upload = [&](void* dst, const void* src, size_t bytes) {
-    if (void* p = ctx->arena_take(bytes)) {
-      std::memcpy(p, src, bytes);
-      src = p;
-    }
-    return cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, ctx->stream);
-  };
-  cudaError_t e = upload(d, head.data(), head.size());
-  if (e == cudaSuccess) e = cudaMemsetAsync(d + o_first, 0xff, size_t(o_pay - o_first), ctx->stream);  // first = ~0, keys empty
-  for (const Span& sp : spans) {
-    if (e != cudaSuccess) break;
-    e = cudaMemcpyAsync(d + o_pay + sp.stage_off, sp.src, sp.len, cudaMemcpyHostToDevice, ctx->stream);
-  }
-  const StrChunk* d_chunks = reinterpret_cast<const StrChunk*>(d);
-  uint32_t* d_count = reinterpret_cast<uint32_t*>(d + o_cnt);
-  if (e == cudaSuccess) e = launch_str_unfront(d_chunks, reinterpret_cast<const StrFrontJob*>(d + o_jobs), uint32_t(n_fronts), ctx->stream);
-  if (e == cudaSuccess) e = launch_str_hash(d_chunks, uint32_t(n), uint32_t(nv), ctx->stream);
-  if (e == cudaSuccess) e = launch_str_compact(d_chunks, uint32_t(n), uint32_t(ns), d_count, ctx->stream);
-  if (e == cudaSuccess && nr > 0) e = launch_str_gather(d_chunks, uint32_t(n), uint32_t(ns), ctx->stream);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(h_count, d_count, n * 4, cudaMemcpyDeviceToHost, ctx->stream);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-  if (e != cudaSuccess) {
-    cudaGetLastError();
-    return fail(FGPU_ERR_CUDA, std::string("PLAIN string interning: ") + cudaGetErrorString(e));
-  }
-  // first occurrences in ascending order (they name the distinct values), remembering each one's rank
-  std::vector<std::vector<uint32_t>> rank_of(items.size());
-  for (size_t i = 0; i < items.size(); i++) {
-    const uint32_t cnt = h_count[i];
-    std::vector<std::pair<uint32_t, uint32_t>> fr(cnt);
-    for (uint32_t r = 0; r < cnt; r++) fr[r] = {h_first[items[i].v0 + r], r};
-    std::sort(fr.begin(), fr.end());
-    items[i].wk->str_firsts.resize(cnt);
-    rank_of[i].resize(cnt);
-    for (uint32_t k = 0; k < cnt; k++) {
-      items[i].wk->str_firsts[k] = fr[k].first;
-      rank_of[i][k] = fr[k].second;
-    }
-    if (!items[i].wk->str_fronts.empty()) items[i].wk->str_rebuilt = pin + pin_rebuilt + items[i].r0;
-  }
-  // the sections: interning of the new strings, holes for the indices; then the chunk-local index per rank
-  std::vector<uint32_t> codes;
-  std::vector<uint64_t> code0(items.size());
-  for (const auto& [part, col] : todo) finish_column(kIndexRows, table, part, col, /*host_intern=*/false);
-  for (size_t i = 0; i < items.size(); i++) {
-    code0[i] = codes.size();
-    codes.resize(codes.size() + rank_of[i].size());
-    const ChunkWalk& wk = *items[i].wk;
-    if (wk.str_codes.size() != rank_of[i].size()) continue;  // the chunk was refused while its sections were written
-    for (size_t k = 0; k < rank_of[i].size(); k++) codes[code0[i] + rank_of[i][k]] = wk.str_codes[k];
-  }
-  if (!codes.empty()) e = upload(d + o_code, codes.data(), codes.size() * 4);
-  if (e != cudaSuccess) {
-    cudaGetLastError();
-    return fail(FGPU_ERR_CUDA, std::string("PLAIN string interning: ") + cudaGetErrorString(e));
-  }
-  size_t i = 0;
-  for (const auto& [part, col] : todo) {
-    ColumnImage& img = part->images[col];
-    for (size_t g = 0; g < img.walks.size(); g++) {
-      const ChunkWalk& wk = img.walks[g];
-      if (i >= items.size() || items[i].wk != &wk) continue;
-      const Item& it = items[i];
-      const uint64_t c0 = code0[i++];
-      if (!img.error.empty()) continue;  // a refused chunk makes the column unreadable: it is never uploaded
-      for (const StrPage& pg : wk.str_pages) {
-        StrCodeJob j{};
-        j.dst = reinterpret_cast<uint8_t*>(uintptr_t(pg.hole));  // image offset: rebased at upload
-        j.slot = reinterpret_cast<const uint32_t*>(d + o_slot) + it.v0 + pg.first;
-        j.rank = reinterpret_cast<const uint32_t*>(d + o_first) + it.s0;
-        j.code = reinterpret_cast<const uint32_t*>(d + o_code) + c0;
-        j.n = pg.n;
-        j.w = wk.str_w;
-        img.str_jobs.push_back(j);
-      }
-    }
-    img.walks.clear();
-  }
-  return FGPU_OK;
-}
-
-// The PLAIN string pages' indices of a column whose image is now at `dev` (queued by intern_plain_strings).
-cudaError_t launch_str_jobs(fgpu_ctx* ctx, ColumnImage& img, void* dev) {
-  if (img.str_jobs.empty()) return cudaSuccess;
-  uint32_t groups = 0;
-  for (StrCodeJob& j : img.str_jobs) {
-    j.dst = static_cast<uint8_t*>(dev) + reinterpret_cast<uintptr_t>(j.dst);
-    j.g0 = groups;
-    groups += (j.n + 7) / 8;
-  }
-  const size_t bytes = img.str_jobs.size() * sizeof(StrCodeJob);
-  DevBuf d_jobs;  // released in stream order
-  cudaError_t e = d_jobs.alloc(bytes, ctx->stream);
-  const void* src = img.str_jobs.data();
-  if (void* pin = ctx->arena_take(bytes)) {
-    std::memcpy(pin, src, bytes);
-    src = pin;
-  }
-  if (e == cudaSuccess) e = cudaMemcpyAsync(d_jobs.p, src, bytes, cudaMemcpyHostToDevice, ctx->stream);
-  if (e == cudaSuccess) e = launch_str_codes(static_cast<const StrCodeJob*>(d_jobs.p), uint32_t(img.str_jobs.size()), groups, ctx->stream);
-  std::vector<StrCodeJob>().swap(img.str_jobs);
-  return e;
-}
-
-// Uploads one column of one part if it is not resident yet: the host-assembled meta region with one
-// copy, the PLAIN value regions straight from the source file (one async copy per contiguous extent),
-// all on the engine stream so that kernels queued behind need no extra synchronisation.
-// A column with PLAIN string values that no caller's intern batch has finished is interned here on its own.
-int32_t ensure_resident(fgpu_ctx* ctx, Table* table, Part* part, const std::string& column, uint64_t* h2d_bytes,
-                        double* build_us = nullptr, double* upload_us = nullptr) {
-  auto t0 = std::chrono::steady_clock::now();
-  walk_column(kIndexRows, table, part, column, /*device_seeds=*/true);
-  StrBatch own;
-  if (!part->images[column].built)
-    if (int32_t rc = intern_plain_strings(ctx, table, {{part, column}}, &own)) return rc;
-  auto t1 = std::chrono::steady_clock::now();
-  if (build_us) *build_us += std::chrono::duration<double, std::micro>(t1 - t0).count();
-  struct Tail {
-    double* out; std::chrono::steady_clock::time_point t;
-    ~Tail() { if (out) *out += std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - t).count(); }
-  } tail{upload_us, t1};
-  ColumnImage& img = part->images[column];
-  if (!img.error.empty()) return FGPU_OK;  // surfaces as an error only if a query projects the column
-  if (img.resident) return FGPU_OK;
-  void* dev = nullptr;
-  CUDA_TRY(cudaMallocAsync(&dev, img.dev_bytes, ctx->stream));
-  const void* meta_src = img.meta.data();
-  if (void* pin = ctx->arena_take(img.meta.size())) {
-    std::memcpy(pin, img.meta.data(), img.meta.size());
-    meta_src = pin;
-  }
-  cudaError_t e = cudaMemcpyAsync(dev, meta_src, img.meta.size(), cudaMemcpyHostToDevice, ctx->stream);
-  // PLAIN pages: neighbouring page payloads (separated by a page header) travel as ONE transfer of the
-  // raw bytes into a staging buffer and are gathered into the dense value array on the device; a payload
-  // without neighbours goes straight to its place.
-  uint64_t copied = img.meta.size();
-  {
-    struct Span { const uint8_t* src; uint64_t len, stage_off; size_t first, n; };
-    std::vector<Span> spans;
-    constexpr uint64_t kGap = 4096;
-    for (size_t i = 0; i < img.extents.size(); i++) {
-      const Extent& x = img.extents[i];
-      if (!spans.empty() && x.src >= spans.back().src + spans.back().len && uint64_t(x.src - (spans.back().src + spans.back().len)) <= kGap) {
-        spans.back().len = uint64_t(x.src - spans.back().src) + x.len;
-        spans.back().n++;
-      } else {
-        spans.push_back({x.src, x.len, 0, i, 1});
-      }
-    }
-    uint64_t stage_bytes = 0;
-    std::vector<PageCopy> copies;
-    for (Span& sp : spans) {
-      if (sp.n == 1) continue;
-      sp.stage_off = stage_bytes;
-      stage_bytes += ((sp.len + 15) & ~uint64_t(15)) + 16;
-      for (size_t i = sp.first; i < sp.first + sp.n; i++)
-        copies.push_back({sp.stage_off + uint64_t(img.extents[i].src - sp.src), img.extents[i].dst_off, img.extents[i].len});
-    }
-    const uint64_t table_off = stage_bytes;
-    // DELTA_BINARY_PACKED pages: their streams (neighbours a page header apart as one transfer, each transfer followed
-    // by 16 pad bytes), then the page and miniblock tables, then the decode's scratch, behind the PLAIN staging
-    struct DSpan { const uint8_t* src; uint64_t len, stage_off; };
-    std::vector<DSpan> dspans;
-    std::vector<DbpPage> dpages;
-    std::vector<DbpMini> dmbs;
-    uint64_t dstream_off = (table_off + copies.size() * sizeof(PageCopy) + 15) & ~uint64_t(15), dbytes = 0, n_groups = 0;
-    for (const DeltaPage& d : img.delta_pages) {
-      if (!dspans.empty() && d.src >= dspans.back().src + dspans.back().len && uint64_t(d.src - (dspans.back().src + dspans.back().len)) <= kGap) {
-        dspans.back().len = uint64_t(d.src - dspans.back().src) + d.len;
-      } else {
-        if (!dspans.empty()) dbytes += ((dspans.back().len + 15) & ~uint64_t(15)) + 16;
-        dspans.push_back({d.src, d.len, dstream_off + dbytes});
-      }
-      DbpPage pg{};
-      pg.dst = reinterpret_cast<unsigned long long*>(static_cast<uint8_t*>(dev) + d.hole);
-      pg.src = dspans.back().stage_off + uint64_t(d.src - dspans.back().src);
-      pg.first = static_cast<unsigned long long>(d.first);
-      pg.n = d.n;
-      pg.g0 = uint32_t(n_groups);
-      pg.mb0 = uint32_t(dmbs.size());
-      pg.per_mb = uint32_t(std::min<uint64_t>(d.per_mb, 0xffffffffu));
-      n_groups += (d.n + 31) / 32;
-      for (uint32_t m = d.mb0; m < d.mb0 + d.n_mb; m++)
-        dmbs.push_back(DbpMini{img.delta_mbs[m].min_delta, uint32_t(img.delta_mbs[m].off), img.delta_mbs[m].width});
-      dpages.push_back(pg);
-    }
-    if (!dspans.empty()) dbytes += ((dspans.back().len + 15) & ~uint64_t(15)) + 16;
-    if (n_groups > 0xffffffffull) e = cudaErrorInvalidValue;  // (more than 2^37 values in one column of one part)
-    const uint64_t dtab_off = dstream_off + dbytes, dtab_bytes = dpages.size() * sizeof(DbpPage) + dmbs.size() * sizeof(DbpMini);
-    const uint64_t dscratch_off = (dtab_off + dtab_bytes + 15) & ~uint64_t(15);
-    DevBuf stage;
-    if ((!copies.empty() || !dpages.empty()) && e == cudaSuccess) {
-      e = stage.alloc(dpages.empty() ? table_off + copies.size() * sizeof(PageCopy) : dscratch_off + dbp_scratch_bytes(uint32_t(n_groups)), ctx->stream);
-      auto upload = [&](uint64_t off, const void* src, size_t bytes) {
-        if (void* pin = ctx->arena_take(bytes)) {
-          std::memcpy(pin, src, bytes);
-          src = pin;
-        }
-        return cudaMemcpyAsync(static_cast<uint8_t*>(stage.p) + off, src, bytes, cudaMemcpyHostToDevice, ctx->stream);
-      };
-      if (e == cudaSuccess && !copies.empty()) e = upload(table_off, copies.data(), copies.size() * sizeof(PageCopy));
-      if (e == cudaSuccess && !dpages.empty()) {
-        std::vector<uint8_t> tab(dtab_bytes);
-        std::memcpy(tab.data(), dpages.data(), dpages.size() * sizeof(DbpPage));
-        std::memcpy(tab.data() + dpages.size() * sizeof(DbpPage), dmbs.data(), dmbs.size() * sizeof(DbpMini));
-        e = upload(dtab_off, tab.data(), tab.size());
-        copied += dtab_bytes;
-      }
-    }
-    for (const Span& sp : spans) {
-      if (e != cudaSuccess) break;
-      copied += sp.len;
-      if (sp.n == 1) e = cudaMemcpyAsync(static_cast<uint8_t*>(dev) + img.extents[sp.first].dst_off, sp.src, sp.len, cudaMemcpyHostToDevice, ctx->stream);
-      else e = cudaMemcpyAsync(static_cast<uint8_t*>(stage.p) + sp.stage_off, sp.src, sp.len, cudaMemcpyHostToDevice, ctx->stream);
-    }
-    for (const DSpan& sp : dspans) {
-      if (e != cudaSuccess) break;
-      copied += sp.len;
-      e = cudaMemcpyAsync(static_cast<uint8_t*>(stage.p) + sp.stage_off, sp.src, sp.len, cudaMemcpyHostToDevice, ctx->stream);
-    }
-    if (e == cudaSuccess && !copies.empty())
-      e = launch_gather_pages(stage.p, dev, reinterpret_cast<const PageCopy*>(static_cast<uint8_t*>(stage.p) + table_off), uint32_t(copies.size()), ctx->stream);
-    if (e == cudaSuccess && !dpages.empty()) {
-      const uint8_t* base = static_cast<const uint8_t*>(stage.p);
-      e = launch_dbp_decode(base, reinterpret_cast<const DbpPage*>(base + dtab_off), uint32_t(dpages.size()),
-                            reinterpret_cast<const DbpMini*>(base + dtab_off + dpages.size() * sizeof(DbpPage)), uint32_t(n_groups),
-                            static_cast<uint8_t*>(stage.p) + dscratch_off, ctx->stream);
-    }
-    // `stage` is released in stream order when it goes out of scope
-  }
-  if (e == cudaSuccess) e = launch_str_jobs(ctx, img, dev);
-  if (e == cudaSuccess) e = launch_make_seeds(dev, img.seed_jobs_off, img.n_seed_jobs, img.max_seed_chunks, ctx->stream);
-  if (e != cudaSuccess) {
-    cudaFreeAsync(dev, ctx->stream);
-    cudaGetLastError();
-    return fail(FGPU_ERR_CUDA, std::string("column upload: ") + cudaGetErrorString(e));
-  }
-  img.dev = dev;
-  img.resident = true;
-  patch_column_pointers(part, column, static_cast<const uint8_t*>(dev));
-  if (h2d_bytes) *h2d_bytes += copied;
-  ctx->pending_uploads.push_back(&img);
-  return FGPU_OK;
-}
-
-int bit_width_u32(uint64_t max_value) {
-  int w = 0;
-  while (w < 64 && (max_value >> w) != 0) w++;
-  return w;
-}
-
-// Host side of several columns of one part in parallel (page walk, run directories, dictionary interning): the
-// columns are independent — every column has its own dictionary, image and chunk records, all created here
-// before the workers start so that no container is resized concurrently.
-void prebuild_columns(Table* table, Part* part, const std::vector<std::string>& columns) {
-  std::vector<const std::string*> todo;
-  for (const std::string& c : columns) {
-    ColumnImage& img = part->images[c];  // creates the entry
-    if (img.built) continue;
-    for (const SchemaLeaf& l : part->pf.leaves)
-      if (l.name == c && l.phys == PT_BYTE_ARRAY) (void)table->dicts[c];
-    todo.push_back(&c);
-  }
-  if (todo.size() < 2) return;  // a single column is built by its caller
-  unsigned hw = std::thread::hardware_concurrency();
-  const size_t n_threads = std::min<size_t>(todo.size(), std::min<size_t>(hw ? hw : 4, 32));  // (a part has ~20 columns: one wave)
-  std::atomic<size_t> next{0};
-  std::vector<std::thread> workers;
-  for (size_t t = 0; t < n_threads; t++)
-    workers.emplace_back([&]() {
-      for (;;) {
-        const size_t i = next.fetch_add(1);
-        if (i >= todo.size()) break;
-        walk_column(kIndexRows, table, part, *todo[i], /*device_seeds=*/true);  // (PLAIN strings: finished after the intern batch)
-      }
-    });
-  for (std::thread& w : workers) w.join();
-}
-
-// Flat code arrays of one dictionary column of a part (every row group, one allocation), derived on the device
-// from the resident hybrid image the first time the tile-aggregate kernel needs the column (k_flatten).
-int32_t ensure_flat(fgpu_ctx* ctx, Part* part, const std::string& column) {
-  ColumnImage& img = part->images[column];
-  if (img.flat_dev) return FGPU_OK;
-  if (!img.resident) return fail(FGPU_ERR_INVALID, "flat codes requested for a column that is not resident: " + column);
-  std::vector<FlatJob> jobs;
-  std::vector<ChunkHost*> chs;
-  std::vector<uint64_t> offs;
-  uint64_t bytes = 0;
-  uint32_t blocks = 0;
-  for (RowGroupHost& rg : part->rgs) {
-    auto it = rg.cols.find(column);
-    if (it == rg.cols.end()) continue;
-    ChunkHost& ch = it->second;
-    if (!ch.error.empty() || ch.desc.kind != CK_DICT_STR) continue;
-    uint32_t max_gid = 0;
-    for (uint32_t g : ch.lut_host) max_gid = std::max(max_gid, g);
-    FlatJob j{};
-    j.chunk = ch.desc;
-    j.bias = ch.desc.has_nulls ? 0u : 1u;
-    const int bits = bit_width_u32(uint64_t(max_gid) + 1u - j.bias);
-    j.w = bits <= 8 ? 8u : (bits <= 16 ? 16u : 32u);  // byte-aligned codes: one shared-memory load per row and column
-    j.first_block = blocks;
-    const uint32_t nb = (rg.n_rows + uint32_t(kIndexRows) - 1) / uint32_t(kIndexRows);
-    blocks += nb;
-    offs.push_back(bytes);
-    bytes += (uint64_t(nb) * (kIndexRows / 8) * j.w + 64 + 127) & ~uint64_t(127);
-    jobs.push_back(j);
-    chs.push_back(&ch);
-  }
-  if (jobs.empty()) return FGPU_OK;
-  void* dev = nullptr;
-  CUDA_TRY(cudaMallocAsync(&dev, bytes + jobs.size() * sizeof(FlatJob), ctx->stream));
-  for (size_t i = 0; i < jobs.size(); i++) jobs[i].out = static_cast<uint8_t*>(dev) + offs[i];
-  const void* src = jobs.data();
-  if (void* pin = ctx->arena_take(jobs.size() * sizeof(FlatJob))) {
-    std::memcpy(pin, jobs.data(), jobs.size() * sizeof(FlatJob));
-    src = pin;
-  }
-  FlatJob* d_jobs = reinterpret_cast<FlatJob*>(static_cast<uint8_t*>(dev) + bytes);
-  cudaError_t e = cudaMemcpyAsync(d_jobs, src, jobs.size() * sizeof(FlatJob), cudaMemcpyHostToDevice, ctx->stream);
-  if (e == cudaSuccess) e = launch_flatten(d_jobs, uint32_t(jobs.size()), blocks, ctx->sm_count, ctx->stream);
-  if (e != cudaSuccess) {
-    cudaFreeAsync(dev, ctx->stream);
-    cudaGetLastError();
-    return fail(FGPU_ERR_CUDA, std::string("flat codes: ") + cudaGetErrorString(e));
-  }
-  img.flat_dev = dev;
-  for (size_t i = 0; i < jobs.size(); i++) {
-    chs[i]->flat = jobs[i].out;
-    chs[i]->flat_w = uint8_t(jobs[i].w);
-    chs[i]->flat_bias = uint8_t(jobs[i].bias);
-  }
-  return FGPU_OK;
-}
-
-// Frame-of-reference images of PLAIN non-null INT64 columns for the sorted-run kernel: for every resident chunk of every
-// listed (part, column) whose range max - min fits 32 bits, one image of uint{8,16,32}(value - min) per row, the
-// narrowest of the three (one allocation per (part, column), kept until the part goes).  The sorted-run kernel then
-// stages 1, 2 or 4 bytes per row instead of 8.  Minimum and maximum come from the values on the device, not from the
-// footer statistics, so that a chunk without statistics narrows as well and wrong statistics cannot change a result.
-// The whole list costs one min / max launch, one synchronisation and one narrowing launch.
-// want_prefix: (part, column) pairs that also get exclusive prefix-sum images for the prefix path of the sorted-run scan
-// (k_runs_prefix): every PLAIN non-null INT64 chunk, whatever its range, n_rows + 1 wrapping int64 sums (one allocation
-// per (part, column), kept until the part goes).  They are written by the same two launches: the min / max pass also
-// leaves every block's sum, the narrowing pass turns the values into the prefix, so the values are read no more often.
-int32_t ensure_narrow(fgpu_ctx* ctx, const std::vector<std::pair<Part*, std::string>>& want,
-                      const std::vector<std::pair<Part*, std::string>>& want_prefix) {
-  struct Job {
-    ColumnImage* img;
-    ChunkHost* ch;
-    bool narrow, prefix;
-  };
-  std::vector<Job> host;
-  std::vector<NarrowJob> jobs;
-  std::vector<ColumnImage*> imgs, pimgs;
-  uint32_t blocks = 0;
-  std::map<std::pair<Part*, std::string>, std::pair<bool, bool>> todo;  // (narrow, prefix), in a fixed order
-  for (const auto& pc : want) todo[pc].first = true;
-  for (const auto& pc : want_prefix) todo[pc].second = true;
-  for (const auto& kv : todo) {
-    Part* part = kv.first.first;
-    const std::string& col = kv.first.second;
-    ColumnImage& img = part->images[col];
-    const bool nar = kv.second.first && !img.narrowed, pre = kv.second.second && !img.prefixed;
-    if (!nar && !pre) continue;
-    if (!img.resident) return fail(FGPU_ERR_INVALID, "narrow image requested for a column that is not resident: " + col);
-    if (nar) {
-      img.narrowed = true;
-      imgs.push_back(&img);
-    }
-    if (pre) {
-      img.prefixed = true;
-      pimgs.push_back(&img);
-    }
-    for (RowGroupHost& rg : part->rgs) {
-      auto it = rg.cols.find(col);
-      if (it == rg.cols.end()) continue;
-      ChunkHost& ch = it->second;
-      if (!ch.error.empty() || ch.desc.kind != CK_PLAIN64 || ch.desc.has_nulls || ch.phys != PT_INT64 || rg.n_rows == 0) continue;
-      NarrowJob j{};
-      j.src = reinterpret_cast<const long long*>(ch.desc.values);
-      j.n_rows = rg.n_rows;
-      j.first_block = blocks;
-      j.sum_block = blocks;
-      blocks += (rg.n_rows + kNarrowRows - 1) / kNarrowRows;
-      jobs.push_back(j);
-      host.push_back({&img, &ch, nar, pre});
-    }
-  }
-  if (jobs.empty()) return FGPU_OK;
-  const size_t jb = jobs.size() * sizeof(NarrowJob), mmb = jobs.size() * 16;
-  std::vector<long long> mm(2 * jobs.size());
-  for (size_t i = 0; i < jobs.size(); i++) {
-    mm[2 * i] = std::numeric_limits<long long>::max();
-    mm[2 * i + 1] = std::numeric_limits<long long>::min();
-  }
-  void* tmp = nullptr;  // [jobs][min, max per job][sum per block]
-  CUDA_TRY(cudaMallocAsync(&tmp, jb + mmb + size_t(blocks) * 8, ctx->stream));
-  NarrowJob* d_jobs = static_cast<NarrowJob*>(tmp);
-  long long* d_mm = reinterpret_cast<long long*>(static_cast<uint8_t*>(tmp) + jb);
-  unsigned long long* d_bsum = reinterpret_cast<unsigned long long*>(static_cast<uint8_t*>(tmp) + jb + mmb);
-  auto upload = [&](const void* src, void* dst, size_t n) {
-    if (void* pin = ctx->arena_take(n)) {
-      std::memcpy(pin, src, n);
-      src = pin;
-    }
-    return cudaMemcpyAsync(dst, src, n, cudaMemcpyHostToDevice, ctx->stream);
-  };
-  cudaError_t e = upload(jobs.data(), d_jobs, jb);
-  if (e == cudaSuccess) e = upload(mm.data(), d_mm, mmb);
-  if (e == cudaSuccess) e = launch_chunk_minmax(d_jobs, uint32_t(jobs.size()), blocks, d_mm, d_bsum, ctx->stream);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(mm.data(), d_mm, mmb, cudaMemcpyDeviceToHost, ctx->stream);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-  // widths, then one image allocation per (part, column) and the narrowing pass over the chunks that fit 32 bits or want
-  // a prefix image
-  std::map<ColumnImage*, uint64_t> bytes, pbytes;
-  std::vector<uint64_t> offs(jobs.size()), poffs(jobs.size());
-  std::vector<NarrowJob> pass2;
-  uint32_t blocks2 = 0;
-  for (size_t i = 0; i < jobs.size() && e == cudaSuccess; i++) {
-    if (host[i].prefix) {
-      uint64_t& b = pbytes[host[i].img];
-      poffs[i] = b;
-      b += (uint64_t(jobs[i].n_rows + 1) * 8 + 127) & ~uint64_t(127);
-    }
-    const uint64_t range = uint64_t(mm[2 * i + 1]) - uint64_t(mm[2 * i]);
-    jobs[i].w = !host[i].narrow ? 0u : range <= 0xffu ? 1u : (range <= 0xffffu ? 2u : (range <= 0xffffffffu ? 4u : 0u));
-    if (!jobs[i].w) continue;  // needs 64 bits: read from the extent as before
-    jobs[i].base = mm[2 * i];
-    uint64_t& b = bytes[host[i].img];
-    offs[i] = b;
-    b += (uint64_t(jobs[i].n_rows) * jobs[i].w + 16 + 127) & ~uint64_t(127);  // 128-byte aligned, >= 16 readable pad bytes (tile copies round up to 16)
-  }
-  for (ColumnImage* img : imgs) {
-    auto it = bytes.find(img);
-    if (it == bytes.end() || e != cudaSuccess) continue;
-    e = cudaMallocAsync(&img->narrow_dev, it->second, ctx->stream);
-  }
-  for (ColumnImage* img : pimgs) {
-    auto it = pbytes.find(img);
-    if (it == pbytes.end() || e != cudaSuccess) continue;
-    e = cudaMallocAsync(&img->prefix_dev, it->second, ctx->stream);
-  }
-  for (size_t i = 0; i < jobs.size() && e == cudaSuccess; i++) {
-    if (jobs[i].w) jobs[i].out = static_cast<uint8_t*>(host[i].img->narrow_dev) + offs[i];
-    if (host[i].prefix) jobs[i].pre = reinterpret_cast<long long*>(static_cast<uint8_t*>(host[i].img->prefix_dev) + poffs[i]);
-    if (!jobs[i].w && !jobs[i].pre) continue;
-    jobs[i].first_block = blocks2;
-    blocks2 += (jobs[i].n_rows + kNarrowRows - 1) / kNarrowRows;
-    pass2.push_back(jobs[i]);
-  }
-  if (e == cudaSuccess && !pass2.empty()) e = upload(pass2.data(), d_jobs, pass2.size() * sizeof(NarrowJob));
-  if (e == cudaSuccess) e = launch_narrow(d_jobs, uint32_t(pass2.size()), blocks2, d_bsum, ctx->stream);
-  cudaFreeAsync(tmp, ctx->stream);
-  if (e != cudaSuccess) {
-    cudaGetLastError();
-    return fail(FGPU_ERR_CUDA, std::string("narrow images: ") + cudaGetErrorString(e));
-  }
-  for (size_t i = 0; i < jobs.size(); i++) {
-    if (jobs[i].pre) host[i].ch->prefix = jobs[i].pre;
-    if (!jobs[i].w) continue;
-    host[i].ch->narrow = jobs[i].out;
-    host[i].ch->narrow_w = uint8_t(jobs[i].w);
-    host[i].ch->narrow_base = jobs[i].base;
-  }
-  return FGPU_OK;
-}
-
-// After the stream has been synchronised the host staging of uploaded columns can go.
-void release_staging(fgpu_ctx* ctx) {
-  ctx->arena_used = 0;
-  for (ColumnImage* img : ctx->pending_uploads) {
-    std::vector<uint8_t>().swap(img->meta);
-    std::vector<Extent>().swap(img->extents);
-    std::vector<DeltaPage>().swap(img->delta_pages);
-    std::vector<DbpMiniblock>().swap(img->delta_mbs);
-  }
-  ctx->pending_uploads.clear();
-}
-
-void free_part(fgpu_ctx* ctx, Part* p) {
-  for (auto& kv : p->images) {
-    if (kv.second.dev) cudaFreeAsync(kv.second.dev, ctx->stream);
-    if (kv.second.flat_dev) cudaFreeAsync(kv.second.flat_dev, ctx->stream);
-    if (kv.second.narrow_dev) cudaFreeAsync(kv.second.narrow_dev, ctx->stream);
-    if (kv.second.prefix_dev) cudaFreeAsync(kv.second.prefix_dev, ctx->stream);
-  }
-}
 
 struct VisibleRG {
   Part* part;
@@ -1667,7 +904,6 @@ void prune_row_groups(const QueryPlan& q, const Switches& w, const std::vector<u
 // FGPU_PUT_BORROW_PINNED upload nothing until a query needs it; optimize.go:36-73 physical projection).
 int32_t make_resident(fgpu_ctx* ctx, Table& table, Compiled* c) {
   PhaseClock pc;
-  double build_us = 0, upload_us = 0;
   std::vector<std::pair<Part*, uint64_t>> reads;  // per part, in row-group order: bit s = some kept row group reads slot s
   for (const VisibleRG& v : c->rgs) {
     if (reads.empty() || reads.back().first != v.part) reads.push_back({v.part, 0});
@@ -1675,42 +911,24 @@ int32_t make_resident(fgpu_ctx* ctx, Table& table, Compiled* c) {
   }
   // numeric columns first: their bytes are the bulk of the transfer, which then runs while the host
   // assembles the dictionary columns' run directories
-  auto upload = [&](Part* part, const std::string& name) -> int32_t {
-    int32_t rc = ensure_resident(ctx, &table, part, name, &c->h2d_bytes, pc.on ? &build_us : nullptr, pc.on ? &upload_us : nullptr);
-    if (rc) return rc;
-    const ColumnImage& img = part->images[name];
-    if (!img.error.empty()) return fail(FGPU_ERR_UNSUPPORTED, "column " + name + ": " + img.error);
-    return FGPU_OK;
-  };
-  std::vector<std::pair<Part*, std::string>> plain_strings;  // walked, waiting for the intern batch
+  std::vector<std::pair<Part*, std::string>> cols;
   for (int pass = 0; pass < 2; pass++) {
     for (auto& [part, read] : reads) {
       for (size_t si = 0; si < c->slot_names.size(); si++) {
         const std::string& name = c->slot_names[si];
         if ((c->slot_types[si] == ST_DICT) != (pass == 1) || !((read >> si) & 1)) continue;
         if (std::find(part->columns.begin(), part->columns.end(), name) == part->columns.end()) continue;
-        if (pass == 1 && !part->images[name].resident) {
-          const auto tw = std::chrono::steady_clock::now();
-          walk_column(kIndexRows, &table, part, name, /*device_seeds=*/true);
-          if (pc.on) build_us += std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - tw).count();
-          if (!part->images[name].built) {
-            plain_strings.push_back({part, name});
-            continue;
-          }
-        }
-        if (int32_t rc = upload(part, name)) return rc;
+        cols.push_back({part, name});
       }
     }
   }
-  if (!plain_strings.empty()) {
-    StrBatch batch;
-    if (int32_t rc = intern_plain_strings(ctx, &table, plain_strings, &batch)) return rc;
-    for (auto& [part, name] : plain_strings)
-      if (int32_t rc = upload(part, name)) return rc;
-  }
+  UploadStats st;
+  const int32_t rc = upload_columns(ctx, &table, cols, &st, /*refuse_unreadable=*/true);
+  c->h2d_bytes += st.h2d_bytes;
+  if (rc) return rc;
   if (pc.on && c->h2d_bytes) {
     char buf[128];
-    snprintf(buf, sizeof buf, " build=%.0fus enqueue=%.0fus bytes=%llu", build_us, upload_us, (unsigned long long)c->h2d_bytes);
+    snprintf(buf, sizeof buf, " build=%.0fus enqueue=%.0fus bytes=%llu", st.build_us, st.enqueue_us, (unsigned long long)c->h2d_bytes);
     pc.line = buf;
     pc.flush("residency");
   }
@@ -3741,29 +2959,7 @@ int32_t fgpu_part_put_parquet(fgpu_ctx* ctx, const char* table, uint64_t part_id
   if (!part->borrowed) {
     // The caller may reuse the buffer on return: every column goes to the device now (host images built in
     // parallel, one worker per column; PLAIN string pages interned in one batch).
-    prebuild_columns(&t, part.get(), part->columns);
-    StrBatch batch;
-    {
-      std::vector<std::pair<Part*, std::string>> cols;
-      for (const std::string& col : part->columns) cols.push_back({part.get(), col});
-      if (int32_t rc = intern_plain_strings(ctx, &t, cols, &batch)) {
-        free_part(ctx, part.get());
-        return rc;
-      }
-    }
-    for (const std::string& col : part->columns) {
-      int32_t rc = ensure_resident(ctx, &t, part.get(), col, nullptr);
-      if (rc) {
-        free_part(ctx, part.get());
-        return rc;
-      }
-    }
-    cudaError_t e = cudaStreamSynchronize(ctx->stream);
-    release_staging(ctx);
-    if (e != cudaSuccess) {
-      free_part(ctx, part.get());
-      return fail(FGPU_ERR_CUDA, std::string("part upload: ") + cudaGetErrorString(e));
-    }
+    if (int32_t rc = upload_part(ctx, &t, part.get())) return rc;
     part->file = nullptr;
   }
   t.parts.push_back(std::move(part));
@@ -3796,19 +2992,7 @@ int32_t fgpu_part_put_arrow(fgpu_ctx* ctx, const char* table, uint64_t part_id, 
   part->arrow = true;
   if (!build_arrow_part(&t, part.get(), schema, array, &err)) return fail(FGPU_ERR_UNSUPPORTED, "Arrow part: " + err);
   // the record's buffers go away on return: every column image is uploaded now
-  for (const std::string& col : part->columns) {
-    int32_t rc = ensure_resident(ctx, &t, part.get(), col, nullptr);
-    if (rc) {
-      free_part(ctx, part.get());
-      return rc;
-    }
-  }
-  cudaError_t e = cudaStreamSynchronize(ctx->stream);
-  release_staging(ctx);
-  if (e != cudaSuccess) {
-    free_part(ctx, part.get());
-    return fail(FGPU_ERR_CUDA, std::string("part upload: ") + cudaGetErrorString(e));
-  }
+  if (int32_t rc = upload_part(ctx, &t, part.get())) return rc;
   t.parts.push_back(std::move(part));
   t.epoch = ++ctx->epoch_counter;
   return FGPU_OK;
@@ -4391,7 +3575,8 @@ int32_t fgpu_part_decode_column(fgpu_ctx* ctx, const char* table, uint64_t part_
     if (p->id == part_id) part = p.get();
   if (!part) return fail(FGPU_ERR_NOT_FOUND, "part not found");
   {
-    int32_t rc = ensure_resident(ctx, &it->second, part, column, nullptr);
+    UploadStats st;
+    int32_t rc = upload_columns(ctx, &it->second, {{part, column}}, &st, /*refuse_unreadable=*/false);
     if (rc) return rc;
     const ColumnImage& img = part->images[column];
     if (!img.error.empty() && img.error != "column not in part") return fail(FGPU_ERR_UNSUPPORTED, std::string(column) + ": " + img.error);

@@ -698,12 +698,12 @@ void finish_image(ImageWriter& w, ColumnImage& img, Part* part, const std::strin
     img.n_seed_jobs = uint32_t(w.jobs.size());
     for (const SeedJob& j : w.jobs) img.max_seed_chunks = std::max(img.max_seed_chunks, j.n_chunks);
   }
-  if (img.meta.empty()) img.meta.resize(kAlign, 0);
+  if (img.staging.meta.empty()) img.staging.meta.resize(kAlign, 0);
   // rebase extent offsets behind the (128-aligned) meta region, the device-only region behind the extents
-  const uint64_t meta_size = (img.meta.size() + kAlign - 1) / kAlign * kAlign;
+  const uint64_t meta_size = (img.staging.meta.size() + kAlign - 1) / kAlign * kAlign;
   const uint64_t dev_base = (meta_size + w.ext_size + kAlign - 1) / kAlign * kAlign;
-  for (Extent& e : img.extents) e.dst_off += meta_size;
-  for (DeltaPage& d : img.delta_pages) d.hole += meta_size;
+  for (Extent& e : img.staging.extents) e.dst_off += meta_size;
+  for (DeltaPage& d : img.staging.delta_pages) d.hole += meta_size;
   for (RowGroupHost& h : part->rgs) {
     ChunkHost& ch = h.cols[column];
     if (ch.off_values < -0) ch.off_values = int64_t(meta_size) + (-ch.off_values - 1);
@@ -712,7 +712,7 @@ void finish_image(ImageWriter& w, ColumnImage& img, Part* part, const std::strin
     if (ch.dev_row_seeds >= 0) ch.off_row_seeds = int64_t(dev_base) + ch.dev_row_seeds;
   }
   for (uint32_t i = 0; i < img.n_seed_jobs; i++) {
-    SeedJob* j = reinterpret_cast<SeedJob*>(img.meta.data() + img.seed_jobs_off) + i;
+    SeedJob* j = reinterpret_cast<SeedJob*>(img.staging.meta.data() + img.seed_jobs_off) + i;
     j->seeds_off += dev_base;
   }
   img.dev_bytes = dev_base + w.dev_size + kAlign;
@@ -794,10 +794,10 @@ void finish_column(int index_rows, Table* table, Part* part, const std::string& 
   GlobalDict* dict = nullptr;
   for (const SchemaLeaf& l : part->pf.leaves)
     if (l.name == column && l.phys == PT_BYTE_ARRAY) dict = &table->dicts[column];
-  ImageWriter w(img.meta, img.extents);
+  ImageWriter w(img.staging.meta, img.staging.extents);
   w.device_seeds = img.device_seeds;
-  w.delta_pages = &img.delta_pages;
-  w.delta_mbs = &img.delta_mbs;
+  w.delta_pages = &img.staging.delta_pages;
+  w.delta_mbs = &img.staging.delta_mbs;
   for (size_t g = 0; g < part->rgs.size(); g++) {
     RowGroupHost& h = part->rgs[g];
     ChunkHost ch;
@@ -855,7 +855,7 @@ bool build_arrow_column(Table* table, Part* part, const std::string& name, const
 
   ColumnImage& img = part->images[name];
   img.built = true;
-  ImageWriter w(img.meta, img.extents);
+  ImageWriter w(img.staging.meta, img.staging.extents);
   w.device_seeds = true;
   ChunkHost ch;
   ch.desc.n_rows = n_rows;
@@ -1089,10 +1089,10 @@ std::string describe_part_json(const uint8_t* file, uint64_t len, int tile_rows,
     build_column(tile_rows, &table, &part, name);
     ColumnImage& img = part.images[name];
     std::vector<uint8_t> flat(size_t(img.dev_bytes), 0);
-    std::memcpy(flat.data(), img.meta.data(), img.meta.size());
-    for (const Extent& e : img.extents) std::memcpy(flat.data() + e.dst_off, e.src, size_t(e.len));
-    for (const DeltaPage& d : img.delta_pages)  // the holes the device fills at upload
-      unpack_delta_binary_packed<int64_t>(d.src, d.first, img.delta_mbs.data() + d.mb0, d.n_mb, d.v0,
+    std::memcpy(flat.data(), img.staging.meta.data(), img.staging.meta.size());
+    for (const Extent& e : img.staging.extents) std::memcpy(flat.data() + e.dst_off, e.src, size_t(e.len));
+    for (const DeltaPage& d : img.staging.delta_pages)  // the holes the device fills at upload
+      unpack_delta_binary_packed<int64_t>(d.src, d.first, img.staging.delta_mbs.data() + d.mb0, d.n_mb, d.v0,
                                           reinterpret_cast<int64_t*>(flat.data() + d.hole));
     host_images.push_back(std::move(flat));
     patch_column_pointers(&part, name, host_images.back().data());  // pointers into the host image

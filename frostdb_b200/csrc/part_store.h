@@ -194,22 +194,27 @@ inline std::string_view chunk_string(const ChunkWalk& wk, uint32_t i) {
 // Rebuilds a walked chunk's DELTA_BYTE_ARRAY values on the host (str_rebuilt_host; no-op without such pages).
 void unfront_strings(ChunkWalk* wk);
 
+// Host staging of one column image, kept until its upload has been synchronised (release_staging).
+struct ImageStaging {
+  std::vector<uint8_t> meta;  // everything that is not an extent
+  std::vector<Extent> extents;
+  // DELTA_BINARY_PACKED int64 pages of every chunk, whose values the device writes at upload (DeltaPage::hole: image
+  // offset), and their miniblocks (DeltaPage::mb0 indexes this list)
+  std::vector<DeltaPage> delta_pages;
+  std::vector<DbpMiniblock> delta_mbs;
+  std::vector<StrCodeJob> str_jobs;  // PLAIN string pages whose indices the device writes at upload (dst: image offset)
+};
+
 // Device residency of one column of one part (all its row groups in one allocation).
 struct ColumnImage {
   bool walked = false;     // page walk done (`walks` holds it until the sections are written)
   bool device_seeds = false;
   std::vector<ChunkWalk> walks;  // per row group, between the walk and the section writing
-  std::vector<StrCodeJob> str_jobs;  // PLAIN string pages whose indices the device writes at upload (dst: image offset)
-  // DELTA_BINARY_PACKED int64 pages of every chunk, whose values the device writes at upload (DeltaPage::hole: image
-  // offset), and their miniblocks (DeltaPage::mb0 indexes this list); kept until uploaded
-  std::vector<DeltaPage> delta_pages;
-  std::vector<DbpMiniblock> delta_mbs;
   bool built = false;      // host side done (ChunkHosts filled, dictionary interned)
   bool resident = false;   // bytes are on the device
   void* dev = nullptr;
   uint64_t dev_bytes = 0;
-  std::vector<uint8_t> meta;     // host staging of everything that is not an extent (kept until uploaded)
-  std::vector<Extent> extents;
+  ImageStaging staging;
   uint64_t seed_jobs_off = 0;    // SeedJob[n_seed_jobs] inside the meta region (device-derived seeds)
   uint32_t n_seed_jobs = 0, max_seed_chunks = 0;
   std::string error;             // whole-column error (a chunk the engine cannot read)
@@ -243,7 +248,7 @@ struct Table {
 bool open_part(const uint8_t* file, uint64_t len, Part* part, std::string* err);
 
 // Builds the host side of one column of a part (no CUDA calls): run directories, seeds, dictionary
-// LUTs into `image.meta`, PLAIN value regions as extents.  Interns dictionary entries into `table`.
+// LUTs into `image.staging.meta`, PLAIN value regions as extents.  Interns dictionary entries into `table`.
 // ChunkDesc pointers are offsets until patch_column_pointers() is called.
 // device_seeds: leave the cursor seeds to k_make_seeds (ColumnImage::seed_jobs_*) instead of building them here.
 // PLAIN string pages are interned here on the host, row by row (ChunkInterner), and their indices packed by the host.
