@@ -142,6 +142,7 @@ _SIGNATURES = {
     "fgpu_xxhash64": ([C.c_char_p, C.c_uint64, C.c_uint64, C.POINTER(C.c_uint64)], C.c_int32),
     "fgpu_bloom_check": ([C.c_void_p, C.c_uint64, C.c_uint64, C.POINTER(C.c_int32)], C.c_int32),
     "fgpu_bloom_insert": ([C.c_void_p, C.c_uint64, C.c_uint64], C.c_int32),
+    "fgpu_lz4_raw_inflate": ([C.c_char_p, C.c_uint64, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)], C.c_int32),
     "fgpu_parquet_rowgroup_may_match_eq": ([C.c_char_p, C.c_uint64, C.c_int32, C.c_char_p, C.c_int32, C.c_int64, C.c_double, C.c_char_p, C.c_uint64,
                                             C.POINTER(C.c_int32)], C.c_int32),
 }
@@ -184,6 +185,15 @@ def describe_parquet(buf: bytes, tile_rows: int = 0) -> dict:
     out = C.create_string_buffer(n.value)
     check(lib.fgpu_parquet_describe(C.addressof(src), len(buf), tile_rows, C.addressof(out), n.value, C.byref(n)))
     return json.loads(out.raw[: n.value].decode("utf-8"))
+
+
+def lz4_raw_inflate(block: bytes, size: int) -> bytes:
+    """Host-only: one LZ4_RAW block that must inflate to exactly `size` bytes (FrostGPUError when it is refused)."""
+    lib = load()
+    out = C.create_string_buffer(max(size, 1))
+    n = C.c_uint64(0)
+    check(lib.fgpu_lz4_raw_inflate(block, len(block), C.addressof(out), size, C.byref(n)))
+    return out.raw[:n.value]
 
 
 def _parse_blob(raw: bytes, count: int):

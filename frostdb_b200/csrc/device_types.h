@@ -266,6 +266,17 @@ struct DbpMini {
 };
 constexpr int kDbpGroupsPerCta = 32;  // one warp per 32-value group: a CTA covers 1 024 values
 
+// ---- LZ4_RAW value pages inflated at upload (lz4_pages.cu) ---------------------------------------------------
+// One PLAIN INT64 / DOUBLE page whose LZ4_RAW block the host validated: the block sits in the upload's staging buffer,
+// its first `out_len` inflated bytes are the page's dense values (a hole in the column image).
+struct Lz4Job {
+  unsigned char* dst;      // its hole in the column image
+  unsigned long long src;  // offset of its block in the staging buffer
+  uint32_t len;            // bytes of the block
+  uint32_t out_len;        // bytes of the hole (8 per non-null value)
+};
+constexpr int kLz4WarpsPerCta = 4;  // one warp per page
+
 // ---- sorted-run scan (k_runs_tma): the plan shape of compacted parts -----------------------------------
 // Row groups whose filter columns and aggregate inputs are PLAIN non-null int64 and whose group-key
 // columns are run-length only (sorted parts) are scanned by a dedicated kernel that walks the key run

@@ -3387,6 +3387,20 @@ int32_t fgpu_xxhash64(const uint8_t* data, uint64_t len, uint64_t seed, uint64_t
   API_CATCH
 }
 
+int32_t fgpu_lz4_raw_inflate(const uint8_t* src, uint64_t len, uint8_t* dst, uint64_t cap, uint64_t* out_len) {
+  API_TRY
+  if ((!src && len) || !out_len) return fail(FGPU_ERR_INVALID, "null argument");
+  *out_len = 0;
+  std::string err;
+  if (!parse_lz4_raw(src, len, cap, &err)) return fail(FGPU_ERR_PARQUET, err);
+  if (dst) {
+    unpack_lz4_raw(src, len, dst, cap);
+    *out_len = cap;
+  }
+  return FGPU_OK;
+  API_CATCH
+}
+
 int32_t fgpu_bloom_check(const uint8_t* bitset, uint64_t nbytes, uint64_t hash, int32_t* out_may_contain) {
   API_TRY
   if (!bitset || !out_may_contain) return fail(FGPU_ERR_INVALID, "null argument");

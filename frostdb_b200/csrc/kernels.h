@@ -55,6 +55,8 @@ cudaError_t launch_str_codes(const StrCodeJob* d_jobs, uint32_t n_jobs, uint32_t
 size_t dbp_scratch_bytes(uint32_t n_groups);
 cudaError_t launch_dbp_decode(const uint8_t* stage, const DbpPage* d_pages, uint32_t n_pages, const DbpMini* d_mbs, uint32_t n_groups,
                               void* scratch, cudaStream_t st);
+// LZ4_RAW PLAIN int64 / double pages -> dense values (lz4_pages.cu): one launch per upload, one warp per page.
+cudaError_t launch_lz4_pages(const uint8_t* stage, const Lz4Job* d_jobs, uint32_t n_jobs, cudaStream_t st);
 // partial-table exchange over peer-mapped mailboxes (comm.cu)
 cudaError_t launch_comm_push(const CommPush& p, int sm_count, cudaStream_t st);
 cudaError_t launch_comm_wait(const CommWait& w, cudaStream_t st);

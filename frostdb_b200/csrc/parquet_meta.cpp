@@ -151,7 +151,7 @@ RawSchemaElement read_schema_element(TReader& r) {
 
 struct RawColumnMeta {
   int32_t type = -1, codec = 0;
-  int64_t num_values = 0, total_compressed = 0, data_page_offset = -1, dict_page_offset = -1;
+  int64_t num_values = 0, total_uncompressed = 0, total_compressed = 0, data_page_offset = -1, dict_page_offset = -1;
   int64_t null_count = -1;
   int64_t bloom_offset = -1;
   int32_t bloom_length = -1;
@@ -195,6 +195,7 @@ RawColumnMeta read_column_meta(TReader& r) {
       }
       case 4: m.codec = int32_t(r.zigzag()); break;
       case 5: m.num_values = r.zigzag(); break;
+      case 6: m.total_uncompressed = r.zigzag(); break;
       case 7: m.total_compressed = r.zigzag(); break;
       case 9: m.data_page_offset = r.zigzag(); break;
       case 11: m.dict_page_offset = r.zigzag(); break;
@@ -309,6 +310,7 @@ void init_chunk(const RawColumnMeta& cm, const SchemaLeaf& leaf, ChunkMeta* out)
   out->codec = cm.codec;
   out->num_values = cm.num_values;
   out->total_compressed_size = cm.total_compressed;
+  out->total_uncompressed_size = cm.total_uncompressed;
   out->null_count = cm.null_count;
   if ((leaf.phys == PT_INT64 || leaf.phys == PT_DOUBLE) && cm.stat_min.size() == 8 && cm.stat_max.size() == 8) {
     out->has_minmax = true;
@@ -321,7 +323,7 @@ void init_chunk(const RawColumnMeta& cm, const SchemaLeaf& leaf, ChunkMeta* out)
     out->min_str = cm.stat_min;
     out->max_str = cm.stat_max;
   }
-  if (cm.codec != 0) {
+  if (cm.codec != 0 && cm.codec != kCodecLz4Raw) {
     out->error = "compressed column chunk (codec " + std::to_string(cm.codec) + ") is not supported";
     return;
   }
@@ -329,6 +331,29 @@ void init_chunk(const RawColumnMeta& cm, const SchemaLeaf& leaf, ChunkMeta* out)
     out->error = "repeated (nested) columns are not supported";
     return;
   }
+}
+
+}  // namespace
+
+namespace {
+
+// LZ4_RAW chunks: the device inflates the values of PLAIN INT64 / DOUBLE pages whose block holds nothing but values
+// (data page v2 of any column, data page v1 of a REQUIRED column); the host inflates every other page.
+bool plain_numeric(const SchemaLeaf& leaf, const RawPageHeader& h) {
+  return h.encoding == ENC_PLAIN && (leaf.phys == PT_INT64 || leaf.phys == PT_DOUBLE);
+}
+bool device_inflates(const SchemaLeaf& leaf, const RawPageHeader& h) {
+  if (!plain_numeric(leaf, h)) return false;
+  return h.type == PG_DATA_V2 ? h.v2_compressed : (h.type == PG_DATA && leaf.max_def == 0);
+}
+
+// Bytes a page of an LZ4_RAW chunk adds to ChunkMeta::inflated (its values region, or all of a v1 page; the levels of a
+// v2 page stay in the file).  Nonsense sizes count 0: the walk refuses the page before it inflates anything.
+uint64_t host_inflated_bytes(const SchemaLeaf& leaf, const RawPageHeader& h) {
+  if (h.type != PG_DICTIONARY && h.type != PG_DATA && h.type != PG_DATA_V2) return 0;
+  if (h.type == PG_DATA_V2 ? plain_numeric(leaf, h) : (h.type == PG_DATA && device_inflates(leaf, h))) return 0;
+  const int64_t raw = h.type == PG_DATA_V2 ? int64_t(h.uncompressed) - h.def_len - h.rep_len : int64_t(h.uncompressed);
+  return raw > 0 ? uint64_t(raw) : 0;
 }
 
 }  // namespace
@@ -350,6 +375,65 @@ void walk_chunk_pages(const uint8_t* file, uint64_t len, const SchemaLeaf& leaf,
   // total_compressed_size bounds the chunk (headers included).
   if (cm.total_compressed > 0 && uint64_t(start) + uint64_t(cm.total_compressed) <= len)
     end = p + cm.total_compressed;
+  const uint8_t* const first = p;
+  const bool lz4 = out->codec == kCodecLz4Raw;
+  if (lz4) {
+    // sizing pass: the host-inflated bytes of every page go into one buffer, allocated once (pointers into it stay valid);
+    // the walk below reports whatever stops this pass
+    uint64_t bytes = 0;
+    int64_t seen = 0;
+    try {
+      while (seen < cm.num_values && p < end) {
+        TReader r(p, end);
+        const RawPageHeader h = read_page_header(r);
+        if (h.compressed < 0 || uint64_t(h.compressed) > uint64_t(end - r.pos())) break;
+        if (h.uncompressed >= 0 && uint64_t(h.uncompressed) <= 256 * uint64_t(h.compressed)) bytes += host_inflated_bytes(leaf, h);
+        if (h.type == PG_DATA || h.type == PG_DATA_V2) seen += h.num_values;
+        p = r.pos() + h.compressed;
+      }
+    } catch (ThriftError&) {
+    }
+    out->inflated.assign(size_t(bytes) + 8, 0);  // (8 pad bytes: hybrid streams are read in 5-byte windows)
+    p = first;
+  }
+  uint64_t at = 0;  // fill of `inflated`
+  // the `raw` bytes that `n` stored bytes at `src` stand for, inflated into `inflated` (LZ4_RAW) or copied there
+  // (`compressed` false: a v2 values region stored as is); false with `error` set when the block is refused
+  auto inflate = [&](const uint8_t* src, uint32_t n, int64_t raw, bool compressed, const uint8_t** dst) {
+    if (raw < 0 || (compressed && n > 0 && uint64_t(raw) > 256 * uint64_t(n))) {
+      out->error = "LZ4_RAW page size out of range";
+      return false;
+    }
+    if (at + uint64_t(raw) > out->inflated.size() - 8) {
+      out->error = "LZ4_RAW page sizes changed between two reads";
+      return false;
+    }
+    uint8_t* q = out->inflated.data() + at;
+    if (!compressed) {
+      if (uint64_t(raw) != n) { out->error = "uncompressed v2 values region differs from its page's size"; return false; }
+      if (n) std::memcpy(q, src, n);
+    } else if (n != 0 || raw != 0) {  // (an empty region may be stored as 0 bytes)
+      std::string e;
+      if (!parse_lz4_raw(src, n, uint64_t(raw), &e)) { out->error = e; return false; }
+      unpack_lz4_raw(src, n, q, uint64_t(raw));
+    }
+    at += uint64_t(raw);
+    *dst = q;
+    return true;
+  };
+  // a device-inflated values region: validated only (parse step), left in the file
+  auto validate = [&](PageInfo* pg, int64_t raw) {
+    if (raw < 0 || (pg->values_len > 0 && uint64_t(raw) > 256 * uint64_t(pg->values_len))) {
+      out->error = "LZ4_RAW page size out of range";
+      return false;
+    }
+    if (pg->values_len == 0 && raw == 0) return true;
+    std::string e;
+    if (!parse_lz4_raw(pg->values, pg->values_len, uint64_t(raw), &e)) { out->error = e; return false; }
+    if (raw == 0) pg->values_len = 0;  // (the block 0x00: no values)
+    pg->lz4_len = uint32_t(raw);
+    return true;
+  };
   int64_t values_seen = 0;
   try {
     while (values_seen < cm.num_values && p < end) {
@@ -367,6 +451,10 @@ void walk_chunk_pages(const uint8_t* file, uint64_t len, const SchemaLeaf& leaf,
         }
         out->dict = payload;
         out->dict_len = uint32_t(h.compressed);
+        if (lz4) {
+          if (!inflate(payload, uint32_t(h.compressed), h.uncompressed, true, &out->dict)) return;
+          out->dict_len = uint32_t(h.uncompressed);
+        }
         out->dict_num_values = uint32_t(h.num_values);
       } else if (h.type == PG_DATA) {
         PageInfo pg;
@@ -375,6 +463,10 @@ void walk_chunk_pages(const uint8_t* file, uint64_t len, const SchemaLeaf& leaf,
         pg.num_values = uint32_t(h.num_values);
         const uint8_t* q = payload;
         const uint8_t* pend = payload + h.compressed;
+        if (lz4 && !device_inflates(leaf, h)) {  // levels and values are one block
+          if (!inflate(payload, uint32_t(h.compressed), h.uncompressed, true, &q)) return;
+          pend = q + h.uncompressed;
+        }
         if (leaf.max_def > 0) {
           if (h.def_encoding != ENC_RLE) {
             out->error = "v1 page with non-RLE definition levels";
@@ -391,6 +483,7 @@ void walk_chunk_pages(const uint8_t* file, uint64_t len, const SchemaLeaf& leaf,
         }
         pg.values = q;
         pg.values_len = uint32_t(pend - q);
+        if (lz4 && device_inflates(leaf, h) && !validate(&pg, h.uncompressed)) return;
         values_seen += h.num_values;
         out->pages.push_back(pg);
       } else if (h.type == PG_DATA_V2) {
@@ -405,6 +498,18 @@ void walk_chunk_pages(const uint8_t* file, uint64_t len, const SchemaLeaf& leaf,
         pg.def_len = uint32_t(h.def_len);
         pg.values = payload + h.def_len;
         pg.values_len = uint32_t(h.compressed - h.def_len);
+        if (lz4) {  // the levels are stored as they are, the values region is one block unless is_compressed says otherwise
+          const int64_t raw = int64_t(h.uncompressed) - h.def_len;
+          if (device_inflates(leaf, h)) {
+            if (!validate(&pg, raw)) return;
+          } else if (!plain_numeric(leaf, h)) {
+            if (!inflate(pg.values, pg.values_len, raw, h.v2_compressed, &pg.values)) return;
+            pg.values_len = uint32_t(raw);
+          } else if (raw != int64_t(pg.values_len)) {  // PLAIN numeric values stored as they are: read from the file
+            out->error = "uncompressed v2 values region differs from its page's size";
+            return;
+          }
+        }
         values_seen += h.num_values;
         out->pages.push_back(pg);
       }  // index pages and unknown page types are skipped
@@ -764,6 +869,90 @@ template bool parse_delta_binary_packed<int64_t>(const uint8_t*, uint64_t, uint3
 template void unpack_delta_binary_packed<int64_t>(const uint8_t*, int64_t, const DbpMiniblock*, size_t, uint32_t, int64_t*);
 template bool decode_delta_binary_packed<int32_t>(const uint8_t*, uint64_t, uint32_t, std::vector<int32_t>*, uint64_t*, std::string*);
 
+// ---- LZ4_RAW blocks ---------------------------------------------------------------------------------------------
+// A block is a chain of sequences: a token (high nibble: literal length, low nibble: match length - 4, 15 in either
+// extended by bytes up to and including the first that is not 255), the literals, then for every sequence but the last a
+// 2-byte little-endian offset and the match length extension.  liblz4's decoder adds the end-of-block rules checked here.
+
+bool parse_lz4_raw(const uint8_t* src, uint64_t len, uint64_t out_len, std::string* err) {
+  auto bad = [&](const char* m) {
+    *err = std::string("LZ4_RAW block: ") + m;
+    return false;
+  };
+  if (len == 0) return bad("empty (a block holds at least one token)");
+  if (out_len == 0) {  // (liblz4 takes the one block 0x00 for an empty output)
+    if (src[0] >> 4) return bad("output longer than the header says");
+    if (src[0] != 0) return bad("the empty output's block is not 0x00");
+    return len == 1 ? true : bad("bytes behind the last sequence");
+  }
+  uint64_t ip = 0, op = 0;
+  for (;;) {
+    if (ip >= len) return bad("block ends without a sequence without a match");
+    const uint32_t token = src[ip++];
+    uint64_t lit = token >> 4;
+    if (lit == 15) {  // the extension stops at the block's last 15 bytes (they hold at least its literals)
+      if (len < 15 || ip >= len - 15) return bad("literal length extension runs past the block");
+      for (;;) {
+        const uint8_t b = src[ip++];
+        lit += b;
+        if (ip > len - 15) return bad("literal length extension runs past the block");
+        if (b != 255) break;
+      }
+    }
+    if (lit > len - ip) return bad("literal run runs past the block");
+    if (lit > out_len - op) return bad("output longer than the header says");
+    // the last sequence: its literals reach into the output's last 12 bytes or the block's last 8
+    if (op + lit + 12 > out_len || ip + lit + 8 > len) {
+      if (ip + lit != len)
+        return bad(op + lit == out_len ? "bytes behind the last sequence"
+                                       : "a match starts in the last 12 bytes of the output or the last 8 of the block");
+      if (op + lit != out_len) return bad("output shorter than the header says");
+      return true;
+    }
+    ip += lit;
+    op += lit;
+    const uint64_t offset = uint64_t(src[ip]) | (uint64_t(src[ip + 1]) << 8);
+    ip += 2;
+    if (offset == 0) return bad("match offset 0");
+    if (offset > op) return bad("match offset reaches before the start of the output");
+    uint64_t ml = token & 15u;
+    if (ml == 15) {  // the extension stops at the block's last 4 bytes
+      for (;;) {
+        const uint8_t b = src[ip++];
+        ml += b;
+        if (ip > len - 4) return bad("match length extension runs past the block");
+        if (b != 255) break;
+      }
+    }
+    ml += 4;
+    if (ml > out_len - op) return bad("output longer than the header says");
+    if (op + ml + 5 > out_len) return bad("a match ends in the last 5 bytes of the output");
+    op += ml;
+  }
+}
+
+void unpack_lz4_raw(const uint8_t* src, uint64_t len, uint8_t* dst, uint64_t cap) {
+  uint64_t ip = 0, op = 0;
+  while (ip < len && op < cap) {
+    const uint32_t token = src[ip++];
+    uint64_t lit = token >> 4;
+    if (lit == 15)
+      for (uint8_t b = 255; b == 255 && ip < len;) lit += (b = src[ip++]);
+    const uint64_t take = std::min(lit, std::min(len - ip, cap - op));
+    std::memcpy(dst + op, src + ip, size_t(take));
+    ip += lit;
+    op += take;
+    if (ip + 2 > len || op >= cap) break;
+    const uint64_t offset = uint64_t(src[ip]) | (uint64_t(src[ip + 1]) << 8);
+    ip += 2;
+    uint64_t ml = token & 15u;
+    if (ml == 15)
+      for (uint8_t b = 255; b == 255 && ip < len;) ml += (b = src[ip++]);
+    ml += 4;
+    if (offset == 0 || offset > op) break;
+    for (const uint64_t e = std::min(cap, op + ml); op < e; op++) dst[op] = dst[op - offset];  // (overlapping: byte by byte)
+  }
+}
 
 // ---- bloom filters ---------------------------------------------------------------------------------------------
 namespace {

@@ -38,13 +38,17 @@ struct PageInfo {
   uint32_t def_len = 0;
   const uint8_t* values = nullptr;  // encoded values region
   uint32_t values_len = 0;
+  // > 0: `values` is one LZ4_RAW block of `values_len` bytes (in the file) that inflates to `lz4_len` bytes of PLAIN
+  // INT64 / DOUBLE values; the page walk has validated it, the device inflates it at upload (lz4_pages.cu)
+  uint32_t lz4_len = 0;
 };
 
 struct ChunkMeta {
   int32_t leaf = -1;  // index into ParsedFile::leaves
   int32_t codec = 0;
   int64_t num_values = 0;
-  int64_t total_compressed_size = 0;  // footer figure: the algorithmic bytes of this chunk
+  int64_t total_compressed_size = 0;  // footer figure: the chunk's bytes in the file
+  int64_t total_uncompressed_size = 0;  // footer figure: the same, pages inflated (== total_compressed_size without a codec)
   int64_t null_count = -1;            // from chunk statistics when present
   bool has_minmax = false;            // INT64 / DOUBLE chunks: footer statistics carry both bounds
   int64_t min_bits = 0, max_bits = 0; // raw 8-byte bounds of the non-null values
@@ -59,6 +63,10 @@ struct ChunkMeta {
   uint32_t dict_len = 0;
   uint32_t dict_num_values = 0;
   std::vector<PageInfo> pages;
+  // LZ4_RAW chunk: the pages the host inflates (dictionary page, then the data pages' values, or whole v1 pages of an
+  // OPTIONAL column, in file order: one address space for a chunk's string values), kept as long as the file is parsed;
+  // `dict` and the PageInfo pointers of these pages point into it
+  std::vector<uint8_t> inflated;
   std::string error;  // non-empty: chunk is unreadable by this engine (reason); only an error if projected
   // page walk state: footers are parsed eagerly, page headers only for the chunks a query touches
   int64_t data_page_offset = -1, dict_page_offset = -1;
@@ -93,6 +101,20 @@ uint64_t xxhash64(const uint8_t* data, size_t len, uint64_t seed);
 bool sbbf_check(const uint8_t* bitset, uint32_t bytes, uint64_t hash);
 // Sets the bits of `hash` (the writer's half; used by the tests to build filters).
 void sbbf_insert(uint8_t* bitset, uint32_t bytes, uint64_t hash);
+
+// Parquet codecs (CompressionCodec): LZ4_RAW is the one the page walk inflates; every other non-zero codec is refused.
+constexpr int32_t kCodecLz4Raw = 7;
+
+// Parse step of one LZ4_RAW block (the LZ4 block format without a frame) that must inflate to exactly `out_len` bytes.
+// Validates every sequence as liblz4's safe decoder does for an output buffer of `out_len` bytes, without writing any
+// output: no literal run, length extension or offset runs past the block, no match offset is 0 or reaches before the
+// start of the output, the output is exactly `out_len` bytes, the block ends right after a sequence without a match,
+// and the end-of-block rules hold (a match may not start in the last 12 bytes of the output or the last 8 of the block,
+// nor end in the last 5 bytes of the output; literal length extensions stop 15 bytes, match length extensions 4 bytes
+// before the block's end).  An empty output is the block 0x00.
+bool parse_lz4_raw(const uint8_t* src, uint64_t len, uint64_t out_len, std::string* err);
+// Unpack step of a block the parse step accepted: its first `cap` (<= out_len) bytes into `dst`.
+void unpack_lz4_raw(const uint8_t* src, uint64_t len, uint8_t* dst, uint64_t cap);
 
 // One run of an RLE/bit-packed hybrid stream (Parquet "RLE" encoding).
 struct HostRun {

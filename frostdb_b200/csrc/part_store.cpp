@@ -67,6 +67,7 @@ struct ImageWriter {
   // DELTA_BINARY_PACKED pages whose holes the device fills (the image's lists; null: the image has none)
   std::vector<DeltaPage>* delta_pages = nullptr;
   std::vector<DbpMiniblock>* delta_mbs = nullptr;
+  std::vector<Lz4Page>* lz4_pages = nullptr;  // LZ4_RAW pages whose holes the device fills
 };
 
 inline void or_bits(std::vector<uint64_t>& bm, uint64_t pos, uint64_t bits8) {
@@ -248,7 +249,8 @@ namespace {
 void walk_chunk(const ChunkMeta& cm, const SchemaLeaf& leaf, uint32_t n_rows, ChunkWalk* wk) {
   ChunkHost* out = &wk->host;
   out->phys = leaf.phys;
-  out->stored_bytes = uint64_t(cm.total_compressed_size);
+  out->stored_bytes = uint64_t(cm.codec != 0 ? cm.total_uncompressed_size : cm.total_compressed_size);
+  out->codec = cm.codec;
   out->has_minmax = cm.has_minmax;
   out->min_bits = cm.min_bits;
   out->max_bits = cm.max_bits;
@@ -389,7 +391,14 @@ void walk_chunk(const ChunkMeta& cm, const SchemaLeaf& leaf, uint32_t n_rows, Ch
         continue;
       }
       uint64_t need = uint64_t(page_nn[p]) * 8;
-      if (need > pg.values_len) { out->error = "PLAIN page shorter than its value count"; return; }
+      if (need > (pg.lz4_len ? pg.lz4_len : pg.values_len)) { out->error = "PLAIN page shorter than its value count"; return; }
+      if (pg.lz4_len && page_nn[p] > 0) {  // (the block's values become a hole the device fills)
+        wk->plain64.push_back({pg.values, page_nn[p], -1, int32_t(wk->lz4_pages.size())});
+        wk->lz4_pages.push_back(Lz4Page{pg.values, pg.values_len, page_nn[p]});
+        out->lz4_pages++;
+        vo += page_nn[p];
+        continue;
+      }
       wk->plain64.push_back({pg.values, page_nn[p], -1});
       vo += page_nn[p];
     }
@@ -566,6 +575,12 @@ void write_chunk(ChunkWalk& wk, uint32_t n_rows, int tile_rows, GlobalDict* dict
     // (a DELTA_BINARY_PACKED page's values are a hole where its PLAIN twin's would be copied to)
     const uint64_t eoff = w.begin_extent();
     for (const Page64& pg : wk.plain64) {
+      if (pg.lz4 >= 0) {
+        Lz4Page z = wk.lz4_pages[size_t(pg.lz4)];
+        z.hole = w.add_hole(uint64_t(pg.n) * 8);  // relative to the extent region until finish_image rebases it
+        w.lz4_pages->push_back(z);
+        continue;
+      }
       if (pg.delta < 0) {
         w.add_extent(pg.values, uint64_t(pg.n) * 8);
         plain_bytes += uint64_t(pg.n) * 8;
@@ -704,6 +719,7 @@ void finish_image(ImageWriter& w, ColumnImage& img, Part* part, const std::strin
   const uint64_t dev_base = (meta_size + w.ext_size + kAlign - 1) / kAlign * kAlign;
   for (Extent& e : img.staging.extents) e.dst_off += meta_size;
   for (DeltaPage& d : img.staging.delta_pages) d.hole += meta_size;
+  for (Lz4Page& z : img.staging.lz4_pages) z.hole += meta_size;
   for (RowGroupHost& h : part->rgs) {
     ChunkHost& ch = h.cols[column];
     if (ch.off_values < -0) ch.off_values = int64_t(meta_size) + (-ch.off_values - 1);
@@ -735,7 +751,7 @@ bool open_part(const uint8_t* file, uint64_t len, Part* part, std::string* err) 
     for (size_t c = 0; c < rg.chunks.size(); c++) {
       ChunkHost ch;  // skeleton: type and footer size are known before the column is built
       ch.phys = part->pf.leaves[c].phys;
-      ch.stored_bytes = uint64_t(rg.chunks[c].total_compressed_size);
+      ch.stored_bytes = uint64_t(rg.chunks[c].codec != 0 ? rg.chunks[c].total_uncompressed_size : rg.chunks[c].total_compressed_size);
       ch.has_minmax = rg.chunks[c].has_minmax;
       ch.min_bits = rg.chunks[c].min_bits;
       ch.max_bits = rg.chunks[c].max_bits;
@@ -798,6 +814,7 @@ void finish_column(int index_rows, Table* table, Part* part, const std::string& 
   w.device_seeds = img.device_seeds;
   w.delta_pages = &img.staging.delta_pages;
   w.delta_mbs = &img.staging.delta_mbs;
+  w.lz4_pages = &img.staging.lz4_pages;
   for (size_t g = 0; g < part->rgs.size(); g++) {
     RowGroupHost& h = part->rgs[g];
     ChunkHost ch;
@@ -1094,6 +1111,7 @@ std::string describe_part_json(const uint8_t* file, uint64_t len, int tile_rows,
     for (const DeltaPage& d : img.staging.delta_pages)  // the holes the device fills at upload
       unpack_delta_binary_packed<int64_t>(d.src, d.first, img.staging.delta_mbs.data() + d.mb0, d.n_mb, d.v0,
                                           reinterpret_cast<int64_t*>(flat.data() + d.hole));
+    for (const Lz4Page& z : img.staging.lz4_pages) unpack_lz4_raw(z.src, z.len, flat.data() + z.hole, uint64_t(z.n) * 8);
     host_images.push_back(std::move(flat));
     patch_column_pointers(&part, name, host_images.back().data());  // pointers into the host image
     image_bytes += img.dev_bytes;
@@ -1122,6 +1140,7 @@ std::string describe_part_json(const uint8_t* file, uint64_t len, int tile_rows,
       o << "\"kind\":" << int(d.kind) << ",\"has_nulls\":" << int(d.has_nulls) << ",\"n_values\":" << d.n_values
         << ",\"n_runs\":" << d.n_runs << ",\"n_defruns\":" << d.n_defruns << ",\"dict_size\":" << d.dict_size
         << ",\"stored_bytes\":" << c.stored_bytes << ",\"meta_bytes\":" << c.meta_bytes << ",\"null_count\":" << c.null_count;
+      if (c.codec != 0) o << ",\"codec\":" << c.codec << ",\"lz4_device_pages\":" << c.lz4_pages;
       if (c.has_minmax && c.phys == PT_INT64) o << ",\"min\":" << c.min_bits << ",\"max\":" << c.max_bits;
       // Decode through the same directories / tile indexes the kernel uses (small inputs only).
       if (rg.n_rows <= 65536) {

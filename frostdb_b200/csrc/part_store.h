@@ -68,7 +68,9 @@ struct ChunkInterner {
 struct ChunkHost {
   ChunkDesc desc{};            // device pointers (valid once the part is uploaded)
   int32_t phys = -1;           // Parquet physical type
-  uint64_t stored_bytes = 0;   // footer total_compressed_size (algorithmic bytes)
+  uint64_t stored_bytes = 0;   // algorithmic bytes: footer total_compressed_size, total_uncompressed_size with a codec
+  int32_t codec = 0;           // Parquet compression codec of the chunk (0 or LZ4_RAW)
+  uint32_t lz4_pages = 0;      // its pages whose values the device inflates at upload
   uint64_t meta_bytes = 0;     // directories / indexes / LUTs
   std::string error;           // non-empty: unreadable; an error only if a query projects it
   bool has_minmax = false;     // footer statistics of an INT64 / DOUBLE chunk (known before the column is built)
@@ -135,11 +137,22 @@ struct DeltaPage {
   uint64_t hole = 0;    // once the sections are written: image offset of its values
 };
 
-// One page of a CK_PLAIN64 chunk: PLAIN (its value region in the file) or DELTA_BINARY_PACKED (an index into delta_pages).
+// One PLAIN INT64 / DOUBLE page of an LZ4_RAW chunk whose block holds nothing but values: its dense values are a hole of
+// 8 * n bytes in the chunk's value array, which the device fills at upload by inflating the block (lz4_pages.cu).
+struct Lz4Page {
+  const uint8_t* src;  // the block (in the file), validated by the page walk
+  uint32_t len;        // its bytes
+  uint32_t n;          // its non-null values: the first 8 * n bytes of what it inflates to
+  uint64_t hole = 0;   // once the sections are written: image offset of its values
+};
+
+// One page of a CK_PLAIN64 chunk: PLAIN (its value region in the file), DELTA_BINARY_PACKED (an index into delta_pages)
+// or an LZ4_RAW block the device inflates (an index into lz4_pages).
 struct Page64 {
   const uint8_t* values;
   uint32_t n;
-  int32_t delta;  // -1: PLAIN
+  int32_t delta;     // -1: not DELTA_BINARY_PACKED
+  int32_t lz4 = -1;  // -1: not inflated by the device
 };
 
 // What the page walk of one chunk leaves for the section writing (the two halves of building a column).
@@ -156,6 +169,7 @@ struct ChunkWalk {
   std::vector<Page64> plain64;           // pages of an int64 / double chunk, in file order
   std::vector<DeltaPage> delta_pages;    // its DELTA_BINARY_PACKED pages
   std::vector<DbpMiniblock> delta_mbs;   // their miniblocks holding values, `first` rebased onto the chunk's value ordinals
+  std::vector<Lz4Page> lz4_pages;        // its pages the device inflates
   // Non-dictionary string values (PLAIN, DELTA_LENGTH_BYTE_ARRAY, DELTA_BYTE_ARRAY pages), validated: every value lies
   // inside its page.  They are addressed in one 32-bit space per chunk: [0, str_span) the file bytes from str_base,
   // [str_rb0, str_rb0 + str_rebuilt_len) the DELTA_BYTE_ARRAY values rebuilt from their prefixes and suffixes.
@@ -202,6 +216,7 @@ struct ImageStaging {
   // offset), and their miniblocks (DeltaPage::mb0 indexes this list)
   std::vector<DeltaPage> delta_pages;
   std::vector<DbpMiniblock> delta_mbs;
+  std::vector<Lz4Page> lz4_pages;    // LZ4_RAW pages of every chunk, whose values the device inflates at upload (hole: image offset)
   std::vector<StrCodeJob> str_jobs;  // PLAIN string pages whose indices the device writes at upload (dst: image offset)
 };
 

@@ -30,8 +30,11 @@ cudaError_t h2d(fgpu_ctx* ctx, void* dst, const void* src, size_t bytes) {
   return cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, ctx->stream);
 }
 
-// A source range; `last`: the transfer ends with it.
-struct Range { const uint8_t* src; uint64_t len; bool last = false; };
+// A source range; `last`: the transfer ends with it; `own`: it lies in a buffer of its own (host-inflated LZ4_RAW pages,
+// not the part's file), so that it is a transfer of its own.
+struct Range { const uint8_t* src; uint64_t len; bool last = false; bool own = false; };
+
+bool outside_file(const Part* part, const uint8_t* p) { return p < part->file || p >= part->file + part->file_bytes; }
 // One transfer of the source ranges [first, first + n); where it goes in the staging buffer is its caller's choice.
 struct Span { const uint8_t* src; uint64_t len, stage_off; size_t first, n; };
 
@@ -43,13 +46,13 @@ std::vector<Span> coalesce(const std::vector<Range>& ranges) {
   for (size_t i = 0; i < ranges.size(); i++) {
     const Range& r = ranges[i];
     const uint8_t* end = closed ? nullptr : spans.back().src + spans.back().len;
-    if (end && r.src >= end && uint64_t(r.src - end) <= kGap) {
+    if (end && !r.own && r.src >= end && uint64_t(r.src - end) <= kGap) {
       spans.back().len = uint64_t(r.src - spans.back().src) + r.len;
       spans.back().n++;
     } else {
       spans.push_back({r.src, r.len, 0, i, 1});
     }
-    closed = r.last;
+    closed = r.last || r.own;
   }
   return spans;
 }
@@ -83,6 +86,7 @@ struct StrBatch {
 int32_t intern_plain_strings(fgpu_ctx* ctx, Table* table, const std::vector<std::pair<Part*, std::string>>& cols, StrBatch* batch) {
   struct Item {
     ChunkWalk* wk;
+    Part* part;
     uint64_t v0, s0, cap, byte_off;
     uint64_t l0, d0, w0, r0;  // in the batch's lengths, prefix / suffix, window and rebuilt-value arrays
   };
@@ -97,7 +101,7 @@ int32_t intern_plain_strings(fgpu_ctx* ctx, Table* table, const std::vector<std:
       if (!wk.host.error.empty() || wk.str_off.empty()) continue;
       uint64_t cap = 16;
       while (cap < 2 * uint64_t(wk.str_off.size())) cap <<= 1;
-      items.push_back({&wk, nv, ns, cap, 0, nl, nd, nw, nr});
+      items.push_back({&wk, pc.first, nv, ns, cap, 0, nl, nd, nw, nr});
       nv += wk.str_off.size();
       ns += cap;
       nl += wk.str_len.size();
@@ -113,7 +117,8 @@ int32_t intern_plain_strings(fgpu_ctx* ctx, Table* table, const std::vector<std:
   // value regions: neighbouring chunks' regions travel as one transfer, 16-byte aligned; a chunk with
   // DELTA_BYTE_ARRAY values ends its span, and its rebuilt values follow at str_rb0 from its first byte
   std::vector<Range> ranges;
-  for (const Item& it : items) ranges.push_back({it.wk->str_base, it.wk->str_span, !it.wk->str_fronts.empty()});
+  for (const Item& it : items)
+    ranges.push_back({it.wk->str_base, it.wk->str_span, !it.wk->str_fronts.empty(), outside_file(it.part, it.wk->str_base)});
   std::vector<Span> spans = coalesce(ranges);
   uint64_t payload = 0;
   for (Span& sp : spans) {
@@ -269,10 +274,10 @@ struct PlainStage {
   uint64_t table_off = 0, end = 0;
 };
 
-PlainStage plan_plain(const std::vector<Extent>& extents) {
+PlainStage plan_plain(const Part* part, const std::vector<Extent>& extents) {
   PlainStage p;
   std::vector<Range> ranges;
-  for (const Extent& x : extents) ranges.push_back({x.src, x.len});
+  for (const Extent& x : extents) ranges.push_back({x.src, x.len, false, outside_file(part, x.src)});
   p.spans = coalesce(ranges);
   for (Span& sp : p.spans) {
     if (sp.n == 1) continue;
@@ -310,10 +315,10 @@ struct DbpStage {
   uint64_t end() const { return scratch_off + dbp_scratch_bytes(uint32_t(n_groups)); }
 };
 
-DbpStage plan_dbp(const ImageStaging& s, uint8_t* dev, uint64_t base) {
+DbpStage plan_dbp(const Part* part, const ImageStaging& s, uint8_t* dev, uint64_t base) {
   DbpStage p;
   std::vector<Range> ranges;
-  for (const DeltaPage& d : s.delta_pages) ranges.push_back({d.src, d.len});
+  for (const DeltaPage& d : s.delta_pages) ranges.push_back({d.src, d.len, false, outside_file(part, d.src)});
   p.spans = coalesce(ranges);
   uint64_t off = base;
   for (Span& sp : p.spans) {
@@ -358,8 +363,48 @@ cudaError_t stage_dbp(fgpu_ctx* ctx, const DbpStage& p, uint8_t* stage, uint64_t
   return e;
 }
 
+// LZ4_RAW PLAIN INT64 / DOUBLE pages: their blocks straight from the source file (neighbours a page header apart as one
+// transfer, each transfer followed by 16 pad bytes), then the job table, from `base` in the staging buffer.
+struct Lz4Stage {
+  std::vector<Span> spans;
+  std::vector<Lz4Job> jobs;
+  uint64_t tab_off = 0;
+  uint64_t end() const { return tab_off + jobs.size() * sizeof(Lz4Job); }
+};
+
+Lz4Stage plan_lz4(const ImageStaging& s, uint8_t* dev, uint64_t base) {
+  Lz4Stage p;
+  std::vector<Range> ranges;
+  for (const Lz4Page& z : s.lz4_pages) ranges.push_back({z.src, z.len});
+  p.spans = coalesce(ranges);
+  uint64_t off = base;
+  for (Span& sp : p.spans) {
+    sp.stage_off = off;
+    off += al16(sp.len) + 16;
+    for (size_t i = sp.first; i < sp.first + sp.n; i++) {
+      const Lz4Page& z = s.lz4_pages[i];
+      p.jobs.push_back(Lz4Job{dev + z.hole, sp.stage_off + uint64_t(z.src - sp.src), z.len, z.n * 8});
+    }
+  }
+  p.tab_off = off;
+  return p;
+}
+
+cudaError_t stage_lz4(fgpu_ctx* ctx, const Lz4Stage& p, uint8_t* stage, uint64_t* copied) {
+  cudaError_t e = h2d(ctx, stage + p.tab_off, p.jobs.data(), p.jobs.size() * sizeof(Lz4Job));
+  *copied += p.jobs.size() * sizeof(Lz4Job);
+  for (const Span& sp : p.spans) {
+    if (e != cudaSuccess) break;
+    *copied += sp.len;
+    e = cudaMemcpyAsync(stage + sp.stage_off, sp.src, sp.len, cudaMemcpyHostToDevice, ctx->stream);
+  }
+  if (e == cudaSuccess) e = launch_lz4_pages(stage, reinterpret_cast<const Lz4Job*>(stage + p.tab_off), uint32_t(p.jobs.size()), ctx->stream);
+  return e;
+}
+
 // Uploads one built column of one part if it is not resident yet: the host-assembled meta region with one copy, the
-// PLAIN value regions and DELTA_BINARY_PACKED streams straight from the source file through one staging allocation,
+// PLAIN value regions, DELTA_BINARY_PACKED streams and LZ4_RAW value blocks straight from the source file (or from the
+// host-inflated pages of an LZ4_RAW chunk) through one staging allocation,
 // then the string pages' indices and the cursor seeds, all on the engine stream so that kernels queued behind need no
 // extra synchronisation.
 int32_t upload_column(fgpu_ctx* ctx, Part* part, const std::string& column, uint64_t* h2d_bytes) {
@@ -373,15 +418,18 @@ int32_t upload_column(fgpu_ctx* ctx, Part* part, const std::string& column, uint
   cudaError_t e = h2d(ctx, dev, s.meta.data(), s.meta.size());
   uint64_t copied = s.meta.size();
   {
-    const PlainStage plain = plan_plain(s.extents);
-    const DbpStage dbp = plan_dbp(s, d, al16(plain.end));
+    const PlainStage plain = plan_plain(part, s.extents);
+    const DbpStage dbp = plan_dbp(part, s, d, al16(plain.end));
+    const uint64_t dbp_end = dbp.pages.empty() ? plain.end : dbp.end();
+    const Lz4Stage lz4 = plan_lz4(s, d, al16(dbp_end));
     if (dbp.n_groups > 0xffffffffull) e = cudaErrorInvalidValue;  // (more than 2^37 values in one column of one part)
     DevBuf stage;  // released in stream order when it goes out of scope
-    if ((!plain.copies.empty() || !dbp.pages.empty()) && e == cudaSuccess)
-      e = stage.alloc(dbp.pages.empty() ? plain.end : dbp.end(), ctx->stream);
+    if ((!plain.copies.empty() || !dbp.pages.empty() || !lz4.jobs.empty()) && e == cudaSuccess)
+      e = stage.alloc(lz4.jobs.empty() ? dbp_end : lz4.end(), ctx->stream);
     uint8_t* st = static_cast<uint8_t*>(stage.p);
     if (e == cudaSuccess) e = stage_plain(ctx, plain, s.extents, d, st, &copied);
     if (e == cudaSuccess && !dbp.pages.empty()) e = stage_dbp(ctx, dbp, st, &copied);
+    if (e == cudaSuccess && !lz4.jobs.empty()) e = stage_lz4(ctx, lz4, st, &copied);
   }
   if (e == cudaSuccess) e = launch_str_jobs(ctx, s.str_jobs, dev);
   if (e == cudaSuccess) e = launch_make_seeds(dev, img.seed_jobs_off, img.n_seed_jobs, img.max_seed_chunks, ctx->stream);

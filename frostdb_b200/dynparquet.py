@@ -32,6 +32,7 @@ class ColumnDefinition:
     dynamic: bool = False
     rle_dictionary: bool = False
     delta_binary_packed: bool = False  # StorageLayout_ENCODING_DELTA_BINARY_PACKED (int64 columns only)
+    compression: str = "NONE"  # StorageLayout.Compression: "NONE" or "LZ4_RAW" (COMPRESSION_LZ4_RAW)
 
 
 @dataclasses.dataclass
@@ -113,6 +114,9 @@ def SampleDefinitionWithFloat() -> Schema:
     return s
 
 
+_CODECS = {"NONE": "NONE", "LZ4_RAW": "LZ4"}
+
+
 def _arrow_column(defn: ColumnDefinition, values, n_rows: int) -> pa.Array:
     if isinstance(values, (pa.Array, pa.ChunkedArray)):
         return values
@@ -185,7 +189,7 @@ def write_part(schema: Schema, columns: Dict[str, object], *, sort: bool = True,
         elif ln != n_rows:
             raise ValueError(f"column {n} has {ln} rows, expected {n_rows}")
     perm = sort_permutation(schema, columns, n_rows) if sort and n_rows > 1 else None
-    fields, arrays, dict_cols, plain_cols = [], [], [], {}
+    fields, arrays, dict_cols, plain_cols, codecs = [], [], [], {}, {}
     dyn: Dict[str, List[str]] = {}
     for n in names:
         defn = schema.definition_for(n)
@@ -208,6 +212,9 @@ def write_part(schema: Schema, columns: Dict[str, object], *, sort: bool = True,
             dict_cols.append(n)
         else:
             plain_cols[n] = "DELTA_BINARY_PACKED" if defn.delta_binary_packed else "PLAIN"
+        if defn.compression not in _CODECS:
+            raise ValueError(f"column {n}: compression {defn.compression!r} is not one of {sorted(_CODECS)}")
+        codecs[n] = _CODECS[defn.compression]
         if defn.dynamic:
             dyn.setdefault(defn.name, []).append(n.split(".", 1)[1])
         fields.append(pa.field(n, arr.type, nullable=nullable))
@@ -222,7 +229,9 @@ def write_part(schema: Schema, columns: Dict[str, object], *, sort: bool = True,
         kwargs["data_page_size"] = data_page_size
     if dictionary_pagesize_limit is not None:
         kwargs["dictionary_pagesize_limit"] = dictionary_pagesize_limit
-    pq.write_table(table, sink, compression="NONE", use_dictionary=dict_cols,
+    # (pyarrow's "lz4" is Parquet's LZ4_RAW, codec 7; every column uncompressed keeps the one-codec call)
+    compression = codecs if any(c != "NONE" for c in codecs.values()) else "NONE"
+    pq.write_table(table, sink, compression=compression, use_dictionary=dict_cols,
                    column_encoding=plain_cols or None, data_page_version=data_page_version,
                    row_group_size=row_group_size or max(n_rows, 1), write_statistics=write_statistics,
                    store_schema=False, **kwargs)

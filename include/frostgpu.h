@@ -333,6 +333,11 @@ int32_t fgpu_xxhash64(const uint8_t* data, uint64_t len, uint64_t seed, uint64_t
 int32_t fgpu_bloom_check(const uint8_t* bitset, uint64_t nbytes, uint64_t hash, int32_t* out_may_contain);
 int32_t fgpu_bloom_insert(uint8_t* bitset, uint64_t nbytes, uint64_t hash);
 
+/* One LZ4_RAW block (Parquet codec 7: the LZ4 block format without a frame) that must inflate to exactly `cap` bytes,
+ * the size a page header records: validated as the page walk validates a page's block, then inflated into dst (NULL:
+ * validate only).  *out_len: the bytes written.  A refused block returns FGPU_ERR_PARQUET naming the rule it breaks. */
+int32_t fgpu_lz4_raw_inflate(const uint8_t* src, uint64_t len, uint8_t* dst, uint64_t cap, uint64_t* out_len);
+
 /* The row-group filter's answer for "column == literal" on one row group of a Parquet file, exactly as
  * fgpu_query_execute decides it before anything is uploaded (null count, bloom filter, bounds; LSM.Scan,
  * index/lsm.go:401-454 -> expr/binaryscalarexpr.go:84-128).  lit_type: FGPU_SCALAR_*.  *out: 1 may match, 0 cannot. */
