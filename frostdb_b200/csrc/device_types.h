@@ -340,7 +340,11 @@ struct RunsDesc {
 // ---- all-pass sorted row groups from prefix sums (k_runs_prefix, runs_prefix.cu) ----------------------------
 // A sorted-run row group whose filter the chunk statistics decided (every row passes) and whose stored aggregates are
 // all Sum(int64) is answered from the run directories of its key columns and the exclusive prefix sums of its Sum inputs
-// (ensure_narrow): the rows [b, e) of one group add P[e] - P[b] and e - b.  The host cuts the row groups into windows.
+// (ensure_narrow): the rows [b, e) of one group add P[e] - P[b] and e - b.
+//
+// The segments [b, e) (maximal stretches of one row group with one dense slot) depend only on the key directories and
+// the dense strides, so a build step (k_prefix_segs) enumerates them once per compiled plan, from windows the host cuts,
+// into a table grouped by slot; every Execute then folds each slot's list (k_runs_prefix).
 struct PrefixRg {
   uint32_t n_rows;
   uint32_t _pad;
@@ -355,11 +359,32 @@ struct alignas(16) PrefixWin {
   uint32_t rg, r0, rows, _pad;  // rows [r0, r0 + rows) of row group rg
 };
 
-struct PrefixDesc {
-  uint32_t n_win, nk, na;
+struct PrefixSeg {
+  uint32_t rg, b, e;  // rows [b, e) of row group rg (index into the launch's PrefixRg array)
+};
+
+// Build step: count the segments of every slot (cnt, zeroed), exclusive scan into seg_off, then scatter them (cnt
+// counts down to 0 again).
+struct PrefixBuildDesc {
+  uint32_t n_win, nk;
   uint32_t stride[kRunsKeys];  // dense-table stride of every key
   const PrefixRg* rgs;
   const PrefixWin* wins;
+  uint32_t* cnt;           // [table_slots + 1]
+  const uint32_t* seg_off;  // [table_slots + 1]
+  PrefixSeg* seg;
+};
+
+// Execute: every slot of the dense table gets its rows and Sums stored (0 without segments), and counters[0..9] are
+// set (rows selected = all rows of the prefix row groups), so this launch replaces k_table_init.
+struct PrefixDesc {
+  uint32_t n_slots, na;
+  uint32_t group_log2;  // lanes per slot: 1 << group_log2 up to 32; above 5: a CTA per slot
+  uint32_t _pad;
+  unsigned long long all_rows;
+  const PrefixRg* rgs;
+  const uint32_t* seg_off;
+  const PrefixSeg* seg;
   unsigned long long* t_rows;
   long long* t_agg[kRunsAggs];
   unsigned long long* counters;

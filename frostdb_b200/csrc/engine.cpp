@@ -225,6 +225,7 @@ struct fgpu_result {
   QueryDesc qd{};
   FinalizeDesc fd{};
   DevBuf table, aux, cnt;
+  DevBuf segs;  // the prefix path's segment table (see ExecCache::segs) when the plan is not cached
   size_t table_bytes = 0;
   unsigned int* cnt_ptr = nullptr;  // group counter inside `aux` when the scan counted the result rows
   bool groups_known = false;  // the scan's own stream already counted the result rows
@@ -365,8 +366,9 @@ uint8_t chunk_leaf_mode(int64_t lo, int64_t hi, bool neg, bool has_bounds, int64
   return stats_leaf_mode(lo, hi, neg, mn, mx, null_count == 0);
 }
 
-// The launches of an aggregate scan between k_table_init and the general k_scan, in issue order: sorted runs
-// (k_runs_tma), prefix sums (k_runs_prefix), tile aggregate (k_tile_agg).
+// The launches of an aggregate scan before the general k_scan, in issue order: k_runs_prefix when the plan has prefix
+// row groups (it stores every slot of the table), k_table_init otherwise, then sorted runs (k_runs_tma) and tile
+// aggregate (k_tile_agg), which add to the table atomically.
 struct ScanLaunch {
   bool runs = false, prefix = false, tile = false;
   RunsDesc rd{};
@@ -381,6 +383,10 @@ struct ScanLaunch {
 // stream synchronisation per Execute; dense tables of this size are compacted into the result record on the host.
 struct ExecCache {
   DevBuf aux, table, out;         // descriptors; [aggregate table | counters 128 B]; compacted result image
+  // The prefix path's segment table (seg_off, seg: PrefixBuildDesc), built by the plan's first Execute.  It holds only
+  // dense slots and row positions derived from the key columns' run directories, never a value: every Execute reads
+  // the Sum inputs' prefix images afresh and stores every slot, so no aggregate survives from one Execute to the next.
+  DevBuf segs;
   DenseOut dout{};
   size_t out_bytes = 0;
   std::vector<std::unique_ptr<OwnedColumn>> dict_template;  // per key: the whole dictionary, ready to copy (small dictionaries)
@@ -1400,13 +1406,14 @@ int32_t cached_merge_tail(fgpu_ctx* ctx, ExecCache& x, uint64_t seq, uint64_t by
   return rc;
 }
 
-// k_table_init, the aggregate-scan launches, k_scan; ev[1] and ev[2] bracket the scan kernels.
+// k_runs_prefix or k_table_init, the other aggregate-scan launches, k_scan; ev[1] and ev[2] bracket the scan kernels
+// (with k_runs_prefix among them).
 int32_t launch_aggregate_scan(fgpu_ctx* ctx, const QueryDesc& qd, const QueryDesc* qdesc_dev, const ScanLaunch& L) {
   cudaStream_t s = ctx->stream;
-  CUDA_TRY(launch_table_init(qd, s));
+  if (!L.prefix) CUDA_TRY(launch_table_init(qd, s));
   CUDA_TRY(cudaEventRecord(ctx->ev[1], s));
-  if (L.runs) CUDA_TRY(launch_runs_tma(L.rd, L.runs_nl, L.runs_nk, L.runs_na, ctx->sm_count, s));
   if (L.prefix) CUDA_TRY(launch_runs_prefix(L.pd, ctx->sm_count, s));
+  if (L.runs) CUDA_TRY(launch_runs_tma(L.rd, L.runs_nl, L.runs_nk, L.runs_na, ctx->sm_count, s));
   if (L.tile) CUDA_TRY(launch_tile_agg(L.td, ctx->sm_count, s));
   CUDA_TRY(launch_scan(qdesc_dev, qd, ctx->sm_count, s));
   CUDA_TRY(cudaEventRecord(ctx->ev[2], s));
@@ -1668,11 +1675,25 @@ bool runs_admit(RunsPlan& P, const Compiled& c, const QueryDesc& qd, const Visib
 // kPrefixRunRows rows: then a step per group run is cheaper than reading its rows.
 constexpr uint64_t kPrefixRunRows = 64;
 struct PrefixPlan {
-  PrefixDesc pd{};
+  PrefixBuildDesc bd{};
   std::vector<PrefixRg> rgs;
   std::vector<std::array<ChunkHost*, kRunsAggs>> sums;  // per row group: the chunk of every Sum input
   std::vector<Part*> parts;
   std::vector<PrefixWin> wins;
+  uint64_t seg_bound = 0;  // segments at most: every run start of every key column and every window start
+  uint64_t all_rows = 0;   // rows of the admitted row groups (they all pass)
+  uint32_t n_sums = 1;     // distinct Sum inputs of the first row group (as the accounting counts them)
+};
+
+// After the build step: its launches, and the bytes an Execute reads per segment (entry + P[b], P[e] of every distinct
+// Sum input), counted once the build's segment count is back on the host.
+struct PrefixBuilt {
+  const uint32_t* count = nullptr;  // page-locked: seg_off[table_slots]
+  uint64_t per_seg = 0;
+  uint32_t launches = 0;
+  void account(fgpu_stats& st) const {
+    if (count) st.algorithmic_bytes += uint64_t(*count) * per_seg;
+  }
 };
 
 bool prefix_query(const RunsPlan& R, const Switches& w) {
@@ -1698,23 +1719,28 @@ bool prefix_admit(PrefixPlan& P, const RunsPlan& R, const RunsCand& rc, fgpu_sta
   if (uint64_t(rr.n_rows) < kPrefixRunRows * sum_runs) return false;
   PrefixRg pr{};
   pr.n_rows = rr.n_rows;
-  for (int k = 0; k < R.nk; k++) {
+  for (int k = 0; k < R.nk; k++) {  // (the directories are read by the plan's build step, not by an Execute)
     pr.runs[k] = rr.runs[k];
     pr.seeds[k] = rr.seeds[k];
     pr.n_runs[k] = rr.n_runs[k];
-    st.algorithmic_bytes += uint64_t(rr.n_runs[k]) * sizeof(Run);  // the directories, read whole
   }
   const uint32_t win = runs_prefix_window_rows(rr.n_rows, uint32_t(sum_runs));
   uint32_t n_win = 0;
   for (uint32_t r0 = 0; r0 < rr.n_rows; r0 += win, n_win++)
     P.wins.push_back(PrefixWin{uint32_t(P.rgs.size()), r0, std::min(win, rr.n_rows - r0), 0u});
-  // a Sum input is read at the segment boundaries (at most every run start, every window start and the end), not
-  // row by row
+  P.seg_bound += sum_runs + n_win;
+  P.all_rows += rr.n_rows;
+  // a Sum input is read at the segment boundaries, not row by row (PrefixBuilt counts those reads)
+  uint32_t n_sums = 0;
   for (int a = 0; a < R.na; a++) {
     bool first = true;
     for (int a2 = 0; a2 < a; a2++) first = first && sums[size_t(a2)] != sums[size_t(a)];
-    if (first) st.algorithmic_bytes = st.algorithmic_bytes - sums[size_t(a)]->stored_bytes + (sum_runs + n_win + 1) * 8;
+    if (first) {
+      st.algorithmic_bytes -= sums[size_t(a)]->stored_bytes;
+      n_sums++;
+    }
   }
+  if (P.rgs.empty()) P.n_sums = n_sums;
   P.rgs.push_back(pr);
   P.sums.push_back(sums);
   P.parts.push_back(rc.cols.part);
@@ -1743,11 +1769,10 @@ int32_t runs_layout(fgpu_ctx* ctx, const Compiled& c, const Switches& w, RunsPla
       }
   }
   if (!P.rgs.empty()) {
-    PrefixDesc& pd = P.pd;
-    pd.n_win = uint32_t(P.wins.size());
-    pd.nk = uint32_t(R.nk);
-    pd.na = uint32_t(R.na);
-    for (int k = 0; k < R.nk; k++) pd.stride[k] = R.rd.stride[k];
+    PrefixBuildDesc& bd = P.bd;
+    bd.n_win = uint32_t(P.wins.size());
+    bd.nk = uint32_t(R.nk);
+    for (int k = 0; k < R.nk; k++) bd.stride[k] = R.rd.stride[k];
   }
   if (R.rgs.empty()) return FGPU_OK;
   RunsDesc& rd = R.rd;
@@ -2150,7 +2175,8 @@ std::unique_ptr<OwnedColumn> dict_column(const std::vector<std::string>& values,
 
 // First Execute of a cached plan: the plan keeps the device state; the dense table comes back compacted by
 // k_finalize_dense (see ExecCache).
-int32_t keep_exec_cache(fgpu_ctx* ctx, const QueryPlan& q, Compiled& c, const QueryDesc& qd, fgpu_result* res, PhaseClock& pc) {
+int32_t keep_exec_cache(fgpu_ctx* ctx, const QueryPlan& q, Compiled& c, const QueryDesc& qd, fgpu_result* res, PhaseClock& pc,
+                        const PrefixBuilt& pb) {
   cudaStream_t s = ctx->stream;
   fgpu_stats& st = res->stats;
   ExecCache& x = *c.exec;
@@ -2200,13 +2226,15 @@ int32_t keep_exec_cache(fgpu_ctx* ctx, const QueryPlan& q, Compiled& c, const Qu
   st.total_device_ms = ms;
   const unsigned long long* cnts = reinterpret_cast<const unsigned long long*>(x.pinned + 32);
   st.rows_selected = cnts[0];
+  pb.account(st);
   x.qd = qd;
   result_shape(q, c, &x.keys, &x.agg_names, &x.agg_is_float);
   for (const KeyOut& k : x.keys) {  // small dictionaries are exported whole: the host then only copies index columns
     x.dict_template.push_back(k.dict_snapshot.size() <= 4096 ? dict_column(k.dict_snapshot, nullptr) : nullptr);
   }
   st.kernel_launches++;  // k_finalize_dense (cached_tail)
-  x.stats = st;  // what a cached Execute reports: no uploads, no compile
+  x.stats = st;  // what a cached Execute reports: no uploads, no compile, no segment-table build
+  x.stats.kernel_launches -= pb.launches;
   x.stats.h2d_bytes = 0;
   x.stats.d2h_bytes = 0;
   x.stats.rows_selected = 0;
@@ -2400,6 +2428,7 @@ int32_t run_scan(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, fgpu_result* re
   CUDA_TRY(cudaEventRecord(ctx->ev[0], s));
   CUDA_TRY(cudaMemcpyAsync(aux, ctx->scratch, aux_bytes, cudaMemcpyHostToDevice, s));
   ScanLaunch L;
+  PrefixBuilt pb;
   if (rows_plan) {
     CUDA_TRY(cudaMemsetAsync(qd.tile_state, 0, size_t(G.tiles) * 8, s));
     CUDA_TRY(cudaEventRecord(ctx->ev[1], s));
@@ -2429,12 +2458,47 @@ int32_t run_scan(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, fgpu_result* re
     L.runs_nk = R.nk;
     L.runs_na = R.na;
     L.prefix = !P.rgs.empty();
-    L.pd = P.pd;
-    L.pd.rgs = reinterpret_cast<const PrefixRg*>(aux + o_prefix);
-    L.pd.wins = reinterpret_cast<const PrefixWin*>(aux + o_win);
-    L.pd.t_rows = qd.t_rows;
-    for (int a = 0; a < R.na; a++) L.pd.t_agg[a] = qd.t_agg[R.agg_index[a]];
-    L.pd.counters = qd.counters;
+    if (L.prefix) {
+      // k_runs_prefix stores every cell of the table in place of k_table_init: only right when the table is dense and
+      // every stored aggregate is Sum(int64) (identity 0), which prefix_query and runs_query let through
+      if (qd.table_mode != TM_DENSE) return fail(FGPU_ERR_INVALID, "prefix path planned for a hash-mode table");
+      for (int a = 0; a < qd.n_aggs; a++)
+        if (qd.aggs[a].func != FGPU_AGG_COUNT && (qd.aggs[a].func != FGPU_AGG_SUM || qd.aggs[a].is_float))
+          return fail(FGPU_ERR_INVALID, "prefix path planned for a table with an aggregate other than Sum(int64)");
+      // the plan's segment table: [seg_off | seg | build scratch]
+      const uint32_t n_slots = uint32_t(qd.table_slots);
+      const size_t off_bytes = HostImage::align16(size_t(n_slots + 1) * 4), seg_bytes = HostImage::align16(P.seg_bound * sizeof(PrefixSeg));
+      DevBuf& sbuf = cache_mode ? c.exec->segs : res->segs;
+      CUDA_TRY(sbuf.alloc(off_bytes + seg_bytes + prefix_build_scratch_bytes(n_slots), s));
+      uint8_t* sb = static_cast<uint8_t*>(sbuf.p);
+      const uint32_t* seg_off = reinterpret_cast<const uint32_t*>(sb);
+      PrefixBuildDesc bd = P.bd;
+      bd.rgs = reinterpret_cast<const PrefixRg*>(aux + o_prefix);
+      bd.wins = reinterpret_cast<const PrefixWin*>(aux + o_win);
+      bd.seg = reinterpret_cast<PrefixSeg*>(sb + off_bytes);
+      CUDA_TRY(launch_prefix_build(bd, n_slots, reinterpret_cast<uint32_t*>(sb), sb + off_bytes + seg_bytes, ctx->sm_count, s));
+      uint32_t* count = reinterpret_cast<uint32_t*>(ctx->scratch + o_ret + 96);
+      CUDA_TRY(cudaMemcpyAsync(count, seg_off + n_slots, 4, cudaMemcpyDeviceToHost, s));
+      pb.count = count;
+      pb.per_seg = sizeof(PrefixSeg) + 16 * uint64_t(P.n_sums);
+      pb.launches = 3;  // count, scan (as one), scatter
+      st.kernel_launches += pb.launches;
+      st.algorithmic_bytes += uint64_t(n_slots + 1) * 4;  // seg_off
+      PrefixDesc& pd = L.pd;
+      pd.n_slots = n_slots;
+      pd.na = uint32_t(R.na);
+      // lanes per slot: about one segment each up to a warp; a CTA per slot for lists of several hundred
+      const uint64_t per_slot = (P.seg_bound + n_slots - 1) / n_slots;
+      while (pd.group_log2 < 5 && (uint64_t(1) << pd.group_log2) < per_slot) pd.group_log2++;
+      if (per_slot >= 256) pd.group_log2 = 8;
+      pd.all_rows = P.all_rows;
+      pd.rgs = bd.rgs;
+      pd.seg_off = seg_off;
+      pd.seg = bd.seg;
+      pd.t_rows = qd.t_rows;
+      for (int a = 0; a < R.na; a++) pd.t_agg[a] = qd.t_agg[R.agg_index[a]];
+      pd.counters = qd.counters;
+    }
     L.tile = !T.rgs.empty();
     L.td = T.td;
     L.td.rgs = reinterpret_cast<const TileAggRg*>(aux + o_tile);
@@ -2448,7 +2512,7 @@ int32_t run_scan(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, fgpu_result* re
     st.row_groups_prefix += uint32_t(P.rgs.size());
     st.row_groups_tiles += uint32_t(T.rgs.size());
   }
-  st.kernel_launches += (rows_plan ? 0 : 1) + (G.tiles ? 1 : 0);
+  st.kernel_launches += (rows_plan || L.prefix ? 0 : 1) + (G.tiles ? 1 : 0);  // k_table_init, k_scan
   st.h2d_bytes += aux_bytes + sizeof(QueryDesc);
   unsigned long long* counters = reinterpret_cast<unsigned long long*>(ctx->scratch + o_ret);
   res->cnt_ptr = reinterpret_cast<unsigned int*>(qd.counters + 8);  // 16 bytes behind the counters, zeroed by the upload / the table init
@@ -2464,7 +2528,7 @@ int32_t run_scan(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, fgpu_result* re
     x.table_bytes = tbytes;
     x.qdesc_dev = qdesc_dev;
     x.launch = L;
-    return keep_exec_cache(ctx, q, c, qd, res, pc);
+    return keep_exec_cache(ctx, q, c, qd, res, pc, pb);
   }
   if (count_groups && !rows_plan) {  // count the result rows behind the scan: one host round trip less
     CUDA_TRY(launch_count_groups(fd, res->cnt_ptr, s));
@@ -2481,6 +2545,7 @@ int32_t run_scan(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, fgpu_result* re
   CUDA_TRY(cudaEventElapsedTime(&ms, ctx->ev[1], ctx->ev[2]));
   st.scan_kernel_ms = ms;
   st.rows_selected = counters[0];
+  pb.account(st);
   if (res->groups_known) res->n_groups = static_cast<unsigned int>(counters[8] & 0xffffffffull);
   st.d2h_bytes += 64;
   if (counters[1]) return fail(FGPU_ERR_UNSUPPORTED, "aggregate hash table overflow (more groups than the sized capacity)");

@@ -27,6 +27,10 @@ int runs_tma_ctas_per_sm(const RunsDesc& d);
 cudaError_t launch_runs_tma(const RunsDesc& d, int nl, int nk, int na, int sm_count, cudaStream_t st);
 // all-pass sorted row groups from the key run directories and prefix-sum images (runs_prefix.cu)
 uint32_t runs_prefix_window_rows(uint32_t n_rows, uint32_t sum_runs);  // rows per window of one row group
+// build step of a plan's segment table: `scratch` of prefix_build_scratch_bytes(n_slots) bytes; the table's segment
+// count ends up in seg_off[n_slots]
+size_t prefix_build_scratch_bytes(uint32_t n_slots);
+cudaError_t launch_prefix_build(PrefixBuildDesc d, uint32_t n_slots, uint32_t* seg_off, void* scratch, int sm_count, cudaStream_t st);
 cudaError_t launch_runs_prefix(const PrefixDesc& d, int sm_count, cudaStream_t st);
 // filter-only plans over PLAIN columns (take_rows.cu): count per span, scan, ordered write
 cudaError_t launch_take(const TakeDesc& d, int sm_count, cudaStream_t st);
