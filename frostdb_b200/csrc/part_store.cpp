@@ -15,18 +15,32 @@ constexpr size_t kTailPad = 16;
 // bytes copied verbatim from the source file].  Section offsets of the extent region are recorded
 // relative to its start and rebased when the meta size is final.
 struct ImageWriter {
-  std::vector<uint8_t>& buf;
-  std::vector<Extent>& extents;
+  ImageStaging& staging;
+  std::vector<uint8_t>& buf;        // staging.meta
   uint64_t ext_size = 0;
   uint64_t dev_size = 0;            // device-only region behind the extents (seeds derived on the device)
   bool device_seeds = false;
   std::vector<SeedJob> jobs;
-  ImageWriter(std::vector<uint8_t>& b, std::vector<Extent>& e) : buf(b), extents(e) {}
+  explicit ImageWriter(ImageStaging& s) : staging(s), buf(s.meta) {}
   uint64_t reserve_dev(uint64_t n) {
     dev_size = (dev_size + kAlign - 1) / kAlign * kAlign;
     uint64_t off = dev_size;
     dev_size += n + kTailPad;
     return off;
+  }
+  // queues k_make_seeds' derivation of n_chunks cursor seeds from the run directory at runs_off (val0_off: the chunks'
+  // first value ordinals, ~0: chunk * 128); returns the seeds' offset in the device-only region
+  int64_t seed_job(int64_t runs_off, uint32_t n_runs, uint32_t total, uint32_t n_chunks, bool is_def, uint64_t val0_off) {
+    SeedJob j{};
+    j.runs_off = uint64_t(runs_off);
+    j.seeds_off = reserve_dev(uint64_t(n_chunks) * sizeof(Seed));
+    j.val0_off = val0_off;
+    j.n_runs = n_runs;
+    j.total = total;
+    j.n_chunks = n_chunks;
+    j.is_def = is_def ? 1 : 0;
+    jobs.push_back(j);
+    return int64_t(j.seeds_off);
   }
   size_t begin() {
     size_t n = (buf.size() + kAlign - 1) / kAlign * kAlign;
@@ -51,23 +65,24 @@ struct ImageWriter {
   }
   void add_extent(const uint8_t* src, uint64_t len) {
     if (len == 0) return;
+    std::vector<Extent>& extents = staging.extents;
     if (!extents.empty() && extents.back().src + extents.back().len == src && extents.back().dst_off + extents.back().len == ext_size)
       extents.back().len += len;  // contiguous in the file too: one copy
     else
       extents.push_back({src, len, ext_size});
     ext_size += len;
   }
-  // reserves `len` bytes of the extent region without a copy (the device writes them); returns their offset in it
-  uint64_t add_hole(uint64_t len) {
-    const uint64_t off = ext_size;
-    ext_size += len;
-    return off;
+  // reserves the values of a page the device fills (8 * n bytes of the extent region, not copied) and queues the page
+  // with its miniblocks (`mbs`: the chunk's list); its hole is relative to the extent region until finish_image rebases it
+  void add_hole(const ValuePage& pg, const std::vector<DbpMiniblock>& mbs) {
+    ValuePage h = pg;
+    h.hole = ext_size;
+    h.mb0 = uint32_t(staging.dbp_mbs.size());
+    staging.dbp_mbs.insert(staging.dbp_mbs.end(), mbs.begin() + pg.mb0, mbs.begin() + pg.mb0 + pg.n_mb);
+    staging.value_pages.push_back(h);
+    ext_size += uint64_t(pg.n) * 8;
   }
   void end_extent() { ext_size += kTailPad; }
-  // DELTA_BINARY_PACKED pages whose holes the device fills (the image's lists; null: the image has none)
-  std::vector<DeltaPage>* delta_pages = nullptr;
-  std::vector<DbpMiniblock>* delta_mbs = nullptr;
-  std::vector<Lz4Page>* lz4_pages = nullptr;  // LZ4_RAW pages whose holes the device fills
 };
 
 inline void or_bits(std::vector<uint64_t>& bm, uint64_t pos, uint64_t bits8) {
@@ -214,14 +229,47 @@ bool walk_delta_int64(const PageInfo& pg, uint32_t n, uint32_t v0, ChunkWalk* wk
     return false;
   }
   if (n == 0) return true;
-  const DeltaPage d{pg.values, s.used, int64_t(s.first), v0, n, s.per_mb, uint32_t(wk->delta_mbs.size()), uint32_t(s.mbs.size())};
+  wk->value_pages.push_back({FILL_DBP, pg.values, s.used, v0, n, int64_t(s.first), s.per_mb, uint32_t(wk->dbp_mbs.size()),
+                             uint32_t(s.mbs.size())});
   for (DbpMiniblock& mb : s.mbs) {
     mb.first += v0;
-    wk->delta_mbs.push_back(mb);
+    wk->dbp_mbs.push_back(mb);
   }
-  wk->plain64.push_back({pg.values, n, int32_t(wk->delta_pages.size())});
-  wk->delta_pages.push_back(d);
   return true;
+}
+
+// The entries of a chunk's string dictionary page, validated, each handed to `entry(bytes, length)`.
+template <typename F>
+bool each_dict_string(const ChunkMeta& cm, F entry, std::string* err) {
+  const uint8_t* p = cm.dict;
+  const uint8_t* end = cm.dict + cm.dict_len;
+  for (uint32_t i = 0; i < cm.dict_num_values; i++) {
+    if (end - p < 4) { *err = "dictionary page truncated"; return false; }
+    uint32_t l;
+    std::memcpy(&l, p, 4);
+    p += 4;
+    if (l > uint64_t(end - p)) { *err = "dictionary entry overruns page"; return false; }
+    entry(p, l);
+    p += l;
+  }
+  return true;
+}
+
+// The footer facts of one chunk: known before its pages are walked (a part's skeleton) and kept by the built chunk.
+ChunkHost chunk_footer(const ChunkMeta& cm, const SchemaLeaf& leaf, uint32_t n_rows) {
+  ChunkHost ch;
+  ch.phys = leaf.phys;
+  ch.stored_bytes = uint64_t(cm.codec != 0 ? cm.total_uncompressed_size : cm.total_compressed_size);
+  ch.codec = cm.codec;
+  ch.has_minmax = cm.has_minmax;
+  ch.min_bits = cm.min_bits;
+  ch.max_bits = cm.max_bits;
+  ch.null_count = (cm.null_count < 0 && leaf.max_def == 0) ? 0 : cm.null_count;  // (a required column has none)
+  ch.has_minmax_str = cm.has_minmax_str;
+  ch.min_str = cm.min_str;
+  ch.max_str = cm.max_str;
+  ch.desc.n_rows = n_rows;
+  return ch;
 }
 
 }  // namespace
@@ -243,22 +291,22 @@ void unfront_strings(ChunkWalk* wk) {
   wk->str_rebuilt = rb;
 }
 
+void fill_value_pages(const ImageStaging& s, uint8_t* image) {
+  for (const ValuePage& pg : s.value_pages) {
+    uint8_t* dst = image + pg.hole;
+    if (pg.fill == FILL_DBP)
+      unpack_delta_binary_packed<int64_t>(pg.src, pg.first, s.dbp_mbs.data() + pg.mb0, pg.n_mb, pg.v0, reinterpret_cast<int64_t*>(dst));
+    else
+      unpack_lz4_raw(pg.src, pg.len, dst, uint64_t(pg.n) * 8);
+  }
+}
+
 namespace {
 
 // Walks and validates every page of one column chunk (first half of building it).
 void walk_chunk(const ChunkMeta& cm, const SchemaLeaf& leaf, uint32_t n_rows, ChunkWalk* wk) {
   ChunkHost* out = &wk->host;
-  out->phys = leaf.phys;
-  out->stored_bytes = uint64_t(cm.codec != 0 ? cm.total_uncompressed_size : cm.total_compressed_size);
-  out->codec = cm.codec;
-  out->has_minmax = cm.has_minmax;
-  out->min_bits = cm.min_bits;
-  out->max_bits = cm.max_bits;
-  out->null_count = (cm.null_count < 0 && leaf.max_def == 0) ? 0 : cm.null_count;
-  out->has_minmax_str = cm.has_minmax_str;
-  out->min_str = cm.min_str;
-  out->max_str = cm.max_str;
-  out->desc.n_rows = n_rows;
+  *out = chunk_footer(cm, leaf, n_rows);
   if (!cm.error.empty()) { out->error = cm.error; return; }
   if (leaf.phys != PT_INT64 && leaf.phys != PT_DOUBLE && leaf.phys != PT_BYTE_ARRAY) {
     out->error = "unsupported physical type " + std::to_string(leaf.phys);
@@ -289,17 +337,12 @@ void walk_chunk(const ChunkMeta& cm, const SchemaLeaf& leaf, uint32_t n_rows, Ch
     uint32_t row = 0;
     for (size_t p = 0; p < cm.pages.size(); p++) {
       const PageInfo& pg = cm.pages[p];
-      size_t first = defruns.size();
-      // a merged RLE run may extend the previous page's last run: remember where this page starts
-      uint32_t page_start = row;
       if (!walk_hybrid(pg.def, pg.def_len, 1, pg.num_values, row, uint32_t(defstream.size()), &defruns, &err)) {
         out->error = "definition levels: " + err;
         return;
       }
       defstream.insert(defstream.end(), pg.def, pg.def + pg.def_len);
-      (void)first;
       row += pg.num_values;
-      (void)page_start;
     }
     if (row != n_rows) { out->error = "definition levels do not cover the row group"; return; }
     all_present = defruns.size() == 1 && (defruns[0].meta & 1u) == 0 && defruns[0].val == 1;
@@ -311,7 +354,6 @@ void walk_chunk(const ChunkMeta& cm, const SchemaLeaf& leaf, uint32_t n_rows, Ch
   }
   if (leaf.max_def == 1 && !all_present) {
     valid.assign((size_t(n_rows) + 63) / 64 + 1, 0);
-    uint32_t row = 0;
     for (size_t k = 0; k < defruns.size(); k++) {
       const HostRun& r = defruns[k];
       uint32_t end = (k + 1 < defruns.size()) ? defruns[k + 1].start : n_rows;
@@ -326,7 +368,7 @@ void walk_chunk(const ChunkMeta& cm, const SchemaLeaf& leaf, uint32_t n_rows, Ch
         }
       }
     }
-    row = 0;
+    uint32_t row = 0;
     uint64_t total_valid = 0;
     for (size_t p = 0; p < cm.pages.size(); p++) {
       const PageInfo& pg = cm.pages[p];
@@ -385,22 +427,19 @@ void walk_chunk(const ChunkMeta& cm, const SchemaLeaf& leaf, uint32_t n_rows, Ch
     uint32_t vo = 0;
     for (size_t p = 0; p < cm.pages.size(); p++) {
       const PageInfo& pg = cm.pages[p];
+      const uint32_t n = page_nn[p];
       if (pg.encoding == ENC_DELTA_BINARY_PACKED) {  // (INT64 only: the encoding check above refuses it elsewhere)
-        if (!walk_delta_int64(pg, page_nn[p], vo, wk, &err)) { out->error = err; return; }
-        vo += page_nn[p];
-        continue;
-      }
-      uint64_t need = uint64_t(page_nn[p]) * 8;
-      if (need > (pg.lz4_len ? pg.lz4_len : pg.values_len)) { out->error = "PLAIN page shorter than its value count"; return; }
-      if (pg.lz4_len && page_nn[p] > 0) {  // (the block's values become a hole the device fills)
-        wk->plain64.push_back({pg.values, page_nn[p], -1, int32_t(wk->lz4_pages.size())});
-        wk->lz4_pages.push_back(Lz4Page{pg.values, pg.values_len, page_nn[p]});
+        if (!walk_delta_int64(pg, n, vo, wk, &err)) { out->error = err; return; }
+      } else if (uint64_t(n) * 8 > (pg.lz4_len ? pg.lz4_len : pg.values_len)) {
+        out->error = "PLAIN page shorter than its value count";
+        return;
+      } else if (pg.lz4_len && n > 0) {  // (the block's values become a hole the device fills)
+        wk->value_pages.push_back({FILL_LZ4, pg.values, pg.values_len, vo, n});
         out->lz4_pages++;
-        vo += page_nn[p];
-        continue;
+      } else {
+        wk->value_pages.push_back({FILL_COPY, pg.values, uint64_t(n) * 8, vo, n});
       }
-      wk->plain64.push_back({pg.values, page_nn[p], -1});
-      vo += page_nn[p];
+      vo += n;
     }
     out->desc.kind = CK_PLAIN64;
   }
@@ -408,18 +447,9 @@ void walk_chunk(const ChunkMeta& cm, const SchemaLeaf& leaf, uint32_t n_rows, Ch
   // ---- dictionary ---------------------------------------------------------------------------
   uint32_t dict_size = 0;
   if (out->desc.kind == CK_DICT_STR) {
-    const uint8_t* p = cm.dict;
-    const uint8_t* end = cm.dict + cm.dict_len;
     wk->dict_entries.reserve(cm.dict_num_values);
-    for (uint32_t i = 0; i < cm.dict_num_values; i++) {
-      if (end - p < 4) { out->error = "dictionary page truncated"; return; }
-      uint32_t l;
-      std::memcpy(&l, p, 4);
-      p += 4;
-      if (l > uint64_t(end - p)) { out->error = "dictionary entry overruns page"; return; }
-      wk->dict_entries.push_back({p, l});
-      p += l;
-    }
+    auto entry = [&](const uint8_t* p, uint32_t l) { wk->dict_entries.push_back({p, l}); };
+    if (!each_dict_string(cm, entry, &err)) { out->error = err; return; }
     dict_size = cm.dict_num_values;
   } else if (out->desc.kind == CK_DICT64) {
     if (uint64_t(cm.dict_num_values) * 8 > cm.dict_len) { out->error = "numeric dictionary page truncated"; return; }
@@ -569,28 +599,13 @@ void write_chunk(ChunkWalk& wk, uint32_t n_rows, int tile_rows, GlobalDict* dict
   out->desc.has_nulls = has_nulls ? 1 : 0;
   out->desc.n_values = n_values;
   out->desc.dict_size = dict_size;
-  uint64_t plain_bytes = 0;
   if (out->desc.kind == CK_PLAIN64) {
     // value regions go to the device straight from the file: negative offsets mark "extent region"
-    // (a DELTA_BINARY_PACKED page's values are a hole where its PLAIN twin's would be copied to)
+    // (a page the device fills is a hole where its PLAIN twin's values would be copied to)
     const uint64_t eoff = w.begin_extent();
-    for (const Page64& pg : wk.plain64) {
-      if (pg.lz4 >= 0) {
-        Lz4Page z = wk.lz4_pages[size_t(pg.lz4)];
-        z.hole = w.add_hole(uint64_t(pg.n) * 8);  // relative to the extent region until finish_image rebases it
-        w.lz4_pages->push_back(z);
-        continue;
-      }
-      if (pg.delta < 0) {
-        w.add_extent(pg.values, uint64_t(pg.n) * 8);
-        plain_bytes += uint64_t(pg.n) * 8;
-        continue;
-      }
-      DeltaPage d = wk.delta_pages[size_t(pg.delta)];
-      d.hole = w.add_hole(uint64_t(pg.n) * 8);  // relative to the extent region until finish_image rebases it
-      w.delta_pages->push_back(d);
-      w.delta_pages->back().mb0 = uint32_t(w.delta_mbs->size());
-      w.delta_mbs->insert(w.delta_mbs->end(), wk.delta_mbs.begin() + d.mb0, wk.delta_mbs.begin() + d.mb0 + d.n_mb);
+    for (const ValuePage& pg : wk.value_pages) {
+      if (pg.fill == FILL_COPY) w.add_extent(pg.src, pg.len);
+      else w.add_hole(pg, wk.dbp_mbs);
     }
     w.end_extent();
     out->off_values = -int64_t(eoff) - 1;
@@ -600,18 +615,6 @@ void write_chunk(ChunkWalk& wk, uint32_t n_rows, int tile_rows, GlobalDict* dict
   }
   uint64_t val0_off = ~0ull;
   if (w.device_seeds && has_nulls) val0_off = uint64_t(w.section(chunk_val0.data(), chunk_val0.size() * 4));
-  auto seed_job = [&](int64_t runs_off, uint32_t n_runs, uint32_t total, bool is_def, bool use_val0 = true) {
-    SeedJob j{};
-    j.runs_off = uint64_t(runs_off);
-    j.seeds_off = w.reserve_dev(uint64_t(n_chunks) * sizeof(Seed));
-    j.val0_off = use_val0 ? val0_off : ~0ull;
-    j.n_runs = n_runs;
-    j.total = total;
-    j.n_chunks = n_chunks;
-    j.is_def = is_def ? 1 : 0;
-    w.jobs.push_back(j);
-    return int64_t(j.seeds_off);
-  };
   // ---- row-space directory of a nullable dictionary column whose two streams are run-length only ----
   // (what a sorted part leaves: NULLs first, then one run per value).  The sorted-run kernel walks it like
   // the directory of a column without NULLs; 0xffffffff stands for NULL (contributes 0 to the dense slot).
@@ -652,7 +655,7 @@ void write_chunk(ChunkWalk& wk, uint32_t n_rows, int tile_rows, GlobalDict* dict
     HostRun sentinel{n_values, 0, 0, 0};
     vruns.push_back(sentinel);
     out->off_runs = w.section(vruns.data(), vruns.size() * sizeof(HostRun));
-    if (w.device_seeds) out->dev_seeds = seed_job(out->off_runs, out->desc.n_runs, n_values, false);
+    if (w.device_seeds) out->dev_seeds = w.seed_job(out->off_runs, out->desc.n_runs, n_values, n_chunks, false, val0_off);
     else out->off_seeds = w.section(seeds.data(), seeds.size() * sizeof(Seed));
   }
   if (has_nulls) {
@@ -663,7 +666,7 @@ void write_chunk(ChunkWalk& wk, uint32_t n_rows, int tile_rows, GlobalDict* dict
     defruns.push_back(sentinel);
     out->off_def = w.section(defstream.data(), defstream.size());
     out->off_def_runs = w.section(defruns.data(), defruns.size() * sizeof(HostRun));
-    if (w.device_seeds) out->dev_def_seeds = seed_job(out->off_def_runs, out->desc.n_defruns, n_rows, true);
+    if (w.device_seeds) out->dev_def_seeds = w.seed_job(out->off_def_runs, out->desc.n_defruns, n_rows, n_chunks, true, val0_off);
     else out->off_def_seeds = w.section(seeds.data(), seeds.size() * sizeof(Seed));
   }
   if (!row_runs.empty()) {
@@ -672,7 +675,7 @@ void write_chunk(ChunkWalk& wk, uint32_t n_rows, int tile_rows, GlobalDict* dict
     if (!w.device_seeds) seeds = make_seeds(row_runs, n_rows, true);
     row_runs.push_back(HostRun{n_rows, 0, 0, 0});
     out->off_row_runs = w.section(row_runs.data(), row_runs.size() * sizeof(HostRun));
-    if (w.device_seeds) out->dev_row_seeds = seed_job(out->off_row_runs, out->desc.n_row_runs, n_rows, true, /*use_val0=*/false);
+    if (w.device_seeds) out->dev_row_seeds = w.seed_job(out->off_row_runs, out->desc.n_row_runs, n_rows, n_chunks, true, ~0ull);
     else out->off_row_seeds = w.section(seeds.data(), seeds.size() * sizeof(Seed));
   }
   // Bit-packed indices are not range-checked row by row (neither here nor in the kernels): the tables they index are
@@ -699,7 +702,6 @@ void write_chunk(ChunkWalk& wk, uint32_t n_rows, int tile_rows, GlobalDict* dict
     if (padded > dict64.size()) dict64.resize(padded, dict64.empty() ? 0 : dict64[0]);
     out->off_dict64 = w.section(dict64.data(), dict64.size() * 8);
   }
-  (void)plain_bytes;
   const size_t payload = vstream.size() + (has_nulls ? defstream.size() : 0);
   out->meta_bytes = (w.buf.size() - before) - std::min(w.buf.size() - before, payload);
   if (out->dev_seeds >= 0) out->meta_bytes += uint64_t(n_chunks) * sizeof(Seed);
@@ -718,11 +720,10 @@ void finish_image(ImageWriter& w, ColumnImage& img, Part* part, const std::strin
   const uint64_t meta_size = (img.staging.meta.size() + kAlign - 1) / kAlign * kAlign;
   const uint64_t dev_base = (meta_size + w.ext_size + kAlign - 1) / kAlign * kAlign;
   for (Extent& e : img.staging.extents) e.dst_off += meta_size;
-  for (DeltaPage& d : img.staging.delta_pages) d.hole += meta_size;
-  for (Lz4Page& z : img.staging.lz4_pages) z.hole += meta_size;
+  for (ValuePage& pg : img.staging.value_pages) pg.hole += meta_size;
   for (RowGroupHost& h : part->rgs) {
     ChunkHost& ch = h.cols[column];
-    if (ch.off_values < -0) ch.off_values = int64_t(meta_size) + (-ch.off_values - 1);
+    if (ch.off_values < 0) ch.off_values = int64_t(meta_size) + (-ch.off_values - 1);
     if (ch.dev_seeds >= 0) ch.off_seeds = int64_t(dev_base) + ch.dev_seeds;
     if (ch.dev_def_seeds >= 0) ch.off_def_seeds = int64_t(dev_base) + ch.dev_def_seeds;
     if (ch.dev_row_seeds >= 0) ch.off_row_seeds = int64_t(dev_base) + ch.dev_row_seeds;
@@ -749,21 +750,10 @@ bool open_part(const uint8_t* file, uint64_t len, Part* part, std::string* err) 
     RowGroupHost h;
     h.n_rows = uint32_t(rg.num_rows);
     for (size_t c = 0; c < rg.chunks.size(); c++) {
-      ChunkHost ch;  // skeleton: type and footer size are known before the column is built
-      ch.phys = part->pf.leaves[c].phys;
-      ch.stored_bytes = uint64_t(rg.chunks[c].codec != 0 ? rg.chunks[c].total_uncompressed_size : rg.chunks[c].total_compressed_size);
-      ch.has_minmax = rg.chunks[c].has_minmax;
-      ch.min_bits = rg.chunks[c].min_bits;
-      ch.max_bits = rg.chunks[c].max_bits;
-      ch.null_count = rg.chunks[c].null_count;
-      if (ch.null_count < 0 && part->pf.leaves[c].max_def == 0) ch.null_count = 0;  // required column
-      ch.has_minmax_str = rg.chunks[c].has_minmax_str;
-      ch.min_str = rg.chunks[c].min_str;
-      ch.max_str = rg.chunks[c].max_str;
+      ChunkHost ch = chunk_footer(rg.chunks[c], part->pf.leaves[c], h.n_rows);  // skeleton until the column is built
       // (parquet-go sizes the filter by the chunk's values, 10 bits each: anything beyond a few MB is left alone)
       if (rg.chunks[c].bloom && rg.chunks[c].bloom_bytes <= (8u << 20))
         ch.bloom.assign(rg.chunks[c].bloom, rg.chunks[c].bloom + rg.chunks[c].bloom_bytes);
-      ch.desc.n_rows = h.n_rows;
       h.cols.emplace(part->pf.leaves[c].name, std::move(ch));
     }
     part->rgs.push_back(std::move(h));
@@ -810,11 +800,8 @@ void finish_column(int index_rows, Table* table, Part* part, const std::string& 
   GlobalDict* dict = nullptr;
   for (const SchemaLeaf& l : part->pf.leaves)
     if (l.name == column && l.phys == PT_BYTE_ARRAY) dict = &table->dicts[column];
-  ImageWriter w(img.staging.meta, img.staging.extents);
+  ImageWriter w(img.staging);
   w.device_seeds = img.device_seeds;
-  w.delta_pages = &img.staging.delta_pages;
-  w.delta_mbs = &img.staging.delta_mbs;
-  w.lz4_pages = &img.staging.lz4_pages;
   for (size_t g = 0; g < part->rgs.size(); g++) {
     RowGroupHost& h = part->rgs[g];
     ChunkHost ch;
@@ -872,7 +859,7 @@ bool build_arrow_column(Table* table, Part* part, const std::string& name, const
 
   ColumnImage& img = part->images[name];
   img.built = true;
-  ImageWriter w(img.staging.meta, img.staging.extents);
+  ImageWriter w(img.staging);
   w.device_seeds = true;
   ChunkHost ch;
   ch.desc.n_rows = n_rows;
@@ -897,18 +884,6 @@ bool build_arrow_column(Table* table, Part* part, const std::string& name, const
 
   uint64_t val0_off = ~0ull;
   if (has_nulls) val0_off = uint64_t(w.section(val0.data(), val0.size() * 4));
-  auto seed_job = [&](int64_t runs_off, uint32_t n_runs, uint32_t total, bool is_def) {
-    SeedJob j{};
-    j.runs_off = uint64_t(runs_off);
-    j.seeds_off = w.reserve_dev(uint64_t(n_chunks) * sizeof(Seed));
-    j.val0_off = val0_off;
-    j.n_runs = n_runs;
-    j.total = total;
-    j.n_chunks = n_chunks;
-    j.is_def = is_def ? 1 : 0;
-    w.jobs.push_back(j);
-    return int64_t(j.seeds_off);
-  };
 
   if (is_i64 || is_f64) {
     ch.phys = is_i64 ? PT_INT64 : PT_DOUBLE;
@@ -969,7 +944,7 @@ bool build_arrow_column(Table* table, Part* part, const std::string& name, const
     vruns.push_back(HostRun{n_values, 0, 0, 0});
     ch.off_values = w.section(idx.data(), idx.size() * 4);
     ch.off_runs = w.section(vruns.data(), vruns.size() * sizeof(HostRun));
-    ch.dev_seeds = seed_job(ch.off_runs, ch.desc.n_runs, n_values, false);
+    ch.dev_seeds = w.seed_job(ch.off_runs, ch.desc.n_runs, n_values, n_chunks, false, val0_off);
     ch.off_lut = w.section(ch.lut_host.data(), ch.lut_host.size() * 4);
     ch.stored_bytes = uint64_t(n_values) * 4 + (has_nulls ? (n_rows + 7) / 8 : 0);
   }
@@ -980,7 +955,7 @@ bool build_arrow_column(Table* table, Part* part, const std::string& name, const
     druns.push_back(HostRun{n_rows, 0, 0, 0});
     ch.off_def = w.section(defbits.data(), defbits.size());
     ch.off_def_runs = w.section(druns.data(), druns.size() * sizeof(HostRun));
-    ch.dev_def_seeds = seed_job(ch.off_def_runs, 1, n_rows, true);
+    ch.dev_def_seeds = w.seed_job(ch.off_def_runs, 1, n_rows, n_chunks, true, val0_off);
   }
   ch.meta_bytes = uint64_t(n_chunks) * sizeof(Seed) * ((ch.dev_seeds >= 0) + (ch.dev_def_seeds >= 0));
   part->rgs[0].cols[name] = std::move(ch);
@@ -1064,17 +1039,8 @@ bool column_dict_values(const ParsedFile& pf, const std::string& column, GlobalD
         }
         continue;
       }
-      const uint8_t* p = cm.dict;
-      const uint8_t* end = cm.dict + cm.dict_len;
-      for (uint32_t i = 0; i < cm.dict_num_values; i++) {
-        if (end - p < 4) { *err = "dictionary page truncated"; return false; }
-        uint32_t l;
-        std::memcpy(&l, p, 4);
-        p += 4;
-        if (l > uint64_t(end - p)) { *err = "dictionary entry overruns page"; return false; }
-        d->intern(reinterpret_cast<const char*>(p), l);
-        p += l;
-      }
+      auto entry = [&](const uint8_t* p, uint32_t l) { d->intern(reinterpret_cast<const char*>(p), l); };
+      if (!each_dict_string(cm, entry, err)) return false;
     }
   }
   return true;
@@ -1108,10 +1074,7 @@ std::string describe_part_json(const uint8_t* file, uint64_t len, int tile_rows,
     std::vector<uint8_t> flat(size_t(img.dev_bytes), 0);
     std::memcpy(flat.data(), img.staging.meta.data(), img.staging.meta.size());
     for (const Extent& e : img.staging.extents) std::memcpy(flat.data() + e.dst_off, e.src, size_t(e.len));
-    for (const DeltaPage& d : img.staging.delta_pages)  // the holes the device fills at upload
-      unpack_delta_binary_packed<int64_t>(d.src, d.first, img.staging.delta_mbs.data() + d.mb0, d.n_mb, d.v0,
-                                          reinterpret_cast<int64_t*>(flat.data() + d.hole));
-    for (const Lz4Page& z : img.staging.lz4_pages) unpack_lz4_raw(z.src, z.len, flat.data() + z.hole, uint64_t(z.n) * 8);
+    fill_value_pages(img.staging, flat.data());
     host_images.push_back(std::move(flat));
     patch_column_pointers(&part, name, host_images.back().data());  // pointers into the host image
     image_bytes += img.dev_bytes;

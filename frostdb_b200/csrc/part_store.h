@@ -125,34 +125,23 @@ struct StrFront {
   uint32_t v0, d0, w0, n;  // first value; its index in str_pre / str_suf; the page's first window in str_wmin; values
 };
 
-// One DELTA_BINARY_PACKED page of an INT64 chunk: its dense values [v0, v0 + n) are a hole of 8 * n bytes in the
-// chunk's value array, which the device fills at upload from the page's stream (delta_int64.cu).
-struct DeltaPage {
-  const uint8_t* src;   // its encoded stream (in the file)
-  uint64_t len;         // bytes of the stream (what follows it in the page is not read)
-  int64_t first;        // its first value
-  uint32_t v0, n;       // its non-null values: ordinals among the chunk's values
-  uint64_t per_mb;      // values per miniblock
-  uint32_t mb0, n_mb;   // its miniblocks holding values, in the walk's (then the image's) miniblock list
-  uint64_t hole = 0;    // once the sections are written: image offset of its values
-};
+// How the 8 * n bytes of one CK_PLAIN64 page's values reach the chunk's value array: copied from `src` as they are, or
+// a hole the device fills at upload from a DELTA_BINARY_PACKED stream (delta_int64.cu) or by inflating an LZ4_RAW block
+// (lz4_pages.cu).
+enum ValueFill : uint8_t { FILL_COPY, FILL_DBP, FILL_LZ4 };
 
-// One PLAIN INT64 / DOUBLE page of an LZ4_RAW chunk whose block holds nothing but values: its dense values are a hole of
-// 8 * n bytes in the chunk's value array, which the device fills at upload by inflating the block (lz4_pages.cu).
-struct Lz4Page {
-  const uint8_t* src;  // the block (in the file), validated by the page walk
-  uint32_t len;        // its bytes
-  uint32_t n;          // its non-null values: the first 8 * n bytes of what it inflates to
-  uint64_t hole = 0;   // once the sections are written: image offset of its values
-};
-
-// One page of a CK_PLAIN64 chunk: PLAIN (its value region in the file), DELTA_BINARY_PACKED (an index into delta_pages)
-// or an LZ4_RAW block the device inflates (an index into lz4_pages).
-struct Page64 {
-  const uint8_t* values;
-  uint32_t n;
-  int32_t delta;     // -1: not DELTA_BINARY_PACKED
-  int32_t lz4 = -1;  // -1: not inflated by the device
+// One page of a CK_PLAIN64 chunk: its dense values [v0, v0 + n) among the chunk's values.
+struct ValuePage {
+  ValueFill fill;
+  const uint8_t* src;   // COPY: the values; DBP: the encoded stream; LZ4: the block, validated by the page walk
+  uint64_t len;         // bytes read from src (DBP: the stream's; what follows it in the page is not read)
+  uint32_t v0, n;
+  // DBP: the header's first value, values per miniblock, and its miniblocks holding values in the walk's (then the
+  // image's) miniblock list
+  int64_t first = 0;
+  uint64_t per_mb = 0;
+  uint32_t mb0 = 0, n_mb = 0;
+  uint64_t hole = 0;    // DBP / LZ4, once the sections are written: image offset of its values
 };
 
 // What the page walk of one chunk leaves for the section writing (the two halves of building a column).
@@ -166,10 +155,8 @@ struct ChunkWalk {
   std::vector<HostRun> vruns;     // a PLAIN page's entry holds its hole's position in `vstream` until the holes exist
   std::vector<std::pair<const uint8_t*, uint32_t>> dict_entries;  // string dictionary page, validated
   std::vector<int64_t> dict64;
-  std::vector<Page64> plain64;           // pages of an int64 / double chunk, in file order
-  std::vector<DeltaPage> delta_pages;    // its DELTA_BINARY_PACKED pages
-  std::vector<DbpMiniblock> delta_mbs;   // their miniblocks holding values, `first` rebased onto the chunk's value ordinals
-  std::vector<Lz4Page> lz4_pages;        // its pages the device inflates
+  std::vector<ValuePage> value_pages;  // pages of an int64 / double chunk, in file order
+  std::vector<DbpMiniblock> dbp_mbs;   // its DBP pages' miniblocks holding values, `first` rebased onto the chunk's values
   // Non-dictionary string values (PLAIN, DELTA_LENGTH_BYTE_ARRAY, DELTA_BYTE_ARRAY pages), validated: every value lies
   // inside its page.  They are addressed in one 32-bit space per chunk: [0, str_span) the file bytes from str_base,
   // [str_rb0, str_rb0 + str_rebuilt_len) the DELTA_BYTE_ARRAY values rebuilt from their prefixes and suffixes.
@@ -212,13 +199,16 @@ void unfront_strings(ChunkWalk* wk);
 struct ImageStaging {
   std::vector<uint8_t> meta;  // everything that is not an extent
   std::vector<Extent> extents;
-  // DELTA_BINARY_PACKED int64 pages of every chunk, whose values the device writes at upload (DeltaPage::hole: image
-  // offset), and their miniblocks (DeltaPage::mb0 indexes this list)
-  std::vector<DeltaPage> delta_pages;
-  std::vector<DbpMiniblock> delta_mbs;
-  std::vector<Lz4Page> lz4_pages;    // LZ4_RAW pages of every chunk, whose values the device inflates at upload (hole: image offset)
+  // the value pages of every chunk whose values the device writes at upload (not FILL_COPY; hole: image offset), and
+  // their miniblocks (ValuePage::mb0 indexes this list)
+  std::vector<ValuePage> value_pages;
+  std::vector<DbpMiniblock> dbp_mbs;
   std::vector<StrCodeJob> str_jobs;  // PLAIN string pages whose indices the device writes at upload (dst: image offset)
 };
+
+// The host's reference of the device's fills: writes the values of every page in s.value_pages into its hole of
+// `image`, a host copy of the column image.
+void fill_value_pages(const ImageStaging& s, uint8_t* image);
 
 // Device residency of one column of one part (all its row groups in one allocation).
 struct ColumnImage {

@@ -35,7 +35,9 @@ cudaError_t h2d(fgpu_ctx* ctx, void* dst, const void* src, size_t bytes) {
 struct Range { const uint8_t* src; uint64_t len; bool last = false; bool own = false; };
 
 bool outside_file(const Part* part, const uint8_t* p) { return p < part->file || p >= part->file + part->file_bytes; }
-// One transfer of the source ranges [first, first + n); where it goes in the staging buffer is its caller's choice.
+// One transfer of the source ranges [first, first + n); where it goes in the staging buffer is its caller's choice
+// (kToImage: not in it).
+constexpr uint64_t kToImage = ~uint64_t(0);
 struct Span { const uint8_t* src; uint64_t len, stage_off; size_t first, n; };
 
 // Source ranges in ascending order, neighbours a few page headers apart joined into one transfer.
@@ -50,7 +52,7 @@ std::vector<Span> coalesce(const std::vector<Range>& ranges) {
       spans.back().len = uint64_t(r.src - spans.back().src) + r.len;
       spans.back().n++;
     } else {
-      spans.push_back({r.src, r.len, 0, i, 1});
+      spans.push_back({r.src, r.len, kToImage, i, 1});
     }
     closed = r.last || r.own;
   }
@@ -265,148 +267,128 @@ cudaError_t launch_str_jobs(fgpu_ctx* ctx, std::vector<StrCodeJob>& jobs, void* 
   return e;
 }
 
-// PLAIN pages: neighbouring page payloads (separated by a page header) travel as ONE transfer of the raw bytes into
-// the staging buffer (16-byte aligned, >= 16 pad bytes behind) and are gathered into the dense value array on the
-// device; a payload without neighbours goes straight to its place.  Staging: [spans][PageCopy table].
-struct PlainStage {
-  std::vector<Span> spans;
-  std::vector<PageCopy> copies;
-  uint64_t table_off = 0, end = 0;
-};
-
-PlainStage plan_plain(const Part* part, const std::vector<Extent>& extents) {
-  PlainStage p;
-  std::vector<Range> ranges;
-  for (const Extent& x : extents) ranges.push_back({x.src, x.len, false, outside_file(part, x.src)});
-  p.spans = coalesce(ranges);
-  for (Span& sp : p.spans) {
-    if (sp.n == 1) continue;
-    sp.stage_off = p.table_off;
-    p.table_off += al16(sp.len) + 16;
-    for (size_t i = sp.first; i < sp.first + sp.n; i++)
-      p.copies.push_back({sp.stage_off + uint64_t(extents[i].src - sp.src), extents[i].dst_off, extents[i].len});
-  }
-  p.end = p.table_off + p.copies.size() * sizeof(PageCopy);
-  return p;
-}
-
-cudaError_t stage_plain(fgpu_ctx* ctx, const PlainStage& p, const std::vector<Extent>& extents, uint8_t* dev, uint8_t* stage,
-                        uint64_t* copied) {
-  cudaError_t e = cudaSuccess;
-  if (!p.copies.empty()) e = h2d(ctx, stage + p.table_off, p.copies.data(), p.copies.size() * sizeof(PageCopy));
-  for (const Span& sp : p.spans) {
-    if (e != cudaSuccess) break;
-    *copied += sp.len;
-    uint8_t* dst = sp.n == 1 ? dev + extents[sp.first].dst_off : stage + sp.stage_off;
-    e = cudaMemcpyAsync(dst, sp.src, sp.len, cudaMemcpyHostToDevice, ctx->stream);
-  }
-  if (e == cudaSuccess && !p.copies.empty())
-    e = launch_gather_pages(stage, dev, reinterpret_cast<const PageCopy*>(stage + p.table_off), uint32_t(p.copies.size()), ctx->stream);
-  return e;
-}
-
-// DELTA_BINARY_PACKED pages: their streams (neighbours a page header apart as one transfer, each transfer followed by
-// 16 pad bytes), then the page and miniblock tables, then the decode's scratch, from `base` in the staging buffer.
-struct DbpStage {
-  std::vector<Span> spans;
-  std::vector<DbpPage> pages;
-  std::vector<DbpMini> mbs;
-  uint64_t n_groups = 0, tab_off = 0, scratch_off = 0;
-  uint64_t end() const { return scratch_off + dbp_scratch_bytes(uint32_t(n_groups)); }
-};
-
-DbpStage plan_dbp(const Part* part, const ImageStaging& s, uint8_t* dev, uint64_t base) {
-  DbpStage p;
-  std::vector<Range> ranges;
-  for (const DeltaPage& d : s.delta_pages) ranges.push_back({d.src, d.len, false, outside_file(part, d.src)});
-  p.spans = coalesce(ranges);
-  uint64_t off = base;
-  for (Span& sp : p.spans) {
+// Source ranges of one kind of page in ascending order, coalesced and placed in the staging buffer from `off`: each
+// transfer 16-byte aligned with >= 16 pad bytes behind it.  direct: a transfer of one range is not placed (stage_off
+// stays kToImage), it goes straight to its place in the image.  row(i, at): range i lies at `at` in the staging buffer.
+// Returns the end of the last placed transfer's padding.
+template <typename Row>
+uint64_t place(const std::vector<Range>& ranges, uint64_t off, bool direct, std::vector<Span>* spans, Row row) {
+  *spans = coalesce(ranges);
+  for (Span& sp : *spans) {
+    if (direct && sp.n == 1) continue;
     sp.stage_off = off;
     off += al16(sp.len) + 16;
-    for (size_t i = sp.first; i < sp.first + sp.n; i++) {
-      const DeltaPage& d = s.delta_pages[i];
+    for (size_t i = sp.first; i < sp.first + sp.n; i++) row(i, sp.stage_off + uint64_t(ranges[i].src - sp.src));
+  }
+  return off;
+}
+
+// The staging buffer of one column upload, one piece per kind of page, each piece 16-byte aligned (a kind without pages
+// takes no space), and the tables the kernels read from it:
+// - PLAIN pages: neighbouring page payloads (separated by a page header) as one transfer, then the PageCopy table;
+//   k_gather_pages copies them into the dense value array.  A payload without neighbours goes straight to its place.
+// - DELTA_BINARY_PACKED pages: their streams, then the page and miniblock tables, then the decode's scratch.
+// - LZ4_RAW PLAIN INT64 / DOUBLE pages: their blocks, then the job table.
+// Ranges of different kinds are never joined into one transfer.
+struct StagePlan {
+  std::vector<Span> plain, dbp, lz4;
+  std::vector<PageCopy> copies;
+  std::vector<DbpPage> dbp_pages;
+  std::vector<DbpMini> dbp_mbs;
+  std::vector<Lz4Job> lz4_jobs;
+  uint64_t n_groups = 0;  // 32-value groups of the DELTA_BINARY_PACKED decode
+  uint64_t copies_off = 0, dbp_tab_off = 0, scratch_off = 0, lz4_tab_off = 0;
+  uint64_t bytes = 0;     // of the buffer (0: nothing is staged)
+};
+
+StagePlan plan_stage(const Part* part, const ImageStaging& s, uint8_t* dev) {
+  StagePlan p;
+  std::vector<Range> ranges;
+  auto range = [&](const uint8_t* src, uint64_t len) { ranges.push_back({src, len, false, outside_file(part, src)}); };
+  for (const Extent& x : s.extents) range(x.src, x.len);
+  p.copies_off = place(ranges, 0, /*direct=*/true, &p.plain, [&](size_t i, uint64_t at) {
+    p.copies.push_back({at, s.extents[i].dst_off, s.extents[i].len});
+  });
+  uint64_t end = p.copies_off + p.copies.size() * sizeof(PageCopy);
+  std::vector<const ValuePage*> dbp, lz4;  // the pages the device fills, per kind in image order
+  for (const ValuePage& pg : s.value_pages) (pg.fill == FILL_DBP ? dbp : lz4).push_back(&pg);
+  if (!dbp.empty()) {
+    ranges.clear();
+    for (const ValuePage* pg : dbp) range(pg->src, pg->len);
+    p.dbp_tab_off = place(ranges, al16(end), false, &p.dbp, [&](size_t i, uint64_t at) {
+      const ValuePage& d = *dbp[i];
       DbpPage pg{};
       pg.dst = reinterpret_cast<unsigned long long*>(dev + d.hole);
-      pg.src = sp.stage_off + uint64_t(d.src - sp.src);
+      pg.src = at;
       pg.first = static_cast<unsigned long long>(d.first);
       pg.n = d.n;
       pg.g0 = uint32_t(p.n_groups);
-      pg.mb0 = uint32_t(p.mbs.size());
+      pg.mb0 = uint32_t(p.dbp_mbs.size());
       pg.per_mb = uint32_t(std::min<uint64_t>(d.per_mb, 0xffffffffu));
       p.n_groups += (d.n + 31) / 32;
       for (uint32_t m = d.mb0; m < d.mb0 + d.n_mb; m++)
-        p.mbs.push_back(DbpMini{s.delta_mbs[m].min_delta, uint32_t(s.delta_mbs[m].off), s.delta_mbs[m].width});
-      p.pages.push_back(pg);
-    }
+        p.dbp_mbs.push_back(DbpMini{s.dbp_mbs[m].min_delta, uint32_t(s.dbp_mbs[m].off), s.dbp_mbs[m].width});
+      p.dbp_pages.push_back(pg);
+    });
+    p.scratch_off = al16(p.dbp_tab_off + p.dbp_pages.size() * sizeof(DbpPage) + p.dbp_mbs.size() * sizeof(DbpMini));
+    end = p.scratch_off + dbp_scratch_bytes(uint32_t(p.n_groups));
   }
-  p.tab_off = off;
-  p.scratch_off = al16(p.tab_off + p.pages.size() * sizeof(DbpPage) + p.mbs.size() * sizeof(DbpMini));
+  if (!lz4.empty()) {
+    ranges.clear();
+    for (const ValuePage* pg : lz4) range(pg->src, pg->len);
+    p.lz4_tab_off = place(ranges, al16(end), false, &p.lz4, [&](size_t i, uint64_t at) {
+      p.lz4_jobs.push_back(Lz4Job{dev + lz4[i]->hole, at, uint32_t(lz4[i]->len), lz4[i]->n * 8});
+    });
+    end = p.lz4_tab_off + p.lz4_jobs.size() * sizeof(Lz4Job);
+  }
+  if (!p.copies.empty() || !dbp.empty() || !lz4.empty()) p.bytes = end;
   return p;
 }
 
-cudaError_t stage_dbp(fgpu_ctx* ctx, const DbpStage& p, uint8_t* stage, uint64_t* copied) {
-  std::vector<uint8_t> tab(p.pages.size() * sizeof(DbpPage) + p.mbs.size() * sizeof(DbpMini));
-  std::memcpy(tab.data(), p.pages.data(), p.pages.size() * sizeof(DbpPage));
-  std::memcpy(tab.data() + p.pages.size() * sizeof(DbpPage), p.mbs.data(), p.mbs.size() * sizeof(DbpMini));
-  cudaError_t e = h2d(ctx, stage + p.tab_off, tab.data(), tab.size());
-  *copied += tab.size();
-  for (const Span& sp : p.spans) {
-    if (e != cudaSuccess) break;
-    *copied += sp.len;
-    e = cudaMemcpyAsync(stage + sp.stage_off, sp.src, sp.len, cudaMemcpyHostToDevice, ctx->stream);
-  }
-  if (e == cudaSuccess)
-    e = launch_dbp_decode(stage, reinterpret_cast<const DbpPage*>(stage + p.tab_off), uint32_t(p.pages.size()),
-                          reinterpret_cast<const DbpMini*>(stage + p.tab_off + p.pages.size() * sizeof(DbpPage)),
-                          uint32_t(p.n_groups), stage + p.scratch_off, ctx->stream);
-  return e;
-}
-
-// LZ4_RAW PLAIN INT64 / DOUBLE pages: their blocks straight from the source file (neighbours a page header apart as one
-// transfer, each transfer followed by 16 pad bytes), then the job table, from `base` in the staging buffer.
-struct Lz4Stage {
-  std::vector<Span> spans;
-  std::vector<Lz4Job> jobs;
-  uint64_t tab_off = 0;
-  uint64_t end() const { return tab_off + jobs.size() * sizeof(Lz4Job); }
-};
-
-Lz4Stage plan_lz4(const ImageStaging& s, uint8_t* dev, uint64_t base) {
-  Lz4Stage p;
-  std::vector<Range> ranges;
-  for (const Lz4Page& z : s.lz4_pages) ranges.push_back({z.src, z.len});
-  p.spans = coalesce(ranges);
-  uint64_t off = base;
-  for (Span& sp : p.spans) {
-    sp.stage_off = off;
-    off += al16(sp.len) + 16;
-    for (size_t i = sp.first; i < sp.first + sp.n; i++) {
-      const Lz4Page& z = s.lz4_pages[i];
-      p.jobs.push_back(Lz4Job{dev + z.hole, sp.stage_off + uint64_t(z.src - sp.src), z.len, z.n * 8});
+// Copies a planned staging buffer's tables and transfers and launches the kernels that read them, in order:
+// k_gather_pages, the DELTA_BINARY_PACKED decode, k_lz4_pages.  copied: the bytes of every transfer and of the
+// DELTA_BINARY_PACKED and LZ4_RAW tables.
+cudaError_t stage_pages(fgpu_ctx* ctx, const StagePlan& p, const std::vector<Extent>& extents, uint8_t* dev, uint8_t* stage,
+                        uint64_t* copied) {
+  cudaError_t e = cudaSuccess;
+  auto send = [&](const std::vector<Span>& spans) {
+    for (const Span& sp : spans) {
+      if (e != cudaSuccess) return;
+      *copied += sp.len;
+      uint8_t* dst = sp.stage_off == kToImage ? dev + extents[sp.first].dst_off : stage + sp.stage_off;
+      e = cudaMemcpyAsync(dst, sp.src, sp.len, cudaMemcpyHostToDevice, ctx->stream);
     }
+  };
+  if (!p.copies.empty()) e = h2d(ctx, stage + p.copies_off, p.copies.data(), p.copies.size() * sizeof(PageCopy));
+  send(p.plain);
+  if (e == cudaSuccess && !p.copies.empty())
+    e = launch_gather_pages(stage, dev, reinterpret_cast<const PageCopy*>(stage + p.copies_off), uint32_t(p.copies.size()), ctx->stream);
+  if (e == cudaSuccess && !p.dbp_pages.empty()) {
+    const size_t pages = p.dbp_pages.size() * sizeof(DbpPage);
+    std::vector<uint8_t> tab(pages + p.dbp_mbs.size() * sizeof(DbpMini));
+    std::memcpy(tab.data(), p.dbp_pages.data(), pages);
+    std::memcpy(tab.data() + pages, p.dbp_mbs.data(), tab.size() - pages);
+    e = h2d(ctx, stage + p.dbp_tab_off, tab.data(), tab.size());
+    *copied += tab.size();
+    send(p.dbp);
+    if (e == cudaSuccess)
+      e = launch_dbp_decode(stage, reinterpret_cast<const DbpPage*>(stage + p.dbp_tab_off), uint32_t(p.dbp_pages.size()),
+                            reinterpret_cast<const DbpMini*>(stage + p.dbp_tab_off + pages), uint32_t(p.n_groups),
+                            stage + p.scratch_off, ctx->stream);
   }
-  p.tab_off = off;
-  return p;
-}
-
-cudaError_t stage_lz4(fgpu_ctx* ctx, const Lz4Stage& p, uint8_t* stage, uint64_t* copied) {
-  cudaError_t e = h2d(ctx, stage + p.tab_off, p.jobs.data(), p.jobs.size() * sizeof(Lz4Job));
-  *copied += p.jobs.size() * sizeof(Lz4Job);
-  for (const Span& sp : p.spans) {
-    if (e != cudaSuccess) break;
-    *copied += sp.len;
-    e = cudaMemcpyAsync(stage + sp.stage_off, sp.src, sp.len, cudaMemcpyHostToDevice, ctx->stream);
+  if (e == cudaSuccess && !p.lz4_jobs.empty()) {
+    e = h2d(ctx, stage + p.lz4_tab_off, p.lz4_jobs.data(), p.lz4_jobs.size() * sizeof(Lz4Job));
+    *copied += p.lz4_jobs.size() * sizeof(Lz4Job);
+    send(p.lz4);
+    if (e == cudaSuccess) e = launch_lz4_pages(stage, reinterpret_cast<const Lz4Job*>(stage + p.lz4_tab_off), uint32_t(p.lz4_jobs.size()), ctx->stream);
   }
-  if (e == cudaSuccess) e = launch_lz4_pages(stage, reinterpret_cast<const Lz4Job*>(stage + p.tab_off), uint32_t(p.jobs.size()), ctx->stream);
   return e;
 }
 
 // Uploads one built column of one part if it is not resident yet: the host-assembled meta region with one copy, the
-// PLAIN value regions, DELTA_BINARY_PACKED streams and LZ4_RAW value blocks straight from the source file (or from the
-// host-inflated pages of an LZ4_RAW chunk) through one staging allocation,
-// then the string pages' indices and the cursor seeds, all on the engine stream so that kernels queued behind need no
-// extra synchronisation.
+// pages' value bytes straight from the source file (or from the host-inflated pages of an LZ4_RAW chunk) through one
+// staging allocation, then the string pages' indices and the cursor seeds, all on the engine stream so that kernels
+// queued behind need no extra synchronisation.
 int32_t upload_column(fgpu_ctx* ctx, Part* part, const std::string& column, uint64_t* h2d_bytes) {
   ColumnImage& img = part->images[column];
   if (!img.error.empty()) return FGPU_OK;  // surfaces as an error only if a query projects the column
@@ -418,18 +400,11 @@ int32_t upload_column(fgpu_ctx* ctx, Part* part, const std::string& column, uint
   cudaError_t e = h2d(ctx, dev, s.meta.data(), s.meta.size());
   uint64_t copied = s.meta.size();
   {
-    const PlainStage plain = plan_plain(part, s.extents);
-    const DbpStage dbp = plan_dbp(part, s, d, al16(plain.end));
-    const uint64_t dbp_end = dbp.pages.empty() ? plain.end : dbp.end();
-    const Lz4Stage lz4 = plan_lz4(s, d, al16(dbp_end));
-    if (dbp.n_groups > 0xffffffffull) e = cudaErrorInvalidValue;  // (more than 2^37 values in one column of one part)
+    const StagePlan plan = plan_stage(part, s, d);
+    if (plan.n_groups > 0xffffffffull) e = cudaErrorInvalidValue;  // (more than 2^37 values in one column of one part)
     DevBuf stage;  // released in stream order when it goes out of scope
-    if ((!plain.copies.empty() || !dbp.pages.empty() || !lz4.jobs.empty()) && e == cudaSuccess)
-      e = stage.alloc(lz4.jobs.empty() ? dbp_end : lz4.end(), ctx->stream);
-    uint8_t* st = static_cast<uint8_t*>(stage.p);
-    if (e == cudaSuccess) e = stage_plain(ctx, plain, s.extents, d, st, &copied);
-    if (e == cudaSuccess && !dbp.pages.empty()) e = stage_dbp(ctx, dbp, st, &copied);
-    if (e == cudaSuccess && !lz4.jobs.empty()) e = stage_lz4(ctx, lz4, st, &copied);
+    if (plan.bytes && e == cudaSuccess) e = stage.alloc(plan.bytes, ctx->stream);
+    if (e == cudaSuccess) e = stage_pages(ctx, plan, s.extents, d, static_cast<uint8_t*>(stage.p), &copied);
   }
   if (e == cudaSuccess) e = launch_str_jobs(ctx, s.str_jobs, dev);
   if (e == cudaSuccess) e = launch_make_seeds(dev, img.seed_jobs_off, img.n_seed_jobs, img.max_seed_chunks, ctx->stream);

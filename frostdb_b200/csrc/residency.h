@@ -10,9 +10,9 @@
 
 namespace fgpu {
 
-// What making columns resident cost.  h2d_bytes counts the meta regions, the PLAIN and DELTA_BINARY_PACKED transfers
-// and the DELTA_BINARY_PACKED page tables; build_us is the host's page walk and string interning, enqueue_us the
-// host's time queueing the uploads.
+// What making columns resident cost.  h2d_bytes counts the meta regions, the transfers of PLAIN value regions,
+// DELTA_BINARY_PACKED streams and LZ4_RAW blocks, the DELTA_BINARY_PACKED page and miniblock tables and the LZ4_RAW job
+// tables; build_us is the host's page walk and string interning, enqueue_us the host's time queueing the uploads.
 struct UploadStats {
   uint64_t h2d_bytes = 0;
   double build_us = 0, enqueue_us = 0;

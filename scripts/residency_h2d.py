@@ -1,6 +1,6 @@
 """Bytes copied to the device by the first Execute over borrowed parts, and what that Execute returned, for every fixture
-family: the layouts of tests/plain_strings.py, tests/delta_strings.py, tests/delta_int64.py and tests/hybrid_pages.py
-(those it can read), an Arrow part, and bench_data parts.
+family: the layouts of tests/plain_strings.py, tests/delta_strings.py, tests/delta_int64.py, tests/lz4_pages.py (numeric
+and string) and tests/hybrid_pages.py (those it can read), an Arrow part, and bench_data parts.
 
 Each file is put with FGPU_PUT_BORROW_PINNED into a table of its own, so nothing goes to the device until a query needs
 it.  One filter-only Execute per table projects every column, so it makes the whole part resident; its filter keeps
@@ -33,6 +33,7 @@ from frostdb_b200.store import ColumnStore  # noqa: E402
 from tests import delta_int64 as di  # noqa: E402
 from tests import delta_strings as ds  # noqa: E402
 from tests import hybrid_pages as hp  # noqa: E402
+from tests import lz4_pages as lz  # noqa: E402
 from tests import plain_strings as ps  # noqa: E402
 
 
@@ -47,6 +48,8 @@ def families():
         "delta_strings": [(ps.schema(), ds.file_of(n, e)) for n, e in ds.CASES],
         "delta_int64": [(di.schema(di.columns(n), delta=True, nullable_value=di.LAYOUT_BY_NAME[n].nullable), di.file_of(n))
                         for n in di.NAMES],
+        "lz4_pages": [(lz.schema(n, lz4=True), lz.file_of(n)) for n in lz.NAMES] +
+                     [(lz.str_schema(), lz.str_file_of(n)) for n in lz.STR_NAMES],
         "hybrid_pages": [(hp.schema(), hp.file_of(l.name)) for l in hp.LAYOUTS if l.error is None],
         "arrow": [(ps.schema(), ps.record_of(n)) for n in ps.NAMES[:2]],
         "bench_data": [(bench_schema, b) for b in bench],

@@ -311,7 +311,7 @@ PYARROW_TAKES = {"offset_0", "output_shorter"}
 
 # ---- a page-level writer -----------------------------------------------------------------------------------------
 PT_INT64 = 2
-ENC_PLAIN, ENC_RLE, ENC_RLE_DICTIONARY = 0, 3, 8
+ENC_PLAIN, ENC_RLE, ENC_DBP, ENC_RLE_DICTIONARY = 0, 3, 5, 8
 PAGE_DATA, PAGE_DICT, PAGE_DATA_V2 = 0, 2, 3
 
 
@@ -329,11 +329,13 @@ def _page(kind: str, n: int, enc: int, raw: bytes, block: Optional[bytes], raw_l
     return h.done() + payload
 
 
-def assemble(pages, dictionary: Optional[List[int]] = None, codec: int = CODEC_LZ4_RAW, check: bool = True) -> bytes:
+def assemble(pages, dictionary: Optional[List[int]] = None, codec: int = CODEC_LZ4_RAW, check: bool = True,
+             encodings: Optional[List[int]] = None) -> bytes:
     """One row group: `value` (REQUIRED INT64, codec `codec`) from `pages`, a list of (kind, values, block or None[,
     stated inflated size]),
     behind a compressed dictionary page of `dictionary` when given (the pages then hold indices into it); `timestamp`
-    (REQUIRED INT64, uncompressed PLAIN) 0 .. n-1.  With `check`, pyarrow must read `value` as the pages' values."""
+    (REQUIRED INT64, uncompressed PLAIN) 0 .. n-1.  `encodings`: per page ENC_PLAIN or ENC_DBP (tests/delta_int64.py's
+    dbp64), PLAIN when not given.  With `check`, pyarrow must read `value` as the pages' values."""
     out = bytearray(b"PAR1")
     n = sum(len(p[1]) for p in pages)
     start = data_off = len(out)
@@ -343,18 +345,21 @@ def assemble(pages, dictionary: Optional[List[int]] = None, codec: int = CODEC_L
         out += _Struct().i32(1, PAGE_DICT).i32(2, len(d)).i32(3, len(blk)).struct(7, _Struct().i32(1, len(dictionary)).i32(2, ENC_PLAIN)).done() + blk
         data_off = len(out)
     expect = []
-    for kind, values, block, *raw_len in pages:
+    encodings = encodings or [ENC_PLAIN] * len(pages)
+    for (kind, values, block, *raw_len), value_enc in zip(pages, encodings):
         if dictionary is not None:
             idx = [dictionary.index(v) for v in values]
             w = max(1, max(idx).bit_length())
             raw, enc = bytes([w]) + encode_hybrid([bp(idx)], w), ENC_RLE_DICTIONARY
+        elif value_enc == ENC_DBP:
+            raw, enc = di.dbp64(values), ENC_DBP
         else:
             raw, enc = np.asarray(values, dtype="<i8").tobytes(), ENC_PLAIN
         pg = _page(kind, len(values), enc, raw, block, *raw_len)
         out += pg
         expect += [int(v) for v in values]
     v_size = len(out) - start
-    encs = sorted({ENC_PLAIN, ENC_RLE} | ({ENC_RLE_DICTIONARY} if dictionary is not None else set()))
+    encs = sorted({ENC_PLAIN, ENC_RLE} | set(encodings) | ({ENC_RLE_DICTIONARY} if dictionary is not None else set()))
     md = (_Struct().i32(1, PT_INT64).list(2, 5, [_zigzag(e) for e in encs]).list(3, 8, [_uleb(5) + b"value"]).i32(4, codec)
           .i64(5, n).i64(6, v_size).i64(7, v_size).i64(9, data_off))
     if dictionary is not None:
@@ -423,3 +428,16 @@ def corrupted_files():
 def codec_file(codec: int) -> bytes:
     """A chunk naming `codec` (its pages are LZ4_RAW, which does not matter: the codec is refused before any page)."""
     return assemble([("v1", list(range(10)), None)], codec=codec, check=False)
+
+
+@functools.lru_cache(maxsize=None)
+def mixed_fills():
+    """(file, expected `value`): every way a page's values reach the dense value array, interleaved in one LZ4_RAW chunk.
+    Its pages in order: a compressed PLAIN v1 page (the device inflates it), a DELTA_BINARY_PACKED v1 page (the host
+    inflates it, the device decodes it from that buffer), a v2 PLAIN page stored uncompressed (copied as it is), a
+    compressed PLAIN v2 page, and DELTA_BINARY_PACKED again."""
+    a, c, d = _i64(_lits(40, 300 * 8)), _i64(_lits(41, 250 * 8)), _i64(_lits(42, 333 * 8))
+    b = di._vals(43, 517)
+    e = list(range(-10**15, -10**15 + 7 * 700, 7))
+    pages = [("v1", a, None), ("v1", b, None), ("v2raw", c, None), ("v2", d, None), ("v1", e, None)]
+    return assemble(pages, encodings=[ENC_PLAIN, ENC_DBP, ENC_PLAIN, ENC_PLAIN, ENC_DBP]), a + b + c + d + e
