@@ -107,6 +107,39 @@ struct PinnedPool {
   }
 };
 
+// One block of a PinnedPool, owned: it goes back to its pool when its owner is destroyed, so no return path can
+// lose it.  A block that becomes Arrow buffers moves into keep(), which a column holds as its ext_keep.
+class PinnedBlock {
+ public:
+  PinnedBlock() = default;
+  PinnedBlock(const std::shared_ptr<PinnedPool>& pool, size_t bytes) : pool_(pool) { p_ = pool->take(bytes, &cap_); }  // empty when out of memory
+  PinnedBlock(PinnedBlock&& o) noexcept : pool_(std::move(o.pool_)), p_(o.p_), cap_(o.cap_) { o.p_ = nullptr; }
+  PinnedBlock& operator=(PinnedBlock&& o) noexcept {  // returns the block it held, takes o's
+    if (this != &o) {
+      reset();
+      pool_ = std::move(o.pool_);
+      p_ = o.p_;
+      cap_ = o.cap_;
+      o.p_ = nullptr;
+    }
+    return *this;
+  }
+  ~PinnedBlock() { reset(); }
+  uint8_t* get() const { return p_; }
+  explicit operator bool() const { return p_ != nullptr; }
+  // The block, shared: it returns to the pool when the last holder lets go (the consumer released every array).
+  std::shared_ptr<void> keep() && { return std::make_shared<PinnedBlock>(std::move(*this)); }
+
+ private:
+  void reset() {
+    if (p_) pool_->give(p_, cap_);
+    p_ = nullptr;
+  }
+  std::shared_ptr<PinnedPool> pool_;
+  uint8_t* p_ = nullptr;
+  size_t cap_ = 0;
+};
+
 constexpr size_t kCommDataOff = 4096;  // flags live in front of the slots
 
 // Mailbox communicator of one rank (see comm.cu).
@@ -154,9 +187,7 @@ struct fgpu_ctx {
     arena_used = off + n;
     return arena + off;
   }
-  std::shared_ptr<fgpu::PinnedPool> pinned = std::make_shared<fgpu::PinnedPool>();
-  uint8_t* pinned_take(size_t bytes, size_t* cap) { return pinned->take(bytes, cap); }
-  void pinned_give(uint8_t* p, size_t cap) { pinned->give(p, cap); }
+  std::shared_ptr<fgpu::PinnedPool> pinned = std::make_shared<fgpu::PinnedPool>();  // blocks are taken as PinnedBlock
   // page-locked scratch for the per-query descriptor upload and the counters read-back (guarded by mu)
   uint8_t* scratch = nullptr;
   size_t scratch_bytes = 0;

@@ -30,6 +30,7 @@
 #include "kernels.h"
 #include "part_store.h"
 #include "residency.h"
+#include "result.h"
 
 using namespace fgpu;
 
@@ -210,14 +211,6 @@ struct fgpu_query {
   std::shared_ptr<QueryPlan> plan;
 };
 
-struct KeyOut {
-  std::string name;
-  bool is_int64 = false;
-  bool is_float = false;
-  const GlobalDict* dict = nullptr;
-  std::vector<std::string> dict_snapshot;  // values by id at execute time
-};
-
 struct fgpu_result {
   fgpu_ctx* ctx = nullptr;
   fgpu_stats stats{};
@@ -230,14 +223,20 @@ struct fgpu_result {
   unsigned int* cnt_ptr = nullptr;  // group counter inside `aux` when the scan counted the result rows
   bool groups_known = false;  // the scan's own stream already counted the result rows
   unsigned int n_groups = 0;
-  std::vector<KeyOut> keys;
-  std::vector<std::string> agg_names;
-  std::vector<uint8_t> agg_is_float;
+  ResultShape shape;
   // finished records
   std::vector<std::vector<OwnedColumn>> records;
   std::vector<int64_t> record_rows;
   size_t next = 0;
   bool finalized = false;
+  // The finished result: an empty one has no record (finishAggregate, aggregate.go:547-549; filter.go:264-266).
+  void finish(std::vector<OwnedColumn>&& cols, size_t rows) {
+    if (rows > 0) {
+      records.push_back(std::move(cols));
+      record_rows.push_back(int64_t(rows));
+    }
+    finalized = true;
+  }
   bool rows_plan = false;
   bool rows_no_nulls = false;  // rows plan produced by the take kernels: no projected value is NULL
   // collective Execute between its two halves: the partial table is pushed, the merge is still to come
@@ -390,22 +389,14 @@ struct ExecCache {
   DenseOut dout{};
   size_t out_bytes = 0;
   std::vector<std::unique_ptr<OwnedColumn>> dict_template;  // per key: the whole dictionary, ready to copy (small dictionaries)
-  fgpu_ctx* ctx = nullptr;
-  uint8_t* pinned = nullptr;      // host image of the compacted result (from the context's page-locked pool)
-  size_t pinned_cap = 0;
+  PinnedBlock pinned;             // host image of the compacted result (from the context's page-locked pool)
   size_t table_bytes = 0;
   bool ready = false;
   QueryDesc qd{};
   const QueryDesc* qdesc_dev = nullptr;
   ScanLaunch launch;
   fgpu_stats stats{};             // everything about the scan that does not change between Executes
-  std::vector<KeyOut> keys;       // with the dictionary snapshots
-  std::vector<std::string> agg_names;
-  std::vector<uint8_t> agg_is_float;
-  std::shared_ptr<PinnedPool> pool;
-  ~ExecCache() {
-    if (pinned && pool) pool->give(pinned, pinned_cap);
-  }
+  ResultShape shape;
 };
 
 struct Compiled {
@@ -1275,7 +1266,7 @@ void bind_finalize(FinalizeDesc* fd, const QueryDesc& qd) {  // the table bind_t
   fd->t_keys = qd.t_keys;
 }
 
-int32_t finalize_dense_host(fgpu_ctx* ctx, fgpu_result* res, ExecCache& x);
+int32_t finalize_dense_host(fgpu_result* res, ExecCache& x);
 
 // FROSTGPU_COMM_TIMEOUT_MS: how long a collective Execute waits for its peers (default 10 s).  It changes no plan, so
 // it is not one of the Switches.
@@ -1377,12 +1368,12 @@ cudaError_t launch_count_groups(FinalizeDesc fd, unsigned int* out, cudaStream_t
 int32_t cached_tail(fgpu_ctx* ctx, ExecCache& x) {
   cudaStream_t s = ctx->stream;
   if (!x.pinned) {
-    x.pinned = ctx->pinned_take(x.out_bytes, &x.pinned_cap);
+    x.pinned = PinnedBlock(ctx->pinned, x.out_bytes);
     if (!x.pinned) return fail(FGPU_ERR_OOM, "page-locked memory for the result image");
   }
   // k_finalize_dense writes the block over PCIe itself: 22 us of kernel time for 400 KB against 4 + 9 for kernel + copy
   // engine, but the Execute is 8 us shorter end to end without the copy operation behind the kernel (measured)
-  x.dout.out = x.pinned;
+  x.dout.out = x.pinned.get();
   CUDA_TRY(launch_finalize_dense(x.dout, s));
   return FGPU_OK;
 }
@@ -1420,6 +1411,25 @@ int32_t launch_aggregate_scan(fgpu_ctx* ctx, const QueryDesc& qd, const QueryDes
   return FGPU_OK;
 }
 
+// End of an Execute's scan launches: one synchronisation, the staging of this Execute's uploads released behind it,
+// then the scan kernels' time (ev[1] to ev[2]) and, with `total`, the device time of the whole Execute (ev[0] to ev[3],
+// which is recorded here behind the last launch).
+int32_t finish_scan(fgpu_ctx* ctx, PhaseClock& pc, fgpu_stats& st, bool total) {
+  if (total) CUDA_TRY(cudaEventRecord(ctx->ev[3], ctx->stream));
+  pc.mark("launch");
+  CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+  pc.mark("sync");
+  release_staging(ctx);
+  float ms = 0;
+  CUDA_TRY(cudaEventElapsedTime(&ms, ctx->ev[1], ctx->ev[2]));
+  st.scan_kernel_ms = ms;
+  if (total) {
+    CUDA_TRY(cudaEventElapsedTime(&ms, ctx->ev[0], ctx->ev[3]));
+    st.total_device_ms = ms;
+  }
+  return FGPU_OK;
+}
+
 // Re-issues the launches of a cached plan (see ExecCache): table init, scans, one copy back, one synchronisation.
 // collective: 0 no exchange, 1 push + wait + merge in one go, 2 push only (fgpu_query_execute_collective_begin)
 int32_t run_cached(fgpu_ctx* ctx, ExecCache& x, fgpu_result* res, int collective) {
@@ -1445,20 +1455,12 @@ int32_t run_cached(fgpu_ctx* ctx, ExecCache& x, fgpu_result* res, int collective
   } else if (int32_t rc = cached_tail(ctx, x)) {
     return rc;
   }
-  CUDA_TRY(cudaEventRecord(ctx->ev[3], s));
-  pc.mark("launch");
-  CUDA_TRY(cudaStreamSynchronize(s));
-  pc.mark("sync");
-  float ms = 0;
-  CUDA_TRY(cudaEventElapsedTime(&ms, ctx->ev[1], ctx->ev[2]));
-  st.scan_kernel_ms = ms;
-  CUDA_TRY(cudaEventElapsedTime(&ms, ctx->ev[0], ctx->ev[3]));
-  st.total_device_ms = ms;
-  const unsigned long long* counters = reinterpret_cast<const unsigned long long*>(x.pinned + 32);
+  if (int32_t rc = finish_scan(ctx, pc, st, /*total=*/true)) return rc;
+  const unsigned long long* counters = reinterpret_cast<const unsigned long long*>(x.pinned.get() + 32);
   st.rows_selected = counters[0];
   st.d2h_bytes += x.out_bytes;
   if (int32_t rc = comm_check(counters[3])) return rc;
-  const int32_t rc = finalize_dense_host(ctx, res, x);
+  const int32_t rc = finalize_dense_host(res, x);
   pc.mark("export");
   return rc;
 }
@@ -2140,11 +2142,11 @@ struct HostImage {
   }
 };
 
-// The result's columns: the keys with their dictionaries snapshotted now (the plan may be reused while they grow),
-// then the aggregates' names and types.
-void result_shape(const QueryPlan& q, const Compiled& c, std::vector<KeyOut>* keys, std::vector<std::string>* agg_names, std::vector<uint8_t>* agg_is_float) {
-  *keys = c.keys;
-  for (KeyOut& k : *keys) {
+// The result's columns (see ResultShape), with the key dictionaries snapshotted now.
+ResultShape result_shape(const QueryPlan& q, const Compiled& c) {
+  ResultShape r;
+  r.keys = c.keys;
+  for (KeyOut& k : r.keys) {
     if (k.dict) {
       const uint32_t card = k.dict->cardinality();
       k.dict_snapshot.reserve(card);
@@ -2153,24 +2155,11 @@ void result_shape(const QueryPlan& q, const Compiled& c, std::vector<KeyOut>* ke
     }
   }
   for (size_t a = 0; a < q.aggs.size(); a++) {
-    agg_names->push_back(std::string(agg_string(q.aggs[a].func)) + "(" + q.expr_name(q.aggs[a].expr) + ")");
+    r.agg_names.push_back(std::string(agg_string(q.aggs[a].func)) + "(" + q.expr_name(q.aggs[a].expr) + ")");
     // Count yields int64; Sum/Min/Max keep the input type (aggregate.go:734-950)
-    agg_is_float->push_back(c.qd.aggs[a].func != FGPU_AGG_COUNT && c.qd.aggs[a].is_float);
+    r.agg_is_float.push_back(c.qd.aggs[a].func != FGPU_AGG_COUNT && c.qd.aggs[a].is_float);
   }
-}
-
-// A utf8 dictionary column of the entries `ids` of `values` (all of them when null), in that order.
-std::unique_ptr<OwnedColumn> dict_column(const std::vector<std::string>& values, const std::vector<uint32_t>* ids) {
-  auto d = std::make_unique<OwnedColumn>();
-  d->format = "z";
-  d->length = int64_t(ids ? ids->size() : values.size());
-  d->offsets.push_back(0);
-  for (size_t i = 0; i < size_t(d->length); i++) {
-    const std::string& v = values[ids ? (*ids)[i] : i];
-    d->data.insert(d->data.end(), v.begin(), v.end());
-    d->offsets.push_back(int32_t(d->data.size()));
-  }
-  return d;
+  return r;
 }
 
 // First Execute of a cached plan: the plan keeps the device state; the dense table comes back compacted by
@@ -2205,31 +2194,21 @@ int32_t keep_exec_cache(fgpu_ctx* ctx, const QueryPlan& q, Compiled& c, const Qu
   CUDA_TRY(cudaMemsetAsync(x.out.p, 0, 256, s));
   f.hdr = static_cast<uint32_t*>(x.out.p);
   f.out = nullptr;  // a page-locked block per Execute (cached_tail)
-  x.pool = ctx->pinned;
-  x.pinned = ctx->pinned_take(x.out_bytes, &x.pinned_cap);
+  x.pinned = PinnedBlock(ctx->pinned, x.out_bytes);
   if (!x.pinned) return fail(FGPU_ERR_OOM, "page-locked memory for the result image");
   if (!res->pending) {
     if (int32_t rc = cached_tail(ctx, x)) return rc;
   } else {
-    CUDA_TRY(cudaMemcpyAsync(x.pinned + 32, qd.counters, 32, cudaMemcpyDeviceToHost, s));  // (rows selected by this rank's scan)
+    CUDA_TRY(cudaMemcpyAsync(x.pinned.get() + 32, qd.counters, 32, cudaMemcpyDeviceToHost, s));  // (rows selected by this rank's scan)
   }
-  CUDA_TRY(cudaEventRecord(ctx->ev[3], s));
-  pc.mark("launch");
-  CUDA_TRY(cudaStreamSynchronize(s));  // the host image stays valid until here
-  pc.mark("sync");
-  release_staging(ctx);
+  if (int32_t rc = finish_scan(ctx, pc, st, /*total=*/true)) return rc;  // the host image stays valid until here
   st.h2d_bytes += c.h2d_bytes;
-  float ms = 0;
-  CUDA_TRY(cudaEventElapsedTime(&ms, ctx->ev[1], ctx->ev[2]));
-  st.scan_kernel_ms = ms;
-  CUDA_TRY(cudaEventElapsedTime(&ms, ctx->ev[0], ctx->ev[3]));
-  st.total_device_ms = ms;
-  const unsigned long long* cnts = reinterpret_cast<const unsigned long long*>(x.pinned + 32);
+  const unsigned long long* cnts = reinterpret_cast<const unsigned long long*>(x.pinned.get() + 32);
   st.rows_selected = cnts[0];
   pb.account(st);
   x.qd = qd;
-  result_shape(q, c, &x.keys, &x.agg_names, &x.agg_is_float);
-  for (const KeyOut& k : x.keys) {  // small dictionaries are exported whole: the host then only copies index columns
+  x.shape = result_shape(q, c);
+  for (const KeyOut& k : x.shape.keys) {  // small dictionaries are exported whole: the host then only copies index columns
     x.dict_template.push_back(k.dict_snapshot.size() <= 4096 ? dict_column(k.dict_snapshot, nullptr) : nullptr);
   }
   st.kernel_launches++;  // k_finalize_dense (cached_tail)
@@ -2247,7 +2226,7 @@ int32_t keep_exec_cache(fgpu_ctx* ctx, const QueryPlan& q, Compiled& c, const Qu
     res->pending_cached = &x;
     return FGPU_OK;
   }
-  return finalize_dense_host(ctx, res, x);
+  return finalize_dense_host(res, x);
 }
 
 // Rows plan: one output array per projected column (worst case every row is selected) + look-back state per tile.
@@ -2536,14 +2515,8 @@ int32_t run_scan(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, fgpu_result* re
     res->groups_known = true;
   }
   CUDA_TRY(cudaMemcpyAsync(counters, qd.counters, 64 + 16, cudaMemcpyDeviceToHost, s));
-  pc.mark("launch");
-  CUDA_TRY(cudaStreamSynchronize(s));  // the host image / counters stay valid until here
-  pc.mark("sync");
-  release_staging(ctx);
+  if (int32_t rc = finish_scan(ctx, pc, st, /*total=*/false)) return rc;  // the host image / counters stay valid until here
   st.h2d_bytes += c.h2d_bytes;
-  float ms = 0;
-  CUDA_TRY(cudaEventElapsedTime(&ms, ctx->ev[1], ctx->ev[2]));
-  st.scan_kernel_ms = ms;
   st.rows_selected = counters[0];
   pb.account(st);
   if (res->groups_known) res->n_groups = static_cast<unsigned int>(counters[8] & 0xffffffffull);
@@ -2554,7 +2527,7 @@ int32_t run_scan(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, fgpu_result* re
   // keep what finalize / merge need
   res->qd = qd;
   res->rows_plan = rows_plan;
-  result_shape(q, c, &res->keys, &res->agg_names, &res->agg_is_float);
+  res->shape = result_shape(q, c);
   pc.mark("keep");
   pc.flush("scan");
   return FGPU_OK;
@@ -2562,78 +2535,41 @@ int32_t run_scan(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, fgpu_result* re
 
 // Compacted result image in page-locked memory -> one Arrow record (finishAggregate, aggregate.go:543-633): the
 // device already produced dictionary indices and aggregate values per result row (k_finalize_dense); the host copies.
-int32_t finalize_dense_host(fgpu_ctx* ctx, fgpu_result* res, ExecCache& x) {
-  (void)ctx;
+int32_t finalize_dense_host(fgpu_result* res, ExecCache& x) {
   PhaseClock pc;
   const QueryDesc& qd = x.qd;
-  const uint32_t* hdr = reinterpret_cast<const uint32_t*>(x.pinned);
+  uint8_t* img = x.pinned.get();
+  const uint32_t* hdr = reinterpret_cast<const uint32_t*>(img);
   const size_t G = std::min<size_t>(hdr[0], x.dout.max_out);
   res->stats.groups = G;
   const int nk = qd.n_keys, na = qd.n_aggs;
   const size_t key_bytes = (size_t(x.dout.max_out) * 4 + 7) & ~size_t(7);
   std::vector<OwnedColumn> cols;
   cols.reserve(size_t(nk + na));
-  // the columns of the record are slices of the page-locked block the kernel wrote; it goes back to the pool when the
-  // consumer has released every array
+  // the columns of the record are slices of the page-locked block the kernel wrote: the record takes the block (the next
+  // Execute takes another one), and it goes back to the pool when the consumer has released every array
   std::shared_ptr<void> keep;
-  if (G > 0) {
-    std::shared_ptr<PinnedPool> pool = x.pool;
-    uint8_t* blk = x.pinned;
-    const size_t cap = x.pinned_cap;
-    keep = std::shared_ptr<void>(blk, [pool, blk, cap](void*) { pool->give(blk, cap); });
-  }
+  if (G > 0) keep = std::move(x.pinned).keep();
   for (int k = 0; k < nk; k++) {
-    const KeyOut& ko = x.keys[size_t(k)];
-    uint32_t* idx = reinterpret_cast<uint32_t*>(x.pinned + 256 + size_t(k) * key_bytes);
+    const KeyOut& ko = x.shape.keys[size_t(k)];
+    uint32_t* idx = reinterpret_cast<uint32_t*>(img + 256 + size_t(k) * key_bytes);
     OwnedColumn col;
     col.name = ko.name;
     col.length = int64_t(G);
-    col.format = "I";  // dictionary<uint32, binary>
     if (G > 0) {
       col.ext = reinterpret_cast<const uint8_t*>(idx);
       col.ext_keep = keep;
     }
-    if (hdr[16 + k]) {  // NULL keys: validity bitmap, index 0 in the NULL slots
-      col.validity.assign((G + 7) / 8, 0);
-      for (size_t i = 0; i < G; i++) {
-        if (idx[i] == 0xffffffffu) {
-          idx[i] = 0;
-          col.null_count++;
-        } else {
-          set_bit(col.validity, int64_t(i));
-        }
-      }
-    }
-    std::unique_ptr<OwnedColumn> dict;
-    if (const OwnedColumn* t = x.dict_template[size_t(k)].get()) {
-      dict = std::make_unique<OwnedColumn>();
-      dict->format = t->format;
-      dict->length = t->length;
-      dict->data = t->data;
-      dict->offsets = t->offsets;
-    } else {  // large dictionary: only the values this result uses
-      std::vector<uint32_t> remap(ko.dict_snapshot.size(), 0xffffffffu), used;
-      const std::vector<uint8_t>& val = col.validity;
-      auto is_valid = [&](size_t i) { return val.empty() || ((val[i >> 3] >> (i & 7)) & 1); };
-      for (size_t i = 0; i < G; i++)
-        if (is_valid(i)) remap[idx[i]] = 0;
-      for (size_t g = 0; g < remap.size(); g++)
-        if (remap[g] == 0) {
-          remap[g] = uint32_t(used.size());
-          used.push_back(uint32_t(g));
-        }
-      for (size_t i = 0; i < G; i++)
-        if (is_valid(i)) idx[i] = remap[idx[i]];
-      dict = dict_column(ko.dict_snapshot, &used);
-    }
-    col.dictionary = std::move(dict);
+    // ids re-indexed in place; hdr[16 + k]: the kernel wrote a NULL key
+    const OwnedColumn* whole = x.dict_template[size_t(k)].get();
+    dict_key_column(col, idx, G, idx, ko.dict_snapshot, whole ? KeyDict::kWhole : KeyDict::kUsed, whole, hdr[16 + k] != 0);
     cols.push_back(std::move(col));
   }
-  const uint8_t* aggs = x.pinned + 256 + size_t(nk) * key_bytes;
+  const uint8_t* aggs = img + 256 + size_t(nk) * key_bytes;
   for (int a = 0; a < na; a++) {
     OwnedColumn col;
-    col.name = x.agg_names[size_t(a)];
-    col.format = x.agg_is_float[size_t(a)] ? "g" : "l";
+    col.name = x.shape.agg_names[size_t(a)];
+    col.format = x.shape.agg_is_float[size_t(a)] ? "g" : "l";
     col.length = int64_t(G);
     if (G > 0) {
       col.ext = aggs + size_t(a) * x.dout.max_out * 8;
@@ -2642,13 +2578,7 @@ int32_t finalize_dense_host(fgpu_ctx* ctx, fgpu_result* res, ExecCache& x) {
     cols.push_back(std::move(col));
   }
   res->stats.algorithmic_bytes += (size_t(nk) + size_t(na)) * G * 8;
-  if (G > 0) {  // finishAggregate skips empty aggregates (aggregate.go:547-549)
-    res->records.push_back(std::move(cols));
-    res->record_rows.push_back(int64_t(G));
-    x.pinned = nullptr;  // the block now belongs to the record; the next Execute takes another one
-    x.pinned_cap = 0;
-  }
-  res->finalized = true;
+  res->finish(std::move(cols), G);
   pc.mark("arrow");
   pc.flush("finalize-host");
   return FGPU_OK;
@@ -2664,21 +2594,18 @@ int32_t finalize_rows(fgpu_ctx* ctx, fgpu_result* res) {
   // Every projected column comes back into a page-locked block of the context's pool with ONE copy each and ONE
   // synchronisation for all of them; the block itself becomes the Arrow buffer (it returns to the pool when the
   // consumer releases the array), so a large selection costs its PCIe transfer and nothing else.
-  struct Block { uint8_t* p = nullptr; size_t cap = 0; };
-  std::shared_ptr<PinnedPool> pool = ctx->pinned;
-  auto keep_of = [pool](Block b) { return std::shared_ptr<void>(b.p, [pool, b](void*) { pool->give(b.p, b.cap); }); };
-  std::vector<Block> data(size_t(qd.n_out)), valid(size_t(qd.n_out));
+  std::vector<PinnedBlock> data(size_t(qd.n_out)), valid(size_t(qd.n_out));
   for (int o = 0; o < qd.n_out && R; o++) {
-    const bool dict = !res->keys[size_t(o)].is_int64;
+    const bool dict = !res->shape.keys[size_t(o)].is_int64;
     const size_t bytes = R * (dict ? 4 : 8);
-    data[size_t(o)].p = pool->take(bytes, &data[size_t(o)].cap);
-    if (!data[size_t(o)].p) return fail(FGPU_ERR_OOM, "page-locked memory for the result rows");
-    CUDA_TRY(cudaMemcpyAsync(data[size_t(o)].p, qd.out_data[o], bytes, cudaMemcpyDeviceToHost, s));
+    data[size_t(o)] = PinnedBlock(ctx->pinned, bytes);
+    if (!data[size_t(o)]) return fail(FGPU_ERR_OOM, "page-locked memory for the result rows");
+    CUDA_TRY(cudaMemcpyAsync(data[size_t(o)].get(), qd.out_data[o], bytes, cudaMemcpyDeviceToHost, s));
     res->stats.d2h_bytes += bytes;
     if (!dict && !res->rows_no_nulls) {
-      valid[size_t(o)].p = pool->take(R, &valid[size_t(o)].cap);
-      if (!valid[size_t(o)].p) return fail(FGPU_ERR_OOM, "page-locked memory for the result rows");
-      CUDA_TRY(cudaMemcpyAsync(valid[size_t(o)].p, qd.out_valid[o], R, cudaMemcpyDeviceToHost, s));
+      valid[size_t(o)] = PinnedBlock(ctx->pinned, R);
+      if (!valid[size_t(o)]) return fail(FGPU_ERR_OOM, "page-locked memory for the result rows");
+      CUDA_TRY(cudaMemcpyAsync(valid[size_t(o)].get(), qd.out_valid[o], R, cudaMemcpyDeviceToHost, s));
       res->stats.d2h_bytes += R;
     }
   }
@@ -2689,60 +2616,25 @@ int32_t finalize_rows(fgpu_ctx* ctx, fgpu_result* res) {
   res->stats.total_device_ms = ms;
   std::vector<OwnedColumn> cols;
   for (int o = 0; o < qd.n_out; o++) {
-    const KeyOut& ko = res->keys[size_t(o)];
+    const KeyOut& ko = res->shape.keys[size_t(o)];
+    uint8_t* p = data[size_t(o)].get();
     OwnedColumn col;
     col.name = ko.name;
     col.length = int64_t(R);
-    if (R) {
-      col.ext = data[size_t(o)].p;
-      col.ext_keep = keep_of(data[size_t(o)]);
-    }
-    if (!ko.is_int64) {
-      // dictionary ids (-1 = NULL): indices into a dictionary of the values this result uses
-      col.format = "I";
-      int32_t* ids = reinterpret_cast<int32_t*>(data[size_t(o)].p);
-      uint32_t* idx = reinterpret_cast<uint32_t*>(data[size_t(o)].p);
-      std::vector<int32_t> remap(ko.dict_snapshot.size(), -1);
-      bool any_null = false;
-      for (size_t i = 0; i < R; i++) {
-        if (ids[i] >= 0) remap[size_t(ids[i])] = 0;
-        else any_null = true;
-      }
-      std::vector<uint32_t> used;
-      for (size_t g = 0; g < remap.size(); g++)
-        if (remap[g] >= 0) {
-          remap[g] = int32_t(used.size());
-          used.push_back(uint32_t(g));
-        }
-      if (any_null) col.validity.assign((R + 7) / 8, 0);
-      for (size_t i = 0; i < R; i++) {
-        if (ids[i] < 0) { idx[i] = 0; col.null_count++; }
-        else { idx[i] = uint32_t(remap[size_t(ids[i])]); if (any_null) set_bit(col.validity, int64_t(i)); }
-      }
-      col.dictionary = dict_column(ko.dict_snapshot, &used);
+    if (!ko.is_int64) {  // dictionary ids (-1 = NULL), re-indexed in place
+      dict_key_column(col, reinterpret_cast<const int32_t*>(p), R, reinterpret_cast<uint32_t*>(p), ko.dict_snapshot, KeyDict::kUsed);
     } else {
       col.format = ko.is_float ? "g" : "l";
-      if (valid[size_t(o)].p) {
-        const uint8_t* v = valid[size_t(o)].p;
-        size_t nulls = 0;
-        for (size_t i = 0; i < R; i++) nulls += v[i] ? 0 : 1;
-        if (nulls) {
-          col.validity.assign((R + 7) / 8, 0);
-          for (size_t i = 0; i < R; i++)
-            if (v[i]) set_bit(col.validity, int64_t(i));
-          col.null_count = int64_t(nulls);
-        }
-        pool->give(valid[size_t(o)].p, valid[size_t(o)].cap);
-      }
+      if (valid[size_t(o)]) validity_from_bytes(col, valid[size_t(o)].get(), R);
+    }
+    if (R) {
+      col.ext = p;
+      col.ext_keep = std::move(data[size_t(o)]).keep();
     }
     res->stats.algorithmic_bytes += R * (ko.is_int64 ? 8 : 4);
     cols.push_back(std::move(col));
   }
-  if (R > 0) {  // an empty selection emits no record (filter.go:264-266)
-    res->records.push_back(std::move(cols));
-    res->record_rows.push_back(int64_t(R));
-  }
-  res->finalized = true;
+  res->finish(std::move(cols), R);
   res->table.reset();
   res->aux.reset();
   return FGPU_OK;
@@ -2771,10 +2663,7 @@ int32_t finalize_result(fgpu_ctx* ctx, fgpu_result* res) {
   const int nk = fd.n_keys, na = fd.n_aggs;
   // every result column lands in its own page-locked block of the context's pool; int64 keys and aggregates hand
   // that block to the Arrow consumer as it is (returned to the pool on release), dictionary keys are re-indexed
-  struct Block { uint8_t* p = nullptr; size_t cap = 0; };
-  std::shared_ptr<PinnedPool> pool = ctx->pinned;
-  auto keep_of = [pool](Block b) { return std::shared_ptr<void>(b.p, [pool, b](void*) { pool->give(b.p, b.cap); }); };
-  std::vector<Block> blocks(size_t(nk + na));
+  std::vector<PinnedBlock> blocks(size_t(nk + na));
   if (G > 0) {
     DevBuf out;
     size_t bytes = (size_t(nk) + size_t(na) + 1) * G * 8;
@@ -2788,9 +2677,9 @@ int32_t finalize_result(fgpu_ctx* ctx, fgpu_result* res) {
     CUDA_TRY(launch_finalize(fd, s));
     res->stats.kernel_launches += 1;
     for (int c = 0; c < nk + na; c++) {
-      blocks[size_t(c)].p = pool->take(G * 8, &blocks[size_t(c)].cap);
-      if (!blocks[size_t(c)].p) return fail(FGPU_ERR_OOM, "page-locked memory for the result columns");
-      CUDA_TRY(cudaMemcpyAsync(blocks[size_t(c)].p, fd.out_keys + size_t(c) * G, G * 8, cudaMemcpyDeviceToHost, s));
+      blocks[size_t(c)] = PinnedBlock(ctx->pinned, G * 8);
+      if (!blocks[size_t(c)]) return fail(FGPU_ERR_OOM, "page-locked memory for the result columns");
+      CUDA_TRY(cudaMemcpyAsync(blocks[size_t(c)].get(), fd.out_keys + size_t(c) * G, G * 8, cudaMemcpyDeviceToHost, s));
     }
     CUDA_TRY(cudaStreamSynchronize(s));
     res->stats.d2h_bytes += (size_t(nk) + size_t(na)) * G * 8;
@@ -2804,65 +2693,25 @@ int32_t finalize_result(fgpu_ctx* ctx, fgpu_result* res) {
 
   // ---- build Arrow columns (aggregate.go:551-625: group columns first, then aggregates) --------
   std::vector<OwnedColumn> cols;
-  for (int k = 0; k < nk; k++) {
-    const KeyOut& ko = res->keys[size_t(k)];
+  for (int c = 0; c < nk + na; c++) {
+    const bool key = c < nk;
     OwnedColumn col;
-    col.name = ko.name;
+    col.name = key ? res->shape.keys[size_t(c)].name : res->shape.agg_names[size_t(c - nk)];
     col.length = int64_t(G);
-    const long long* codes = reinterpret_cast<const long long*>(blocks[size_t(k)].p);
-    if (ko.is_int64) {
-      col.format = "l";
-      if (G) {
-        col.ext = blocks[size_t(k)].p;
-        col.ext_keep = keep_of(blocks[size_t(k)]);
-      }
+    if (key && !res->shape.keys[size_t(c)].is_int64) {  // codes (id + 1, 0 = NULL) re-indexed into col.data
+      dict_key_column(col, reinterpret_cast<const long long*>(blocks[size_t(c)].get()), G, nullptr, res->shape.keys[size_t(c)].dict_snapshot,
+                      KeyDict::kUsed);
     } else {
-      // dictionary<uint32, binary> holding only the values this result uses
-      col.format = "I";
-      col.validity.assign((G + 7) / 8, 0);
-      col.data.resize(G * 4);
-      uint32_t* idx = reinterpret_cast<uint32_t*>(col.data.data());
-      // used dictionary ids in increasing order -> dense indices (O(groups + cardinality))
-      std::vector<uint32_t> remap(ko.dict_snapshot.size(), 0xffffffffu), used;
-      for (size_t i = 0; i < G; i++)
-        if (codes[i] != 0) remap[size_t(codes[i] - 1)] = 0;
-      for (size_t g = 0; g < remap.size(); g++)
-        if (remap[g] == 0) {
-          remap[g] = uint32_t(used.size());
-          used.push_back(uint32_t(g));
-        }
-      for (size_t i = 0; i < G; i++) {
-        if (codes[i] == 0) {
-          idx[i] = 0;
-          col.null_count++;
-        } else {
-          idx[i] = remap[size_t(codes[i] - 1)];
-          set_bit(col.validity, int64_t(i));
-        }
+      col.format = !key && res->shape.agg_is_float[size_t(c - nk)] ? "g" : "l";
+      if (G) {
+        col.ext = blocks[size_t(c)].get();
+        col.ext_keep = std::move(blocks[size_t(c)]).keep();
       }
-      if (col.null_count == 0) col.validity.clear();
-      col.dictionary = dict_column(ko.dict_snapshot, &used);
-      if (G) pool->give(blocks[size_t(k)].p, blocks[size_t(k)].cap);  // the codes are re-indexed into col.data
-    }
-    cols.push_back(std::move(col));
-  }
-  for (int a = 0; a < na; a++) {
-    OwnedColumn col;
-    col.name = res->agg_names[size_t(a)];
-    col.format = res->agg_is_float[size_t(a)] ? "g" : "l";
-    col.length = int64_t(G);
-    if (G) {
-      col.ext = blocks[size_t(nk + a)].p;
-      col.ext_keep = keep_of(blocks[size_t(nk + a)]);
     }
     cols.push_back(std::move(col));
   }
   res->stats.algorithmic_bytes += (size_t(nk) + size_t(na)) * G * 8;
-  if (G > 0) {  // finishAggregate skips empty aggregates (aggregate.go:547-549)
-    res->records.push_back(std::move(cols));
-    res->record_rows.push_back(int64_t(G));
-  }
-  res->finalized = true;
+  res->finish(std::move(cols), G);
   res->table.reset();
   res->aux.reset();
   res->cnt.reset();
@@ -2871,61 +2720,86 @@ int32_t finalize_result(fgpu_ctx* ctx, fgpu_result* res) {
   return FGPU_OK;
 }
 
+// One partial table to fold: a table of the result's layout at `slots` slots.
+struct Partial {
+  const void* table;
+  uint32_t slots;
+};
+
+// Folds partial tables into a fresh table of `slots` slots (k_table_init, then one k_merge per partial) and installs it
+// in the result: table, table_bytes, qd, fd.  zero_counters: whether the table init zeroes the query's counters.
+int32_t fold_partials(fgpu_ctx* ctx, fgpu_result* res, uint32_t slots, const std::vector<Partial>& parts, bool zero_counters) {
+  cudaStream_t s = ctx->stream;
+  QueryDesc qd = res->qd;
+  qd.table_slots = slots;
+  size_t off_aggs, off_tags, off_keys;
+  const size_t tbytes = table_layout(qd, &off_aggs, &off_tags, &off_keys);
+  DevBuf merged;
+  CUDA_TRY(merged.alloc(tbytes + 128, s));  // (slack for the 16-byte exchange copies)
+  bind_table(&qd, static_cast<uint8_t*>(merged.p));
+  CUDA_TRY(launch_table_init(qd, s, zero_counters));
+  for (const Partial& p : parts) CUDA_TRY(launch_merge(qd, p.table, p.slots, s));
+  std::swap(res->table.p, merged.p);
+  std::swap(res->table.n, merged.n);
+  res->table_bytes = tbytes;
+  res->qd = qd;
+  res->fd.table_slots = slots;
+  bind_finalize(&res->fd, qd);
+  return FGPU_OK;
+}
+
+// Behind a merge: counts the final table's groups (when the result counts them on the device), reads the counters back
+// into the context's scratch (to *counters when asked) and fails on a hash table overflow.
+int32_t count_merged(fgpu_ctx* ctx, fgpu_result* res, const unsigned long long** counters) {
+  cudaStream_t s = ctx->stream;
+  if (res->cnt_ptr) {
+    CUDA_TRY(cudaMemsetAsync(res->cnt_ptr, 0, 16, s));
+    CUDA_TRY(launch_count_groups(res->fd, res->cnt_ptr, s));
+    res->stats.kernel_launches++;
+  }
+  CUDA_TRY(ctx->ensure_scratch(128));
+  unsigned long long* c = reinterpret_cast<unsigned long long*>(ctx->scratch);
+  CUDA_TRY(cudaMemcpyAsync(c, res->qd.counters, 64 + 16, cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(cudaStreamSynchronize(s));
+  if (c[1]) return fail(FGPU_ERR_UNSUPPORTED, "aggregate hash table overflow while merging partials");
+  if (res->cnt_ptr) {
+    res->n_groups = static_cast<unsigned int>(c[8] & 0xffffffffull);
+    res->groups_known = true;
+  }
+  if (counters) *counters = c;
+  return FGPU_OK;
+}
 
 // Second half of a collective Execute: wait for the peers, merge, bring the final result to the host.
 int32_t collective_end(fgpu_ctx* ctx, fgpu_result* res) {
   if (!res->pending) return fail(FGPU_ERR_INVALID, "no collective Execute pending on this result");
   res->pending = false;
-  cudaStream_t s = ctx->stream;
   if (ExecCache* x = static_cast<ExecCache*>(res->pending_cached)) {
     if (int32_t rc = cached_merge_tail(ctx, *x, res->pending_seq, res->pending_bytes)) return rc;
-    CUDA_TRY(cudaStreamSynchronize(s));
-    const unsigned long long* counters = reinterpret_cast<const unsigned long long*>(x->pinned + 32);
+    CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    const unsigned long long* counters = reinterpret_cast<const unsigned long long*>(x->pinned.get() + 32);
     res->stats.d2h_bytes += x->out_bytes;
     if (int32_t rcc = comm_check(counters[3])) return rcc;
-    return finalize_dense_host(ctx, res, *x);
+    return finalize_dense_host(res, *x);
   }
-  QueryDesc& qd = res->qd;
+  const QueryDesc& qd = res->qd;
   int32_t rc = comm_wait_merge(ctx, qd, res->table.p, res->pending_seq, res->pending_bytes);
   if (rc) return rc;
-  FinalizeDesc& fd = res->fd;
   if (qd.table_mode != TM_DENSE) {  // hash tables: fold every rank's slot, at its own size, into a fresh table
     uint32_t src_slots[kMaxRanks];
     if (int32_t rcs = hash_partial_slots(ctx, qd, res->pending_seq, src_slots)) return rcs;
     uint64_t total = 0;
-    for (int r = 0; r < ctx->comm.n; r++) total += src_slots[r];
-    QueryDesc q2 = qd;
-    q2.table_slots = hash_slots(total);
-    size_t off_aggs, off_tags, off_keys;
-    const size_t tbytes = table_layout(q2, &off_aggs, &off_tags, &off_keys);
-    DevBuf merged;
-    CUDA_TRY(merged.alloc(tbytes + 128, s));
-    bind_table(&q2, static_cast<uint8_t*>(merged.p));
-    CUDA_TRY(launch_table_init(q2, s, /*zero_counters=*/false));
-    for (int r = 0; r < ctx->comm.n; r++)
-      CUDA_TRY(launch_merge(q2, ctx->comm.mailbox + ctx->comm.data_off(res->pending_seq & 1u, r), src_slots[r], s));
-    std::swap(res->table.p, merged.p);
-    std::swap(res->table.n, merged.n);
-    res->table_bytes = tbytes;
-    qd = q2;
-    fd.table_slots = qd.table_slots;
-    bind_finalize(&fd, qd);
+    std::vector<Partial> parts;
+    for (int r = 0; r < ctx->comm.n; r++) {
+      total += src_slots[r];
+      parts.push_back({ctx->comm.mailbox + ctx->comm.data_off(res->pending_seq & 1u, r), src_slots[r]});
+    }
+    // (counters[3] carries the exchange's error: the init leaves the counters alone)
+    if (int32_t rcf = fold_partials(ctx, res, hash_slots(total), parts, /*zero_counters=*/false)) return rcf;
   }
-  if (res->cnt_ptr) {  // count the groups of the final table behind the merge
-    CUDA_TRY(cudaMemsetAsync(res->cnt_ptr, 0, 16, s));
-    CUDA_TRY(launch_count_groups(fd, res->cnt_ptr, s));
-    res->stats.kernel_launches++;
-  }
-  CUDA_TRY(ctx->ensure_scratch(128));
-  unsigned long long* counters = reinterpret_cast<unsigned long long*>(ctx->scratch);
-  CUDA_TRY(cudaMemcpyAsync(counters, qd.counters, 64 + 16, cudaMemcpyDeviceToHost, s));
-  CUDA_TRY(cudaStreamSynchronize(s));
-  if (counters[1]) return fail(FGPU_ERR_UNSUPPORTED, "aggregate hash table overflow while merging partials");
+  const unsigned long long* counters = nullptr;
+  if (int32_t rcc = count_merged(ctx, res, &counters)) return rcc;
   if (int32_t rcc = comm_check(counters[3])) return rcc;
-  if (res->cnt_ptr) {
-    res->n_groups = static_cast<unsigned int>(counters[8] & 0xffffffffull);
-    res->groups_known = true;
-  }
   return finalize_result(ctx, res);
 }
 
@@ -3249,42 +3123,14 @@ int32_t fgpu_result_merge_partials(fgpu_ctx* ctx, fgpu_result* r, const void* ga
     if (nbytes != r->table_bytes) return fail(FGPU_ERR_INVALID, "partial table size differs between ranks (dictionaries not preloaded identically?)");
     // Start from an empty table and fold every rank's partial in, this rank's own included.  A hash table takes the
     // groups of n partials: it is sized for n times this rank's slots.
-    QueryDesc qd = r->qd;
-    const uint32_t src_slots = qd.table_slots;
-    if (qd.table_mode != TM_DENSE) qd.table_slots = hash_slots(uint64_t(n) * src_slots);
-    size_t off_aggs, off_tags, off_keys;
-    const size_t tbytes = table_layout(qd, &off_aggs, &off_tags, &off_keys);
-    DevBuf merged;
-    CUDA_TRY(merged.alloc(tbytes, ctx->stream));
-    bind_table(&qd, static_cast<uint8_t*>(merged.p));
-    CUDA_TRY(launch_table_init(qd, ctx->stream));
-    for (int32_t i = 0; i < n; i++) {
-      CUDA_TRY(launch_merge(qd, static_cast<const uint8_t*>(gathered) + size_t(i) * nbytes, src_slots, ctx->stream));
-      r->stats.kernel_launches++;
-    }
-    // the result now lives in the merged table; its groups are counted right behind the merges so that
-    // finalisation needs one host round trip less
-    FinalizeDesc& fd = r->fd;
-    fd.table_slots = qd.table_slots;
-    bind_finalize(&fd, qd);
-    if (r->cnt_ptr) {
-      CUDA_TRY(cudaMemsetAsync(r->cnt_ptr, 0, 16, ctx->stream));
-      CUDA_TRY(launch_count_groups(fd, r->cnt_ptr, ctx->stream));
-      r->stats.kernel_launches++;
-    }
-    CUDA_TRY(ctx->ensure_scratch(128));
-    unsigned long long* counters = reinterpret_cast<unsigned long long*>(ctx->scratch);
-    CUDA_TRY(cudaMemcpyAsync(counters, qd.counters, 64 + 16, cudaMemcpyDeviceToHost, ctx->stream));
-    CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-    if (counters[1]) return fail(FGPU_ERR_UNSUPPORTED, "aggregate hash table overflow while merging partials");
-    if (r->cnt_ptr) {
-      r->n_groups = static_cast<unsigned int>(counters[8] & 0xffffffffull);
-      r->groups_known = true;
-    }
-    std::swap(r->table.p, merged.p);
-    std::swap(r->table.n, merged.n);
-    r->table_bytes = tbytes;
-    r->qd = qd;
+    const uint32_t src_slots = r->qd.table_slots;
+    std::vector<Partial> parts;
+    for (int32_t i = 0; i < n; i++) parts.push_back({static_cast<const uint8_t*>(gathered) + size_t(i) * nbytes, src_slots});
+    const uint32_t slots = r->qd.table_mode == TM_DENSE ? src_slots : hash_slots(uint64_t(n) * src_slots);
+    if (int32_t rc = fold_partials(ctx, r, slots, parts, /*zero_counters=*/true)) return rc;
+    r->stats.kernel_launches += uint32_t(n);  // k_merge
+    // the groups are counted right behind the merges, so that finalisation needs one host round trip less
+    if (int32_t rc = count_merged(ctx, r, nullptr)) return rc;
   }
   return finalize_result(ctx, r);
   API_CATCH
@@ -3573,21 +3419,7 @@ int32_t fgpu_dict_export(fgpu_ctx* ctx, const char* table, const char* column, u
   if (it == ctx->tables.end()) return FGPU_OK;
   auto dit = it->second.dicts.find(column);
   if (dit == it->second.dicts.end()) return FGPU_OK;
-  const GlobalDict& d = dit->second;
-  uint64_t need = 0;
-  for (auto& v : d.values) need += 4 + v.size();
-  *out_len = need;
-  *out_count = uint32_t(d.values.size());
-  if (!buf) return FGPU_OK;
-  if (cap < need) return fail(FGPU_ERR_INVALID, "buffer too small");
-  uint8_t* p = buf;
-  for (auto& v : d.values) {
-    uint32_t l = uint32_t(v.size());
-    std::memcpy(p, &l, 4);
-    p += 4;
-    std::memcpy(p, v.data(), v.size());
-    p += v.size();
-  }
+  if (!write_dict_blob(dit->second.values, buf, cap, out_len, out_count)) return fail(FGPU_ERR_INVALID, "buffer too small");
   return FGPU_OK;
   API_CATCH
 }
@@ -3623,20 +3455,7 @@ int32_t fgpu_parquet_dict_values(const uint8_t* file, uint64_t len, const char* 
   if (!parse_parquet(file, len, &pf, &err)) return fail(FGPU_ERR_PARQUET, err);
   GlobalDict d;  // first-seen order over the file's row groups
   if (!column_dict_values(pf, column, &d, &err)) return fail(FGPU_ERR_PARQUET, err);
-  uint64_t need = 0;
-  for (auto& v : d.values) need += 4 + v.size();
-  *out_len = need;
-  *out_count = uint32_t(d.values.size());
-  if (!buf) return FGPU_OK;
-  if (cap < need) return fail(FGPU_ERR_INVALID, "buffer too small");
-  uint8_t* o = buf;
-  for (auto& v : d.values) {
-    uint32_t l = uint32_t(v.size());
-    std::memcpy(o, &l, 4);
-    o += 4;
-    std::memcpy(o, v.data(), v.size());
-    o += v.size();
-  }
+  if (!write_dict_blob(d.values, buf, cap, out_len, out_count)) return fail(FGPU_ERR_INVALID, "buffer too small");
   return FGPU_OK;
   API_CATCH
 }
@@ -3688,26 +3507,7 @@ int32_t fgpu_part_decode_column(fgpu_ctx* ctx, const char* table, uint64_t part_
     std::vector<int32_t> ids(total);
     CUDA_TRY(cudaMemcpyAsync(ids.data(), d_vals.p, total * 4, cudaMemcpyDeviceToHost, ctx->stream));
     CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-    const GlobalDict& gd = it->second.dicts.at(column);
-    col.format = "I";
-    col.validity.assign((total + 7) / 8, 0);
-    col.data.resize(total * 4);
-    uint32_t* idx = reinterpret_cast<uint32_t*>(col.data.data());
-    for (uint64_t i = 0; i < total; i++) {
-      if (ids[i] < 0) { idx[i] = 0; col.null_count++; }
-      else { idx[i] = uint32_t(ids[i]); set_bit(col.validity, int64_t(i)); }
-    }
-    if (col.null_count == 0) col.validity.clear();
-    auto dict = std::make_unique<OwnedColumn>();
-    dict->format = "z";
-    dict->length = int64_t(gd.cardinality());
-    dict->offsets.push_back(0);
-    for (uint32_t g = 0; g < gd.cardinality(); g++) {
-      const std::string& v = gd.value(g);
-      dict->data.insert(dict->data.end(), v.begin(), v.end());
-      dict->offsets.push_back(int32_t(dict->data.size()));
-    }
-    col.dictionary = std::move(dict);
+    dict_key_column(col, ids.data(), total, nullptr, it->second.dicts.at(column).values, KeyDict::kWhole);
   } else {
     col.format = phys == PT_DOUBLE ? "g" : "l";
     col.data.resize(total * 8);
@@ -3715,12 +3515,7 @@ int32_t fgpu_part_decode_column(fgpu_ctx* ctx, const char* table, uint64_t part_
     CUDA_TRY(cudaMemcpyAsync(col.data.data(), d_vals.p, total * 8, cudaMemcpyDeviceToHost, ctx->stream));
     CUDA_TRY(cudaMemcpyAsync(valid.data(), d_valid.p, total, cudaMemcpyDeviceToHost, ctx->stream));
     CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-    col.validity.assign((total + 7) / 8, 0);
-    for (uint64_t i = 0; i < total; i++) {
-      if (valid[i]) set_bit(col.validity, int64_t(i));
-      else col.null_count++;
-    }
-    if (col.null_count == 0) col.validity.clear();
+    validity_from_bytes(col, valid.data(), total);
   }
   release_staging(ctx);
   export_column(std::move(col), out_schema, out_array);

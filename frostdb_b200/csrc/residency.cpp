@@ -139,12 +139,11 @@ int32_t intern_plain_strings(fgpu_ctx* ctx, Table* table, const std::vector<std:
                  o_keys = o_first + al(ns * 4), o_pay = o_keys + ns * 8;
   CUDA_TRY(batch->scratch.alloc(o_pay + payload, ctx->stream));
   uint8_t* d = static_cast<uint8_t*>(batch->scratch.p);
-  size_t pin_cap = 0;
   // first occurrences (written by k_str_compact), counts, rebuilt regions (the distinct values written by k_str_gather)
   const uint64_t pin_rebuilt = al(nv * 4 + n * 4);
-  uint8_t* pin = ctx->pinned_take(size_t(pin_rebuilt + nr), &pin_cap);
-  if (!pin) return fail(FGPU_ERR_OOM, "PLAIN string interning: page-locked result buffer");
-  struct Give { fgpu_ctx* ctx; uint8_t* p; size_t cap; ~Give() { ctx->pinned_give(p, cap); } } give{ctx, pin, pin_cap};
+  const PinnedBlock pin_block(ctx->pinned, size_t(pin_rebuilt + nr));
+  if (!pin_block) return fail(FGPU_ERR_OOM, "PLAIN string interning: page-locked result buffer");
+  uint8_t* pin = pin_block.get();
   uint32_t* h_first = reinterpret_cast<uint32_t*>(pin);
   uint32_t* h_count = h_first + nv;
   std::vector<uint8_t> head(o_slot, 0);  // chunk table, zero counts, value addresses, front jobs
