@@ -112,9 +112,12 @@ struct KeyDesc {
   uint8_t shift;     // packed mode: bit offset inside the word
   uint32_t bits;     // packed mode: field width
   uint32_t dense_stride;  // dense mode: multiplier of (gid + 1)
-  uint8_t prog_off, prog_len;  // computed int64 key ((timestamp / 1000) * 1000): its program in QueryDesc::prog (prog_len > 0)
-  uint16_t _pad;
+  uint8_t prog_off, prog_len;  // computed int64 key ((timestamp / 1000) * 1000): its program in QueryDesc::prog (prog_len > 0);
+                               // boolean key: its program in BoolKeys::prog
+  uint8_t is_bool;   // boolean key (Distinct(..., value > 0)): code 1 false, 2 true in a 2-entry code key (radix 3)
+  uint8_t _pad;
 };
+static_assert(sizeof(KeyDesc) == 16, "KeyDesc");
 
 enum ProgOpCode : uint8_t { PO_LOAD = 0, PO_CONST = 1, PO_ADD = 2, PO_SUB = 3, PO_MUL = 4, PO_DIV = 5 };
 struct ProgOp {
@@ -183,6 +186,21 @@ struct QueryDesc {
   void* out_data[kMaxOut];       // int32 global ids (dictionary columns) or raw 8-byte values
   uint8_t* out_valid[kMaxOut];   // numeric columns: 0/1 per output row
   unsigned long long* tile_state;  // [n_tiles] decoupled look-back state
+  const struct BoolKeys* bool_keys;  // boolean Distinct keys (k_scan only); null: the plan has none
+};
+// Every kernel holds QueryDesc in shared memory or takes it by value as a kernel parameter: keep it inside 4 KB.
+static_assert(sizeof(QueryDesc) <= 4096, "QueryDesc grew past 4 KB");
+
+// The boolean keys of a Distinct (`Distinct(labels.a, value > 0)`, project.go:397-467): each key is a postfix program
+// over its own predicate leaves, which are compiled like the filter's but never select or drop a row.  The block is
+// uploaded with the plan; k_scan copies it, and the key leaves' LeafRt of the row group it works on, into the warp's
+// shared-memory region at wr_keys.
+struct BoolKeys {
+  int32_t n_leaves;  // key leaves (filter leaves + key leaves <= kMaxLeaves)
+  uint32_t wr_keys;  // offset of the per-warp copy: [BoolKeys][LeafRt x n_leaves]
+  const LeafRt* leaf_rt;  // [n_rg][n_leaves]
+  uint8_t prog[kMaxFilterProg];  // postfix programs of every key (KeyDesc::prog_off / prog_len): 0..31 push leaf; 0x80 AND; 0x81 OR
+  LeafDesc leaves[kMaxLeaves];
 };
 
 // Dense/hash table -> compacted result rows.

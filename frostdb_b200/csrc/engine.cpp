@@ -253,6 +253,7 @@ struct VisibleRG {
   RowGroupHost* rg;
   uint64_t skip_slots = 0;               // bit s: slot s is not read in this row group (its leaf is decided by statistics)
   uint8_t leaf_mode[kMaxLeaves] = {0};   // LeafMode per leaf decided from the chunk statistics (LM_EVAL: undecided)
+  uint8_t key_leaf_mode[kMaxLeaves] = {0};  // the same for the boolean keys' leaves (never drops the row group)
 };
 
 
@@ -407,6 +408,11 @@ struct Compiled {
   std::vector<uint8_t> slot_needed;  // 0: only named by Count(), whose result does not depend on the values
   std::vector<LeafHost> leaves;
   std::vector<uint8_t> filter_prog;
+  // boolean Distinct keys: their leaves and postfix programs, apart from the filter's (see BoolKeys)
+  std::vector<LeafHost> key_leaves;
+  std::vector<uint8_t> key_prog;
+  size_t filter_leaves = 0;  // the filter's leaves as written, before fuse_conjunction: the keys' share of kMaxLeaves
+  BoolKeys bool_keys{};
   std::vector<KeyOut> keys;
   std::vector<int> key_slots;
   QueryDesc qd{};
@@ -417,17 +423,21 @@ struct Compiled {
   uint32_t pruned_row_groups = 0;
   uint64_t touched_rows = ~uint64_t(0);  // rows of the row groups that survive pruning (~0: nothing was pruned)
   uint32_t radix(int k) const { return dense_radix[size_t(k)] ? dense_radix[size_t(k)] : 1; }  // (int64 keys have none)
+  bool has_bool_keys() const { return !key_leaves.empty(); }  // (every boolean key has a leaf)
 };
 
-int32_t compile_filter(const QueryPlan& q, int node, Compiled* c, const std::map<std::string, int>& slot_of) {
+// A boolean expression -> postfix program over its leaves, appended to *leaves and *prog.  `other`: leaves of the plan
+// kept elsewhere, which share the kMaxLeaves budget (the filter's, when a boolean key is compiled).
+int32_t compile_filter(const QueryPlan& q, int node, std::vector<LeafHost>* leaves, std::vector<uint8_t>* prog,
+                       const std::map<std::string, int>& slot_of, size_t other = 0) {
   const ExprNode& e = q.exprs[size_t(node)];
   if (e.kind != FGPU_EXPR_BINARY) return fail(FGPU_ERR_UNSUPPORTED, "unsupported boolean expression");
   if (e.op == FGPU_OP_AND || e.op == FGPU_OP_OR) {
-    int32_t rc = compile_filter(q, e.left, c, slot_of);
+    int32_t rc = compile_filter(q, e.left, leaves, prog, slot_of, other);
     if (rc) return rc;
-    rc = compile_filter(q, e.right, c, slot_of);
+    rc = compile_filter(q, e.right, leaves, prog, slot_of, other);
     if (rc) return rc;
-    c->filter_prog.push_back(e.op == FGPU_OP_AND ? 0x80 : 0x81);
+    prog->push_back(e.op == FGPU_OP_AND ? 0x80 : 0x81);
     return FGPU_OK;
   }
   switch (e.op) {
@@ -443,7 +453,7 @@ int32_t compile_filter(const QueryPlan& q, int node, Compiled* c, const std::map
   if (r.kind != FGPU_EXPR_LITERAL) return fail(FGPU_ERR_INVALID, "right side of binary expression must be a literal");
   if ((e.op == FGPU_OP_REGEX_MATCH || e.op == FGPU_OP_REGEX_NOT_MATCH) && !e.match)
     return fail(FGPU_ERR_INVALID, "regex leaf without a matcher");
-  if (c->leaves.size() >= size_t(kMaxLeaves)) return fail(FGPU_ERR_UNSUPPORTED, "too many predicate leaves");
+  if (leaves->size() + other >= size_t(kMaxLeaves)) return fail(FGPU_ERR_UNSUPPORTED, "too many predicate leaves");
   LeafHost lh;
   lh.column = l.name;
   lh.op = e.op;
@@ -451,8 +461,8 @@ int32_t compile_filter(const QueryPlan& q, int node, Compiled* c, const std::map
   lh.bin = &e;
   auto it = slot_of.find(l.name);
   lh.slot = (it == slot_of.end()) ? -1 : it->second;
-  c->filter_prog.push_back(uint8_t(c->leaves.size()));
-  c->leaves.push_back(std::move(lh));
+  prog->push_back(uint8_t(leaves->size()));
+  leaves->push_back(std::move(lh));
   return FGPU_OK;
 }
 
@@ -607,6 +617,7 @@ struct Columns {
   std::map<std::string, int> slot_of;
   std::vector<std::string> key_names;       // group-by / distinct / projected columns and computed keys, in plan order
   std::map<std::string, int32_t> key_expr;  // computed keys: name -> expression node
+  std::map<std::string, int32_t> bool_key;  // boolean Distinct keys (value > 0): name -> expression node
 
   // 1 for the slot of each column whose values the plan reads: keys, computed-key and aggregate inputs and,
   // with_filter, the filter's.  Count(col) counts rows, NULLs included (aggregate.go:929-950): its input column is
@@ -615,6 +626,8 @@ struct Columns {
     std::vector<std::string> need = key_names;
     for (auto& kv : key_expr) collect_columns(q, kv.second, &need);
     if (with_filter) collect_columns(q, q.filter, &need);
+    for (auto& kv : bool_key)  // read like the filter's: not in a row group where statistics decide every leaf on them
+      if (with_filter) collect_columns(q, kv.second, &need);
     for (const fgpu_agg& a : q.aggs)
       if (a.func != FGPU_AGG_COUNT) collect_columns(q, a.expr, &need);
     std::vector<uint8_t> out(slot_of.size(), 0);
@@ -662,6 +675,16 @@ int32_t resolve_columns(const QueryPlan& q, const Table& table, Compiled* c, Col
       if (present.count(name)) return fail(FGPU_ERR_UNSUPPORTED, "computed group key shadows a column: " + name);
       add_key_name(name);
       k->key_expr[name] = g;
+    } else if (e.kind == FGPU_EXPR_BINARY && q.kind == FGPU_PLAN_DISTINCT &&
+               ((e.op >= FGPU_OP_EQ && e.op <= FGPU_OP_GT_EQ) || e.op == FGPU_OP_REGEX_MATCH || e.op == FGPU_OP_REGEX_NOT_MATCH ||
+                e.op == FGPU_OP_AND || e.op == FGPU_OP_OR || e.op == FGPU_OP_CONTAINS || e.op == FGPU_OP_NOT_CONTAINS)) {
+      // boolean key: Builder.Distinct projects its expressions first (builder.go:117-134), a comparison as the filter's
+      // bitmap (boolExprProjection, project.go:397-467).  Present whatever the parts hold, so the key set and the
+      // partial-table shape of a multi-rank run do not depend on them.
+      const std::string name = q.expr_name(g);
+      if (present.count(name)) return fail(FGPU_ERR_UNSUPPORTED, "boolean key shadows a column: " + name);
+      add_key_name(name);
+      k->bool_key[name] = g;
     } else {
       return fail(FGPU_ERR_UNSUPPORTED, "this group-by expression is not supported on the GPU path");
     }
@@ -670,9 +693,10 @@ int32_t resolve_columns(const QueryPlan& q, const Table& table, Compiled* c, Col
   // slots: key columns first, then the computed keys', the filter's and the aggregates' input columns
   std::vector<std::string> cols;
   for (auto& n : key_names)
-    if (!k->key_expr.count(n)) cols.push_back(n);
+    if (!k->key_expr.count(n) && !k->bool_key.count(n)) cols.push_back(n);
   for (auto& kv : k->key_expr) collect_columns(q, kv.second, &cols);
   collect_columns(q, q.filter, &cols);
+  for (auto& kv : k->bool_key) collect_columns(q, kv.second, &cols);
   for (const fgpu_agg& a : q.aggs) collect_columns(q, a.expr, &cols);
   for (auto& name : cols) {
     auto it = present.find(name);
@@ -762,43 +786,84 @@ void fuse_conjunction(Compiled* c) {
   set_filter_prog(c);
 }
 
+// Stack depth of a postfix program (the kernels keep the stack in 32 bits).
+int postfix_depth(const std::vector<uint8_t>& prog, size_t off) {
+  int depth = 0, maxd = 0;
+  for (size_t i = off; i < prog.size(); i++) {
+    if (prog[i] < 0x80) depth++; else depth--;
+    maxd = std::max(maxd, depth);
+  }
+  return maxd;
+}
+
+// Missing-column rules and canonical form of every leaf (see LeafHost).
+int32_t canonical_leaves(std::vector<LeafHost>* leaves, const std::vector<uint8_t>& slot_types) {
+  for (LeafHost& lh : *leaves) {
+    lh.missing_mode = missing_column_mode(lh);
+    if (lh.slot < 0) continue;
+    int32_t rc = canonical_leaf(&lh, slot_types[size_t(lh.slot)]);
+    if (rc) return rc;
+  }
+  return FGPU_OK;
+}
+
+LeafDesc leaf_desc(const LeafHost& lh) {
+  LeafDesc ld{};
+  ld.slot = uint8_t(lh.slot < 0 ? 0xff : lh.slot);
+  ld.op = uint8_t(lh.op);
+  if (lh.slot < 0) return ld;
+  ld.cmp_float = lh.cmp_float;
+  ld.neg = lh.neg;
+  ld.lo_i = lh.lo_i; ld.hi_i = lh.hi_i;
+  ld.lo_f = lh.lo_f; ld.hi_f = lh.hi_f;
+  return ld;
+}
+
 // The filter: its program, its leaves in canonical form, fused under a conjunction, and their descriptors.
 int32_t compile_predicate(const QueryPlan& q, const Switches& w, const std::map<std::string, int>& slot_of, Compiled* c) {
   QueryDesc& qd = c->qd;
   if (q.filter >= 0) {
-    int32_t rc = compile_filter(q, q.filter, c, slot_of);
+    int32_t rc = compile_filter(q, q.filter, &c->leaves, &c->filter_prog, slot_of);
     if (rc) return rc;
     if (c->filter_prog.size() > size_t(kMaxFilterProg)) return fail(FGPU_ERR_UNSUPPORTED, "filter expression too large");
-    // stack depth check (the kernel keeps the stack in 32 bits)
-    int depth = 0, maxd = 0;
-    for (uint8_t op : c->filter_prog) {
-      if (op < 0x80) depth++; else depth--;
-      maxd = std::max(maxd, depth);
-    }
-    if (maxd > 30) return fail(FGPU_ERR_UNSUPPORTED, "filter expression too deep");
+    if (postfix_depth(c->filter_prog, 0) > 30) return fail(FGPU_ERR_UNSUPPORTED, "filter expression too deep");
     set_filter_prog(c);
   }
-  for (LeafHost& lh : c->leaves) {
-    lh.missing_mode = missing_column_mode(lh);
-    if (lh.slot < 0) continue;
-    int32_t rc = canonical_leaf(&lh, c->slot_types[size_t(lh.slot)]);
-    if (rc) return rc;
-  }
+  if (int32_t rc = canonical_leaves(&c->leaves, c->slot_types)) return rc;
+  c->filter_leaves = c->leaves.size();
   if (qd.filter_kind == FK_AND && !w.no_fuse) fuse_conjunction(c);
   qd.n_leaves = int32_t(c->leaves.size());
   for (int l = 0; l < qd.n_leaves; l++) {
     const LeafHost& lh = c->leaves[size_t(l)];
-    LeafDesc& ld = qd.leaves[l];
-    ld = LeafDesc{};
-    ld.slot = uint8_t(lh.slot < 0 ? 0xff : lh.slot);
-    ld.op = uint8_t(lh.op);
-    if (lh.slot < 0) continue;
-    qd.slot_used_by_leaf[lh.slot] = 1;
-    ld.cmp_float = lh.cmp_float;
-    ld.neg = lh.neg;
-    ld.lo_i = lh.lo_i; ld.hi_i = lh.hi_i;
-    ld.lo_f = lh.lo_f; ld.hi_f = lh.hi_f;
+    qd.leaves[l] = leaf_desc(lh);
+    if (lh.slot >= 0) qd.slot_used_by_leaf[lh.slot] = 1;
   }
+  return FGPU_OK;
+}
+
+// Boolean Distinct keys: each expression is compiled exactly as a filter would be (same leaves, refusals and
+// missing-column rules), into the key leaves and one postfix program per key.  Their leaves share the filter's
+// kMaxLeaves budget, counted with the filter's leaves as written (before fusion), so that FROSTGPU_NO_FUSE accepts and
+// refuses the same plans; they never take part in the filter's program, its fusion or row-group pruning.
+int32_t compile_bool_keys(const QueryPlan& q, const Columns& k, Compiled* c) {
+  BoolKeys& bk = c->bool_keys;
+  for (size_t i = 0; i < k.key_names.size(); i++) {
+    const auto it = k.bool_key.find(k.key_names[i]);
+    if (it == k.bool_key.end()) continue;
+    const size_t off = c->key_prog.size();
+    int32_t rc = compile_filter(q, it->second, &c->key_leaves, &c->key_prog, k.slot_of, c->filter_leaves);
+    if (rc) return rc;
+    if (c->key_prog.size() > size_t(kMaxFilterProg)) return fail(FGPU_ERR_UNSUPPORTED, "boolean key expressions too large");
+    if (postfix_depth(c->key_prog, off) > 30) return fail(FGPU_ERR_UNSUPPORTED, "boolean key expression too deep");
+    KeyDesc& kd = c->qd.keys[i];
+    kd.is_bool = 1;
+    kd.prog_off = uint8_t(off);
+    kd.prog_len = uint8_t(c->key_prog.size() - off);
+  }
+  if (int32_t rc = canonical_leaves(&c->key_leaves, c->slot_types)) return rc;
+  bk.n_leaves = int32_t(c->key_leaves.size());
+  std::memcpy(bk.prog, c->key_prog.data(), c->key_prog.size());
+  for (size_t l = 0; l < c->key_leaves.size(); l++) bk.leaves[l] = leaf_desc(c->key_leaves[l]);
   return FGPU_OK;
 }
 
@@ -881,10 +946,14 @@ void prune_row_groups(const QueryPlan& q, const Switches& w, const std::vector<u
       if (conj && v.leaf_mode[l] == LM_NONE) drop = true;
     }
     if (drop) continue;
+    // a boolean key's leaf decided LM_NONE makes the key false on the row group: the row group stays
+    for (size_t l = 0; l < c->key_leaves.size() && prune_on; l++) v.key_leaf_mode[l] = leaf_mode(*c, c->key_leaves[l], v);
     for (size_t s = 0; s < c->slot_names.size(); s++) {
       bool needed = base[s] != 0;
       for (size_t l = 0; l < c->leaves.size() && !needed; l++)
         if (c->leaves[l].slot == int(s) && v.leaf_mode[l] == LM_EVAL) needed = true;
+      for (size_t l = 0; l < c->key_leaves.size() && !needed; l++)
+        if (c->key_leaves[l].slot == int(s) && v.key_leaf_mode[l] == LM_EVAL) needed = true;
       if (!needed || !c->slot_needed[s]) v.skip_slots |= 1ull << s;
     }
     kept.push_back(v);
@@ -1028,13 +1097,14 @@ int32_t compile_aggregates(const QueryPlan& q, const std::map<std::string, int>&
   return FGPU_OK;
 }
 
-// One result key column of the plan (slot -1: a computed key).
-void add_key(Compiled* c, Table& table, const std::string& name, uint8_t type, int slot) {
+// One result key column of the plan (slot -1: a computed or boolean key).
+void add_key(Compiled* c, Table& table, const std::string& name, uint8_t type, int slot, bool is_bool = false) {
   KeyOut ko;
   ko.name = name;
-  ko.is_int64 = type != ST_DICT;
+  ko.is_bool = is_bool;
+  ko.is_int64 = !is_bool && type != ST_DICT;
   ko.is_float = type == ST_F64;
-  if (!ko.is_int64) ko.dict = &table.dicts[name];  // (a column whose every row group was pruned was never built: empty dictionary)
+  if (!ko.is_int64 && !is_bool) ko.dict = &table.dicts[name];  // (a column whose every row group was pruned was never built: empty dictionary)
   c->keys.push_back(std::move(ko));
   c->key_slots.push_back(slot);
 }
@@ -1060,9 +1130,10 @@ uint32_t hash_slots(uint64_t groups) {
   return uint32_t(cap);
 }
 
-// Group keys (dictionary and int64 columns, and computed int64 keys, whose programs follow the aggregates' in qd.prog)
-// and the aggregate table: dense over the dictionary ids when every key is a dictionary column and the product of
-// their radices is at most kDenseMax, a hash table of packed keys otherwise.
+// Group keys (dictionary and int64 columns, computed int64 keys, whose programs follow the aggregates' in qd.prog, and
+// boolean Distinct keys, which key like a dictionary column of two values) and the aggregate table: dense over the
+// dictionary ids when every key is a dictionary or boolean key and the product of their radices is at most kDenseMax,
+// a hash table of packed keys otherwise.
 int32_t table_shape(const QueryPlan& q, const Columns& k, Table& table, std::vector<ProgOp>* prog, Compiled* c) {
   QueryDesc& qd = c->qd;
   qd.n_keys = int32_t(k.key_names.size());
@@ -1085,6 +1156,14 @@ int32_t table_shape(const QueryPlan& q, const Columns& k, Table& table, std::vec
       if (!in_every_row_group(q, kx->second, c->rgs, &missing)) return fail(FGPU_ERR_NOT_FOUND, "group-by expression column not found: " + missing);
       qd.keys[i].prog_off = uint8_t(off);
       qd.keys[i].prog_len = uint8_t(prog->size() - off);
+    }
+    if (k.bool_key.count(name)) {  // a two-entry code key (compile_bool_keys filled its program)
+      add_key(c, table, name, ST_DICT, -1, /*is_bool=*/true);
+      c->dense_radix[i] = 3;  // 0 NULL (never), 1 false, 2 true
+      product *= 3;
+      qd.keys[i].slot = 0xff;
+      qd.keys[i].is_int64 = 0;
+      continue;
     }
     const int slot = kx != k.key_expr.end() ? -1 : k.slot_of.at(name);
     const uint8_t type = slot < 0 ? uint8_t(ST_I64) : c->slot_types[size_t(slot)];
@@ -1140,7 +1219,8 @@ bool plain_load(const QueryDesc& qd, int a) { return qd.aggs[a].prog_len == 1 &&
 // fused fast path of k_scan: conjunction of numeric leaves, dense dictionary keys, simple aggregates
 bool fast_path_ok(const Compiled& c, const Switches& w) {
   const QueryDesc& qd = c.qd;
-  if (w.no_fast || qd.table_mode != TM_DENSE || (qd.n_filter_prog != 0 && qd.filter_kind != FK_AND) || qd.n_leaves > 2 || qd.n_keys > 3)
+  if (w.no_fast || c.has_bool_keys() || qd.table_mode != TM_DENSE || (qd.n_filter_prog != 0 && qd.filter_kind != FK_AND) ||
+      qd.n_leaves > 2 || qd.n_keys > 3)
     return false;
   for (int l = 0; l < qd.n_leaves; l++) {
     const LeafHost& lh = c.leaves[size_t(l)];
@@ -1161,7 +1241,8 @@ void scan_layout(const Switches& w, Compiled* c) {
   int vl = w.vl, ring = w.ring;
   bool any_expr = false;
   for (int k = 0; k < qd.n_keys; k++)
-    if (qd.keys[k].prog_len) any_expr = true;
+    if (qd.keys[k].prog_len && !qd.keys[k].is_bool) any_expr = true;
+  const bool bool_keys = c->has_bool_keys();  // leafw holds the key leaves' bits once the selection is done
   for (int a = 0; a < qd.n_aggs; a++)
     if (qd.aggs[a].func != FGPU_AGG_COUNT && !plain_load(qd, a)) any_expr = true;
   auto r128 = [](size_t x) { return (x + 127) & ~size_t(127); };
@@ -1172,7 +1253,7 @@ void scan_layout(const Switches& w, Compiled* c) {
     qd.slot_bytes = uint32_t(slot);
     qd.wr_ring = uint32_t(off); off += size_t(ring) * slot;
     qd.wr_act = uint32_t(off); off = r128(off + size_t(vl / 32) * 4);
-    qd.wr_leaf = uint32_t(off); off = r128(off + ((qd.n_filter_prog > 0 && qd.filter_kind != FK_AND) ? size_t(vl) * 4 : 0));
+    qd.wr_leaf = uint32_t(off); off = r128(off + ((qd.n_filter_prog > 0 && qd.filter_kind != FK_AND) || bool_keys ? size_t(vl) * 4 : 0));
     qd.wr_slot = uint32_t(off); off = r128(off + size_t(vl) * 4);
     qd.wr_keyw = uint32_t(off); off = r128(off + (qd.table_mode == TM_HASH ? size_t(qd.key_words) * vl * 8 : 0));
     qd.wr_tmp1 = uint32_t(off); off = r128(off + (any_expr ? size_t(vl) * 8 : 0));
@@ -1182,6 +1263,7 @@ void scan_layout(const Switches& w, Compiled* c) {
     qd.wr_clrt = uint32_t(off); off = r128(off + size_t(std::max(qd.n_leaves, 1)) * sizeof(LeafRt));
     qd.wr_fplan = uint32_t(off); off = r128(off + 512);
     qd.wr_iplan = uint32_t(off); off = r128(off + 8 + 16 * size_t(kMaxStagePlain + kMaxStageSeeds));
+    c->bool_keys.wr_keys = uint32_t(off); off = r128(off + (bool_keys ? sizeof(BoolKeys) + c->key_leaves.size() * sizeof(LeafRt) : 0));
     qd.wr_bytes = uint32_t(off);
     if (size_t(qd.wr_bytes) * (kVecThreads / 32) <= 200 * 1024 || vl == 128) break;
     vl /= 2;  // many staged columns / wide keys: shorter vectors
@@ -1214,6 +1296,8 @@ int32_t compile(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, const Switches& 
   int32_t rc = resolve_columns(q, table, c, &k);
   if (rc) return rc;
   rc = compile_predicate(q, w, k.slot_of, c);
+  if (rc) return rc;
+  rc = compile_bool_keys(q, k, c);
   if (rc) return rc;
   prune_row_groups(q, w, q.kind == FGPU_PLAN_FILTER ? std::vector<uint8_t>(c->slot_names.size(), 1) : k.value_slots(q, false), c);
   rc = make_resident(ctx, table, c);
@@ -1473,13 +1557,16 @@ int32_t run_cached(fgpu_ctx* ctx, ExecCache& x, fgpu_result* res, int collective
 struct GeneralTables {
   std::vector<ChunkDesc> chunks;  // [row group][slot]
   std::vector<LeafRt> lrt;        // [row group][leaf]
+  std::vector<LeafRt> key_lrt;    // [row group][boolean key leaf]
   std::vector<uint32_t> first_tile, rg_rows;
   std::vector<uint8_t> lutbytes;                   // dictionary leaves: one result byte per global dictionary id
   std::vector<std::pair<size_t, size_t>> lut_fix;  // (index into lrt, offset into lutbytes)
+  std::vector<std::pair<size_t, size_t>> key_lut_fix;  // (index into key_lrt, offset into lutbytes)
   uint32_t tiles = 0;
   int n = 0;  // row groups that stay with the general kernel
-  GeneralTables(int n_rg, int n_slots, int n_leaves)
-      : chunks(size_t(n_rg) * std::max(n_slots, 1)), lrt(size_t(n_rg) * std::max(n_leaves, 1)), first_tile(size_t(n_rg) + 1), rg_rows(std::max(n_rg, 1)) {}
+  GeneralTables(int n_rg, int n_slots, int n_leaves, int n_key_leaves)
+      : chunks(size_t(n_rg) * std::max(n_slots, 1)), lrt(size_t(n_rg) * std::max(n_leaves, 1)), key_lrt(size_t(n_rg) * n_key_leaves),
+        first_tile(size_t(n_rg) + 1), rg_rows(std::max(n_rg, 1)) {}
 };
 
 // Fills row G.n of the general tables from row group g0 of the plan.
@@ -1502,8 +1589,8 @@ int32_t describe_row_group(fgpu_ctx* ctx, const QueryPlan& q, Compiled& c, int g
     }
     G.chunks[g * n_slots + s] = d;
   }
-  for (int l = 0; l < n_leaves; l++) {
-    LeafHost& lh = c.leaves[size_t(l)];
+  // the LeafRt of one leaf, stored at (*lrt)[at]; `decided`: what the statistics decided (LM_EVAL: nothing)
+  auto describe_leaf = [&](LeafHost& lh, uint8_t decided, std::vector<LeafRt>* lrt, std::vector<std::pair<size_t, size_t>>* lut_fix, size_t at) {
     LeafRt rt{};
     auto it = lh.slot < 0 ? v.rg->cols.end() : v.rg->cols.find(lh.column);
     if (it == v.rg->cols.end()) {
@@ -1518,13 +1605,16 @@ int32_t describe_row_group(fgpu_ctx* ctx, const QueryPlan& q, Compiled& c, int g
         G.lutbytes.resize(lh.lut_off + gd.values.size() + 1);
         for (size_t i = 0; i < gd.values.size(); i++) G.lutbytes[lh.lut_off + i] = dict_leaf_value(lh, gd.values[i]) ? 1 : 0;
       }
-      G.lut_fix.emplace_back(g * n_leaves + l, lh.lut_off);
+      lut_fix->emplace_back(at, lh.lut_off);
     } else {
       rt.mode = lh.null_literal ? LM_NONE : LM_EVAL;
     }
-    if (v.leaf_mode[l] != LM_EVAL) rt.mode = v.leaf_mode[l];
-    G.lrt[g * n_leaves + l] = rt;
-  }
+    if (decided != LM_EVAL) rt.mode = decided;
+    (*lrt)[at] = rt;
+  };
+  for (int l = 0; l < n_leaves; l++) describe_leaf(c.leaves[size_t(l)], v.leaf_mode[l], &G.lrt, &G.lut_fix, g * n_leaves + l);
+  const size_t nk = c.key_leaves.size();
+  for (size_t l = 0; l < nk; l++) describe_leaf(c.key_leaves[l], v.key_leaf_mode[l], &G.key_lrt, &G.key_lut_fix, g * nk + l);
   return FGPU_OK;
 }
 
@@ -1577,8 +1667,8 @@ struct RunsPlan {
 // Dense keys (up to kRunsKeys), a conjunction of int64 range leaves and of dictionary leaves (evaluated once per run),
 // up to kRunsAggs Sum / Min / Max of plain columns.
 bool runs_query(const Compiled& c, const QueryDesc& qd, const Switches& w, RunsPlan* P) {
-  if (w.no_fast || w.no_runs || qd.table_mode != TM_DENSE || (qd.n_filter_prog != 0 && qd.filter_kind != FK_AND) || qd.n_keys > kRunsKeys ||
-      qd.n_leaves > kRunsLeaves + kRunsPreds)
+  if (w.no_fast || w.no_runs || c.has_bool_keys() || qd.table_mode != TM_DENSE || (qd.n_filter_prog != 0 && qd.filter_kind != FK_AND) ||
+      qd.n_keys > kRunsKeys || qd.n_leaves > kRunsLeaves + kRunsPreds)
     return false;
   RunsDesc& rd = P->rd;
   auto col_of = [&](int slot) { return uint32_t(find_or_add(P->col_slot, &rd.n_cols, kRunsCols, slot)); };
@@ -1698,8 +1788,8 @@ struct PrefixBuilt {
   }
 };
 
-bool prefix_query(const RunsPlan& R, const Switches& w) {
-  if (w.no_prefix) return false;
+bool prefix_query(const Compiled& c, const RunsPlan& R, const Switches& w) {
+  if (w.no_prefix || c.has_bool_keys()) return false;
   for (int a = 0; a < R.na; a++)
     if (R.rd.agg_func[a] != uint32_t(FGPU_AGG_SUM)) return false;  // Min / Max / float64 Sum stay with k_runs_tma
   return true;
@@ -1845,7 +1935,8 @@ struct TilePlan {
 };
 
 bool tile_query(const Compiled& c, const QueryDesc& qd, const Switches& w, TilePlan* T) {
-  if (w.no_tile || qd.table_mode != TM_DENSE || (qd.n_filter_prog != 0 && qd.filter_kind != FK_AND) || qd.n_keys > kTaKeys) return false;
+  if (w.no_tile || c.has_bool_keys() || qd.table_mode != TM_DENSE || (qd.n_filter_prog != 0 && qd.filter_kind != FK_AND) || qd.n_keys > kTaKeys)
+    return false;
   TileAggDesc& td = T->td;
   auto plain_of = [&](int slot) { return find_or_add(T->plain_slot, &td.n_plain, kTaPlain, slot); };
   auto code_of = [&](int slot) { return find_or_add(T->code_slot, &td.n_codes, kTaCodes, slot); };
@@ -2209,7 +2300,7 @@ int32_t keep_exec_cache(fgpu_ctx* ctx, const QueryPlan& q, Compiled& c, const Qu
   x.qd = qd;
   x.shape = result_shape(q, c);
   for (const KeyOut& k : x.shape.keys) {  // small dictionaries are exported whole: the host then only copies index columns
-    x.dict_template.push_back(k.dict_snapshot.size() <= 4096 ? dict_column(k.dict_snapshot, nullptr) : nullptr);
+    x.dict_template.push_back(!k.is_bool && k.dict_snapshot.size() <= 4096 ? dict_column(k.dict_snapshot, nullptr) : nullptr);
   }
   st.kernel_launches++;  // k_finalize_dense (cached_tail)
   x.stats = st;  // what a cached Execute reports: no uploads, no compile, no segment-table build
@@ -2278,6 +2369,7 @@ int32_t run_scan(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, fgpu_result* re
   if (cacheable && c.exec && c.exec->ready && !w.no_exec_cache) return run_cached(ctx, *c.exec, res, collective);
   c.exec.reset();
   for (LeafHost& lh : c.leaves) lh.lut_off = size_t(-1);  // per-Execute state of the plan
+  for (LeafHost& lh : c.key_leaves) lh.lut_off = size_t(-1);
   pc.mark("compile");
   QueryDesc qd = c.qd;  // a copy: the plan in `c` may be reused by the next Execute
   const int n_rg = qd.n_rg, n_slots = qd.n_slots, n_leaves = qd.n_leaves;
@@ -2289,13 +2381,13 @@ int32_t run_scan(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, fgpu_result* re
   st.row_groups_pruned = c.pruned_row_groups;
 
   // ---- where every row group goes ----
-  GeneralTables G(n_rg, n_slots, n_leaves);
+  GeneralTables G(n_rg, n_slots, n_leaves, int(c.key_leaves.size()));
   const uint32_t tile_len = rows_plan ? uint32_t(kTileRows) : uint32_t(qd.vl);  // rows plan: CTA tiles; scan: warp vectors
   RunsPlan R;
   PrefixPlan P;
   TilePlan T;
   const bool runs_q = !rows_plan && runs_query(c, qd, w, &R);
-  const bool prefix_q = runs_q && prefix_query(R, w);
+  const bool prefix_q = runs_q && prefix_query(c, R, w);
   const bool tile_q = !rows_plan && tile_query(c, qd, w, &T);
   for (int g0 = 0; g0 < n_rg; g0++) {
     const size_t lut_mark = G.lut_fix.size();
@@ -2356,6 +2448,8 @@ int32_t run_scan(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, fgpu_result* re
   HostImage img;
   const size_t o_chunks = img.add(G.chunks), o_lrt = img.add(G.lrt), o_first = img.add(G.first_tile), o_rows = img.add(G.rg_rows);
   const size_t o_lut = img.add(G.lutbytes);
+  BoolKeys bk = c.bool_keys;
+  const size_t o_klrt = img.add(G.key_lrt), o_bk = c.has_bool_keys() ? img.add(&bk, sizeof bk) : 0;
   const size_t o_runs = img.add(R.rgs), o_runs_span = img.add(R.first_span);
   const size_t o_prefix = img.add(P.rgs), o_win = img.add(P.wins);
   const size_t o_tile = img.add(T.rgs), o_tile_first = img.add(T.first_tile);
@@ -2373,6 +2467,11 @@ int32_t run_scan(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, fgpu_result* re
   uint8_t* aux = static_cast<uint8_t*>(abuf.p);
   const uint8_t* lut = aux + o_lut;
   for (auto& fx : G.lut_fix) G.lrt[fx.first].lut = lut + fx.second;
+  for (auto& fx : G.key_lut_fix) G.key_lrt[fx.first].lut = lut + fx.second;
+  if (c.has_bool_keys()) {
+    bk.leaf_rt = reinterpret_cast<const LeafRt*>(aux + o_klrt);
+    qd.bool_keys = reinterpret_cast<const BoolKeys*>(aux + o_bk);
+  }
   for (RunsRg& r : R.rgs)
     for (const uint8_t*& p : r.pred_lut) lut_rebase(p, lut);
   for (TileAggRg& r : T.rgs)
@@ -2560,6 +2659,11 @@ int32_t finalize_dense_host(fgpu_result* res, ExecCache& x) {
       col.ext = reinterpret_cast<const uint8_t*>(idx);
       col.ext_keep = keep;
     }
+    if (ko.is_bool) {  // bits packed in place
+      bool_key_column(col, idx, G);
+      cols.push_back(std::move(col));
+      continue;
+    }
     // ids re-indexed in place; hdr[16 + k]: the kernel wrote a NULL key
     const OwnedColumn* whole = x.dict_template[size_t(k)].get();
     dict_key_column(col, idx, G, idx, ko.dict_snapshot, whole ? KeyDict::kWhole : KeyDict::kUsed, whole, hdr[16 + k] != 0);
@@ -2698,7 +2802,13 @@ int32_t finalize_result(fgpu_ctx* ctx, fgpu_result* res) {
     OwnedColumn col;
     col.name = key ? res->shape.keys[size_t(c)].name : res->shape.agg_names[size_t(c - nk)];
     col.length = int64_t(G);
-    if (key && !res->shape.keys[size_t(c)].is_int64) {  // codes (id + 1, 0 = NULL) re-indexed into col.data
+    if (key && res->shape.keys[size_t(c)].is_bool) {  // codes (1 false, 2 true) packed into bits in place
+      bool_key_column(col, reinterpret_cast<long long*>(blocks[size_t(c)].get()), G);
+      if (G) {
+        col.ext = blocks[size_t(c)].get();
+        col.ext_keep = std::move(blocks[size_t(c)]).keep();
+      }
+    } else if (key && !res->shape.keys[size_t(c)].is_int64) {  // codes (id + 1, 0 = NULL) re-indexed into col.data
       dict_key_column(col, reinterpret_cast<const long long*>(blocks[size_t(c)].get()), G, nullptr, res->shape.keys[size_t(c)].dict_snapshot,
                       KeyDict::kUsed);
     } else {

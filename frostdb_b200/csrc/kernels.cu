@@ -248,6 +248,26 @@ __device__ __forceinline__ bool leaf_range(const LeafDesc& ld, long long bits, b
   return in != (ld.neg != 0);
 }
 
+// A boolean key's postfix program over its leaf bits (0..31 push leaf; 0x80 AND; 0x81 OR), as eval_filter runs the filter's.
+__device__ __forceinline__ bool eval_postfix(const uint8_t* prog, int n, uint32_t bits) {
+  uint32_t stack = 0;  // stack kept in a 32-bit word
+  int sp = 0;
+  for (int i = 0; i < n; i++) {
+    uint8_t op = prog[i];
+    if (op < 0x80) {
+      stack = (stack & ~(1u << sp)) | (((bits >> op) & 1u) << sp);
+      sp++;
+    } else {
+      uint32_t b = (stack >> (sp - 1)) & 1u, a = (stack >> (sp - 2)) & 1u;
+      uint32_t r = (op == 0x80) ? (a & b) : (a | b);
+      sp -= 2;
+      stack = (stack & ~(1u << sp)) | (r << sp);
+      sp++;
+    }
+  }
+  return stack & 1u;
+}
+
 __device__ __forceinline__ bool eval_filter(const QueryDesc& q, uint32_t bits) {
   if (q.filter_kind == FK_AND) return (bits & q.filter_mask) == q.filter_mask;
   if (q.filter_kind == FK_OR) return (bits & q.filter_mask) != 0;
@@ -810,13 +830,92 @@ __device__ __noinline__ void vec_eval_expr(const VecCtx& v, uint8_t* wb, const A
   }
 }
 
+// ---- boolean keys -----------------------------------------------------------------------------------------
+// The per-warp copy of the plan's BoolKeys block, followed by the key leaves' LeafRt of the current row group.
+__device__ __forceinline__ const BoolKeys& warp_bool_keys(const QueryDesc& q, uint8_t* wb) {
+  return *reinterpret_cast<const BoolKeys*>(wb + __ldg(&q.bool_keys->wr_keys));
+}
+
+// leafw[row] bit l = key leaf l holds on that row: the filter's leaf rules (vec_selection), so a NULL numeric value is
+// false and a dictionary leaf takes null_result.  The selection is done with leafw by now.
+__device__ __noinline__ void vec_key_leaves(const VecCtx& v, uint8_t* wb, int lane) {
+  const WarpMem m = warp_mem(*v.q, wb);
+  const QueryDesc& q = *v.q;
+  const BoolKeys& bk = warp_bool_keys(q, wb);
+  const LeafRt* klrt = reinterpret_cast<const LeafRt*>(&bk + 1);
+  uint32_t cbits = 0;
+  for (int l = 0; l < bk.n_leaves; l++)
+    if (klrt[l].mode == LM_ALL) cbits |= 1u << l;
+  for (int s = 0; s < v.steps; s++) m.leafw[s * 32 + lane] = cbits;
+  for (int l = 0; l < bk.n_leaves; l++) {
+    const LeafDesc& ld = bk.leaves[l];
+    const LeafRt& rt = klrt[l];
+    if (rt.mode != LM_EVAL) continue;
+    if (q.slot_type[ld.slot] == ST_DICT) {
+      DictReader rd;
+      rd.init(v, ld.slot, lane);
+      const uint8_t* lut = rt.lut;
+      const uint32_t nullres = rt.null_result;
+#pragma unroll 1
+      for (int s = 0; s < v.steps; s++) {
+        const uint32_t gid = rd.next(v.r0 + uint32_t(s) * 32 + lane, v.n_rows);
+        const uint32_t res = (gid == kNullIdx) ? nullres : uint32_t(__ldg(lut + gid));
+        m.leafw[s * 32 + lane] |= (res & 1u) << l;
+      }
+    } else {
+      NumReader rd;
+      rd.init(v, ld.slot, lane);
+      const bool f64col = q.slot_type[ld.slot] == ST_F64;
+#pragma unroll 1
+      for (int s = 0; s < v.steps; s++) {
+        bool null;
+        const long long bits = rd.next(v.r0 + uint32_t(s) * 32 + lane, v.n_rows, null);
+        m.leafw[s * 32 + lane] |= uint32_t(!null && leaf_range(ld, bits, f64col)) << l;
+      }
+    }
+  }
+  __syncwarp();
+}
+
+// Code of a boolean key on this lane's row of step s: 1 false, 2 true, as hashBooleanArray hashes them
+// (dynparquet/hashed.go:228-242): neither is the NULL code 0.
+__device__ __forceinline__ uint32_t bool_key_code(const BoolKeys& bk, const KeyDesc& kd, const WarpMem& m, int s, int lane) {
+  return 1u + uint32_t(eval_postfix(bk.prog + kd.prog_off, kd.prog_len, m.leafw[s * 32 + lane]));
+}
+
+// Copies the key leaves' LeafRt of row group rg behind the warp's copy of the BoolKeys block, and the block itself at
+// the warp's first row group.
+__device__ __noinline__ void load_bool_keys(const QueryDesc& q, uint8_t* wb, int rg, bool first, int lane) {
+  uint32_t* dst = reinterpret_cast<uint32_t*>(wb + __ldg(&q.bool_keys->wr_keys));
+  if (first) {
+    const uint32_t* src = reinterpret_cast<const uint32_t*>(q.bool_keys);
+    for (uint32_t i = lane; i < sizeof(BoolKeys) / 4; i += 32) dst[i] = __ldg(src + i);
+    __syncwarp();
+  }
+  const BoolKeys& bk = *reinterpret_cast<const BoolKeys*>(dst);
+  const uint32_t* src = reinterpret_cast<const uint32_t*>(bk.leaf_rt + size_t(rg) * bk.n_leaves);
+  dst = reinterpret_cast<uint32_t*>(reinterpret_cast<BoolKeys*>(dst) + 1);
+  for (uint32_t i = lane; i < uint32_t(bk.n_leaves) * sizeof(LeafRt) / 4; i += 32) dst[i] = __ldg(src + i);
+}
+
 // ---- table slot per row ----------------------------------------------------------------------------------
 __device__ __noinline__ void vec_slots_dense(const VecCtx& v, uint8_t* wb, int lane) {
   const WarpMem m = warp_mem(*v.q, wb);
   const QueryDesc& q = *v.q;
   bool first = true;
+  if (q.bool_keys) vec_key_leaves(v, wb, lane);
   for (int k = 0; k < q.n_keys; k++) {
     const KeyDesc& kd = q.keys[k];
+    if (kd.is_bool) {
+      const BoolKeys& bk = warp_bool_keys(q, wb);
+#pragma unroll 1
+      for (int s = 0; s < v.steps; s++) {
+        const uint32_t add = bool_key_code(bk, kd, m, s, lane) * kd.dense_stride;
+        m.slotv[s * 32 + lane] = first ? add : m.slotv[s * 32 + lane] + add;
+      }
+      first = false;
+      continue;
+    }
     DictReader rd;
     rd.init(v, kd.slot, lane);
     const uint32_t stride = kd.dense_stride;
@@ -842,10 +941,16 @@ __device__ __noinline__ bool vec_slots_hash(const VecCtx& v, uint8_t* wb, int la
   bool overflow = false;
   for (int w = 0; w < W; w++)
     for (int s = 0; s < v.steps; s++) m.keyw[size_t(w) * q.vl + s * 32 + lane] = 0;
+  if (q.bool_keys) vec_key_leaves(v, wb, lane);
   for (int k = 0; k < q.n_keys; k++) {
     const KeyDesc& kd = q.keys[k];
     unsigned long long* kwp = m.keyw + size_t(kd.word) * q.vl;
-    if (kd.is_int64 && kd.prog_len) {
+    if (kd.is_bool) {
+      const BoolKeys& bk = warp_bool_keys(q, wb);
+      const uint32_t shift = kd.shift;
+#pragma unroll 1
+      for (int s = 0; s < v.steps; s++) kwp[s * 32 + lane] |= (unsigned long long)bool_key_code(bk, kd, m, s, lane) << shift;
+    } else if (kd.is_int64 && kd.prog_len) {
       // computed key (the sqlparse pre-projection `(timestamp / 1000) * 1000 as bucket`, project.go:58-167): the
       // expression is evaluated into the warp's temporaries; Div by zero yields 0, which groups like NULL
       AggDesc kx{};
@@ -1619,6 +1724,7 @@ __global__ void __launch_bounds__(kVecThreads, 4) k_scan(const QueryDesc* __rest
       src = reinterpret_cast<const uint32_t*>(q.leaf_rt + size_t(rg) * q.n_leaves);
       dst = reinterpret_cast<uint32_t*>(reinterpret_cast<LeafRt*>(wb + q.wr_clrt));
       for (uint32_t i = lane; i < uint32_t(q.n_leaves) * sizeof(LeafRt) / 4; i += 32) dst[i] = __ldg(src + i);
+      if (q.bool_keys) load_bool_keys(q, wb, rg, cached_rg < 0, lane);
       cached_rg = rg;
       cached_rows = __ldg(&q.rg_rows[rg]);
       __syncwarp();

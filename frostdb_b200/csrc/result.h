@@ -2,6 +2,7 @@
 // host (dictionary keys, validity from per-row bytes, dictionaries).  The device half (launches, copies back,
 // synchronisations) stays with each result path in engine.cpp.
 #pragma once
+#include <algorithm>
 #include <cstdint>
 #include <memory>
 #include <string>
@@ -17,6 +18,7 @@ struct KeyOut {
   std::string name;
   bool is_int64 = false;
   bool is_float = false;
+  bool is_bool = false;  // boolean Distinct key: no dictionary, never NULL
   const GlobalDict* dict = nullptr;
   std::vector<std::string> dict_snapshot;  // values by id at execute time
 };
@@ -95,6 +97,20 @@ void dict_key_column(OwnedColumn& col, const T* ids, size_t n, uint32_t* out, co
     col.dictionary->offsets = prepared->offsets;
   } else {
     col.dictionary = dict_column(values, nullptr);
+  }
+}
+
+// Makes `col` a boolean key column (format "b") of n rows from the per-row ids a kernel wrote for a two-entry code key
+// (id 0 false, 1 true; see row_id), bit-packed in place over `ids`: byte j is written once ids[8j .. 8j+7] are read, and
+// it never lies past them.  A boolean key is never NULL (project.go:397-467 builds it without validity).
+template <class T>
+void bool_key_column(OwnedColumn& col, T* ids, size_t n) {
+  col.format = "b";
+  uint8_t* bits = reinterpret_cast<uint8_t*>(ids);
+  for (size_t j = 0; j * 8 < n; j++) {
+    uint8_t b = 0;
+    for (size_t i = j * 8; i < std::min(n, j * 8 + 8); i++) b |= uint8_t(row_id(ids[i]) == 1) << (i & 7);
+    bits[j] = b;
   }
 }
 

@@ -234,7 +234,8 @@ int32_t fgpu_query_execute(fgpu_ctx* ctx, fgpu_query* q, uint64_t tx_watermark, 
 
 /* Next result record as an Arrow struct array (one child per output column).  Ownership passes
  * to the caller through the release callbacks.  Group-by columns are dictionary<uint32, binary>
- * (or int64), aggregate columns are named "sum(value)", "count(value)", ... exactly as
+ * (or int64; a boolean Distinct key such as `value > 0` is a bool column named after its expression, never NULL),
+ * aggregate columns are named "sum(value)", "count(value)", ... exactly as
  * aggregate.go:615-618 names them.  Returns FGPU_ERR_END after the last record. */
 int32_t fgpu_result_next(fgpu_result* r, struct ArrowSchema* out_schema, struct ArrowArray* out_array);
 int32_t fgpu_result_stats(const fgpu_result* r, fgpu_stats* out);
