@@ -1552,7 +1552,48 @@ int32_t run_cached(fgpu_ctx* ctx, ExecCache& x, fgpu_result* res, int collective
 // ---- Execute planning -----------------------------------------------------------------------------------------------
 // Every row group gets a row of the general tables that k_scan / k_rows read.  The specialised kernels may then take it,
 // in run_scan's order; each has a planner of three steps: a query-level check that fills its plan (or says no), an
-// admit step over the row group's rows of the general tables, and a layout step once every row group is placed.
+// admit step over the row group's rows of the general tables, and a layout step once every row group is placed.  Each
+// plan (the general tables included) then places its tables in the Execute's descriptor block (place), binds their
+// device addresses into its descriptor once the block is allocated (bind, before the block's image is copied), and says
+// how many launches it issues (launches).
+
+// The host image of an Execute's descriptor block: pieces at 16-byte aligned offsets, in the order they are added,
+// copied into page-locked scratch and uploaded with one copy.  A piece without a source is left zero.
+struct HostImage {
+  struct Piece { const void* src; size_t bytes, off; };
+  std::vector<Piece> pieces;
+  size_t end = 0;
+  static size_t align16(size_t x) { return (x + 15) & ~size_t(15); }
+  size_t add(const void* src, size_t bytes) {
+    const size_t off = align16(end);
+    pieces.push_back({src, bytes, off});
+    end = off + bytes;
+    return off;
+  }
+  template <class T> size_t add(const std::vector<T>& v) { return add(v.data(), v.size() * sizeof(T)); }
+  void copy_to(uint8_t* dst) const {
+    for (const Piece& p : pieces)
+      if (p.src && p.bytes) std::memcpy(dst + p.off, p.src, p.bytes);
+  }
+};
+
+template <class T> T* dev_at(uint8_t* block, size_t off) { return reinterpret_cast<T*>(block + off); }
+
+// The per-row-group descriptors of the specialised kernels refer to the LUT block before it has a device address: their
+// pred_lut entries hold its byte offset + 1 (null: no LUT) until lut_rebase turns them into pointers.
+const uint8_t* lut_ref(size_t off) { return reinterpret_cast<const uint8_t*>(uintptr_t(off) + 1); }
+template <class Rg> void lut_rebase(std::vector<Rg>& rgs, const uint8_t* lut) {
+  for (Rg& r : rgs)
+    for (const uint8_t*& p : r.pred_lut)
+      if (p) p = lut + (size_t(uintptr_t(p)) - 1);
+}
+
+// The table a specialised kernel adds to (the one k_scan adds to): its aggregate i is the query's agg_index[i].
+template <class D> void bind_target(D& d, const QueryDesc& qd, const int* agg_index, int na) {
+  d.t_rows = qd.t_rows;
+  for (int a = 0; a < na; a++) d.t_agg[a] = qd.t_agg[agg_index[a]];
+  d.counters = qd.counters;
+}
 
 struct GeneralTables {
   std::vector<ChunkDesc> chunks;  // [row group][slot]
@@ -1564,9 +1605,39 @@ struct GeneralTables {
   std::vector<std::pair<size_t, size_t>> key_lut_fix;  // (index into key_lrt, offset into lutbytes)
   uint32_t tiles = 0;
   int n = 0;  // row groups that stay with the general kernel
+  BoolKeys bk{};
+  bool has_bk = false;
+  size_t o_chunks = 0, o_lrt = 0, o_first = 0, o_rows = 0, o_lut = 0, o_klrt = 0, o_bk = 0;
   GeneralTables(int n_rg, int n_slots, int n_leaves, int n_key_leaves)
       : chunks(size_t(n_rg) * std::max(n_slots, 1)), lrt(size_t(n_rg) * std::max(n_leaves, 1)), key_lrt(size_t(n_rg) * n_key_leaves),
         first_tile(size_t(n_rg) + 1), rg_rows(std::max(n_rg, 1)) {}
+  void place(HostImage& img, const Compiled& c) {
+    o_chunks = img.add(chunks);
+    o_lrt = img.add(lrt);
+    o_first = img.add(first_tile);
+    o_rows = img.add(rg_rows);
+    o_lut = img.add(lutbytes);
+    o_klrt = img.add(key_lrt);
+    has_bk = c.has_bool_keys();
+    bk = c.bool_keys;
+    if (has_bk) o_bk = img.add(&bk, sizeof bk);
+  }
+  // Returns the device address of the LUT block, which the other plans' bind steps rebase onto.
+  const uint8_t* bind(uint8_t* block, QueryDesc& qd) {
+    const uint8_t* lut = block + o_lut;
+    for (auto& fx : lut_fix) lrt[fx.first].lut = lut + fx.second;
+    for (auto& fx : key_lut_fix) key_lrt[fx.first].lut = lut + fx.second;
+    if (has_bk) {
+      bk.leaf_rt = dev_at<const LeafRt>(block, o_klrt);
+      qd.bool_keys = dev_at<const BoolKeys>(block, o_bk);
+    }
+    qd.chunks = dev_at<const ChunkDesc>(block, o_chunks);
+    qd.leaf_rt = dev_at<const LeafRt>(block, o_lrt);
+    qd.rg_first_tile = dev_at<const uint32_t>(block, o_first);
+    qd.rg_rows = dev_at<const uint32_t>(block, o_rows);
+    return lut;
+  }
+  uint32_t launches() const { return tiles ? 1 : 0; }  // k_scan, or k_rows
 };
 
 // Fills row G.n of the general tables from row group g0 of the plan.
@@ -1618,13 +1689,6 @@ int32_t describe_row_group(fgpu_ctx* ctx, const QueryPlan& q, Compiled& c, int g
   return FGPU_OK;
 }
 
-// The per-row-group descriptors of the specialised kernels refer to the LUT block before it has a device address: they
-// hold its byte offset + 1 (null: no LUT) until lut_rebase turns that into a pointer.
-const uint8_t* lut_ref(size_t off) { return reinterpret_cast<const uint8_t*>(uintptr_t(off) + 1); }
-void lut_rebase(const uint8_t*& p, const uint8_t* lut) {
-  if (p) p = lut + (size_t(uintptr_t(p)) - 1);
-}
-
 // Index of `slot` in slots[0, *n), appended when missing (-1: the list is full at cap).
 int find_or_add(int* slots, uint32_t* n, int cap, int slot) {
   for (uint32_t i = 0; i < *n; i++)
@@ -1662,6 +1726,23 @@ struct RunsPlan {
   std::vector<RunsRg> rgs;
   std::vector<RunsRgCols> cols;
   std::vector<uint32_t> first_span;
+  size_t o_rgs = 0, o_span = 0;
+  void place(HostImage& img) {
+    o_rgs = img.add(rgs);
+    o_span = img.add(first_span);
+  }
+  void bind(uint8_t* block, const uint8_t* lut, const QueryDesc& qd, ScanLaunch& L) {
+    lut_rebase(rgs, lut);
+    L.runs = !rgs.empty();
+    L.rd = rd;
+    L.rd.rgs = dev_at<const RunsRg>(block, o_rgs);
+    L.rd.rg_first_span = dev_at<const uint32_t>(block, o_span);
+    bind_target(L.rd, qd, agg_index, na);
+    L.runs_nl = nl;
+    L.runs_nk = nk;
+    L.runs_na = na;
+  }
+  uint32_t launches() const { return rgs.empty() ? 0 : 1; }  // k_runs_tma
 };
 
 // Dense keys (up to kRunsKeys), a conjunction of int64 range leaves and of dictionary leaves (evaluated once per run),
@@ -1775,6 +1856,17 @@ struct PrefixPlan {
   uint64_t seg_bound = 0;  // segments at most: every run start of every key column and every window start
   uint64_t all_rows = 0;   // rows of the admitted row groups (they all pass)
   uint32_t n_sums = 1;     // distinct Sum inputs of the first row group (as the accounting counts them)
+  size_t o_rgs = 0, o_wins = 0;
+  void place(HostImage& img) {
+    o_rgs = img.add(rgs);
+    o_wins = img.add(wins);
+  }
+  void bind(uint8_t* block, ScanLaunch& L) {  // (k_runs_prefix's own descriptor is filled by prefix_build)
+    L.prefix = !rgs.empty();
+    bd.rgs = dev_at<const PrefixRg>(block, o_rgs);
+    bd.wins = dev_at<const PrefixWin>(block, o_wins);
+  }
+  uint32_t launches() const { return rgs.empty() ? 0 : 1; }  // k_runs_prefix (the segment-table build: PrefixBuilt)
 };
 
 // After the build step: its launches, and the bytes an Execute reads per segment (entry + P[b], P[e] of every distinct
@@ -1919,6 +2011,44 @@ int32_t runs_layout(fgpu_ctx* ctx, const Compiled& c, const Switches& w, RunsPla
   return FGPU_OK;
 }
 
+// The plan's segment table [seg_off | seg | build scratch] in sbuf, built behind the upload (count, scan, scatter),
+// and the k_runs_prefix launch that reads it.  The build's segment count comes back to the page-locked word *count.
+int32_t prefix_build(fgpu_ctx* ctx, const PrefixPlan& P, const RunsPlan& R, const QueryDesc& qd, DevBuf& sbuf, uint32_t* count, PrefixDesc* pd,
+                     PrefixBuilt* pb, fgpu_stats& st) {
+  // k_runs_prefix stores every cell of the table in place of k_table_init: only right when the table is dense and
+  // every stored aggregate is Sum(int64) (identity 0), which prefix_query and runs_query let through
+  if (qd.table_mode != TM_DENSE) return fail(FGPU_ERR_INVALID, "prefix path planned for a hash-mode table");
+  for (int a = 0; a < qd.n_aggs; a++)
+    if (qd.aggs[a].func != FGPU_AGG_COUNT && (qd.aggs[a].func != FGPU_AGG_SUM || qd.aggs[a].is_float))
+      return fail(FGPU_ERR_INVALID, "prefix path planned for a table with an aggregate other than Sum(int64)");
+  cudaStream_t s = ctx->stream;
+  const uint32_t n_slots = uint32_t(qd.table_slots);
+  const size_t off_bytes = HostImage::align16(size_t(n_slots + 1) * 4), seg_bytes = HostImage::align16(P.seg_bound * sizeof(PrefixSeg));
+  CUDA_TRY(sbuf.alloc(off_bytes + seg_bytes + prefix_build_scratch_bytes(n_slots), s));
+  uint8_t* sb = static_cast<uint8_t*>(sbuf.p);
+  const uint32_t* seg_off = reinterpret_cast<const uint32_t*>(sb);
+  PrefixBuildDesc bd = P.bd;
+  bd.seg = reinterpret_cast<PrefixSeg*>(sb + off_bytes);
+  CUDA_TRY(launch_prefix_build(bd, n_slots, reinterpret_cast<uint32_t*>(sb), sb + off_bytes + seg_bytes, ctx->sm_count, s));
+  CUDA_TRY(cudaMemcpyAsync(count, seg_off + n_slots, 4, cudaMemcpyDeviceToHost, s));
+  pb->count = count;
+  pb->per_seg = sizeof(PrefixSeg) + 16 * uint64_t(P.n_sums);
+  pb->launches = 3;  // count, scan (as one), scatter
+  st.algorithmic_bytes += uint64_t(n_slots + 1) * 4;  // seg_off
+  pd->n_slots = n_slots;
+  pd->na = uint32_t(R.na);
+  // lanes per slot: about one segment each up to a warp; a CTA per slot for lists of several hundred
+  const uint64_t per_slot = (P.seg_bound + n_slots - 1) / n_slots;
+  while (pd->group_log2 < 5 && (uint64_t(1) << pd->group_log2) < per_slot) pd->group_log2++;
+  if (per_slot >= 256) pd->group_log2 = 8;
+  pd->all_rows = P.all_rows;
+  pd->rgs = bd.rgs;
+  pd->seg_off = seg_off;
+  pd->seg = bd.seg;
+  bind_target(*pd, qd, R.agg_index, R.na);
+  return FGPU_OK;
+}
+
 // ---- tile aggregate (tile_agg.cu) ----
 // Row groups the sorted-run kernel does not take (bit-packed / short-run / nullable keys, L0 records) go to the
 // tile-aggregate kernel when the plan is a conjunction of range + dictionary leaves over a dense table with plain
@@ -1932,6 +2062,20 @@ struct TilePlan {
   int leaf_q[kTaLeaves] = {0}, pred_q[kTaPreds] = {0}, agg_index[kTaAggs] = {0};
   bool agg_bounded = true;  // every int64 Sum input of every row group has statistics inside [0, 2^32)
   uint64_t agg_max = 0;     // the largest of those chunk maxima
+  size_t o_rgs = 0, o_first = 0;
+  void place(HostImage& img) {
+    o_rgs = img.add(rgs);
+    o_first = img.add(first_tile);
+  }
+  void bind(uint8_t* block, const uint8_t* lut, const QueryDesc& qd, ScanLaunch& L) {
+    lut_rebase(rgs, lut);
+    L.tile = !rgs.empty();
+    L.td = td;
+    L.td.rgs = dev_at<const TileAggRg>(block, o_rgs);
+    L.td.rg_first_tile = dev_at<const uint32_t>(block, o_first);
+    bind_target(L.td, qd, agg_index, int(td.na));
+  }
+  uint32_t launches() const { return rgs.empty() ? 0 : 1; }  // k_tile_agg
 };
 
 bool tile_query(const Compiled& c, const QueryDesc& qd, const Switches& w, TilePlan* T) {
@@ -2116,6 +2260,21 @@ struct TakePlan {
   std::vector<uint32_t> first_span;
   int range[kTakeLeaves] = {0}, pred[kTakePreds] = {0};  // range leaves (PLAIN int64 columns) and dictionary leaves (flat
   int n_range = 0, n_pred = 0;                           // codes + result byte per dictionary id) of the plan
+  size_t o_rgs = 0, o_span = 0, o_count = 0;
+  void place(HostImage& img) {
+    o_rgs = img.add(rgs);
+    o_span = img.add(first_span);
+    o_count = img.add(nullptr, (size_t(td.n_spans) + 1) * 8);
+  }
+  void bind(uint8_t* block, const uint8_t* lut, const QueryDesc& qd) {
+    lut_rebase(rgs, lut);
+    td.rgs = dev_at<const TakeRg>(block, o_rgs);
+    td.rg_first_span = dev_at<const uint32_t>(block, o_span);
+    td.span_count = dev_at<unsigned long long>(block, o_count);
+    td.total = qd.counters;
+    for (int o = 0; o < qd.n_out; o++) td.out_data[o] = static_cast<long long*>(qd.out_data[o]);
+  }
+  uint32_t launches() const { return td.n_spans ? 3 : 0; }  // count per span, scan, ordered write
 };
 
 // general: row groups left with the general kernel (all of them unless pruning dropped some).
@@ -2213,26 +2372,6 @@ void take_layout(TakePlan& P, const QueryDesc& qd, int sm_count) {
   td.n_out = uint32_t(qd.n_out);
 }
 
-// The host image of an Execute's descriptor block: pieces at 16-byte aligned offsets, in the order they are added,
-// copied into page-locked scratch and uploaded with one copy.  A piece without a source is left zero.
-struct HostImage {
-  struct Piece { const void* src; size_t bytes, off; };
-  std::vector<Piece> pieces;
-  size_t end = 0;
-  static size_t align16(size_t x) { return (x + 15) & ~size_t(15); }
-  size_t add(const void* src, size_t bytes) {
-    const size_t off = align16(end);
-    pieces.push_back({src, bytes, off});
-    end = off + bytes;
-    return off;
-  }
-  template <class T> size_t add(const std::vector<T>& v) { return add(v.data(), v.size() * sizeof(T)); }
-  void copy_to(uint8_t* dst) const {
-    for (const Piece& p : pieces)
-      if (p.src && p.bytes) std::memcpy(dst + p.off, p.src, p.bytes);
-  }
-};
-
 // The result's columns (see ResultShape), with the key dictionaries snapshotted now.
 ResultShape result_shape(const QueryPlan& q, const Compiled& c) {
   ResultShape r;
@@ -2302,7 +2441,6 @@ int32_t keep_exec_cache(fgpu_ctx* ctx, const QueryPlan& q, Compiled& c, const Qu
   for (const KeyOut& k : x.shape.keys) {  // small dictionaries are exported whole: the host then only copies index columns
     x.dict_template.push_back(!k.is_bool && k.dict_snapshot.size() <= 4096 ? dict_column(k.dict_snapshot, nullptr) : nullptr);
   }
-  st.kernel_launches++;  // k_finalize_dense (cached_tail)
   x.stats = st;  // what a cached Execute reports: no uploads, no compile, no segment-table build
   x.stats.kernel_launches -= pb.launches;
   x.stats.h2d_bytes = 0;
@@ -2318,6 +2456,21 @@ int32_t keep_exec_cache(fgpu_ctx* ctx, const QueryPlan& q, Compiled& c, const Qu
     return FGPU_OK;
   }
   return finalize_dense_host(res, x);
+}
+
+FinalizeDesc finalize_desc(const Compiled& c, const QueryDesc& qd) {
+  FinalizeDesc fd{};
+  fd.table_mode = qd.table_mode;
+  fd.key_words = qd.key_words;
+  fd.n_keys = qd.n_keys;
+  fd.n_aggs = qd.n_aggs;
+  fd.table_slots = qd.table_slots;
+  for (int k = 0; k < qd.n_keys; k++) {
+    fd.keys[k] = qd.keys[k];
+    fd.dense_radix[k] = c.radix(k);
+  }
+  bind_finalize(&fd, qd);
+  return fd;
 }
 
 // Rows plan: one output array per projected column (worst case every row is selected) + look-back state per tile.
@@ -2344,52 +2497,35 @@ int32_t alloc_rows_out(fgpu_ctx* ctx, uint64_t total_rows, uint32_t tiles, DevBu
   return FGPU_OK;
 }
 
-// Plans and launches one Execute.  On success the result owns the device table (or, for a cached plan, the plan does).
-// collective: 0 no exchange; 1 / 2: the first run of a plan pushes its partial table and leaves the result pending
-// (the merge half is collective_end); a cached plan does what run_cached does for the mode.
-int32_t run_scan(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, fgpu_result* res, bool count_groups = false, bool cacheable = false,
-                 int collective = 0) {
-  PhaseClock pc;
+// The query's compiled plan in q.plan_cache: the one it holds while the table epoch, the read transaction and the
+// switches are those it was compiled for, a fresh one otherwise.
+int32_t compiled_plan(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, const Switches& w) {
   Table& plan_table = ctx->tables[q.table];
   if (plan_table.epoch == 0) plan_table.epoch = ++ctx->epoch_counter;
-  const Switches w = switches();
-  if (!q.plan_cache || q.cache_epoch != plan_table.epoch || q.cache_tx != tx || q.cache_env != w.key || w.no_plan_cache) {
-    std::shared_ptr<void> fresh(new Compiled(), [](void* p) { delete static_cast<Compiled*>(p); });
-    int32_t rc0 = compile(ctx, q, tx, w, static_cast<Compiled*>(fresh.get()));
-    q.plan_cache.reset();
-    if (rc0) return rc0;
-    q.plan_cache = std::move(fresh);
-    q.cache_epoch = plan_table.epoch;
-    q.cache_tx = tx;
-    q.cache_env = w.key;
-  } else {
+  if (q.plan_cache && q.cache_epoch == plan_table.epoch && q.cache_tx == tx && q.cache_env == w.key && !w.no_plan_cache) {
     static_cast<Compiled*>(q.plan_cache.get())->h2d_bytes = 0;  // nothing is uploaded by a cached plan
+    return FGPU_OK;
   }
-  Compiled& c = *static_cast<Compiled*>(q.plan_cache.get());
-  if (cacheable && c.exec && c.exec->ready && !w.no_exec_cache) return run_cached(ctx, *c.exec, res, collective);
-  c.exec.reset();
-  for (LeafHost& lh : c.leaves) lh.lut_off = size_t(-1);  // per-Execute state of the plan
-  for (LeafHost& lh : c.key_leaves) lh.lut_off = size_t(-1);
-  pc.mark("compile");
-  QueryDesc qd = c.qd;  // a copy: the plan in `c` may be reused by the next Execute
-  const int n_rg = qd.n_rg, n_slots = qd.n_slots, n_leaves = qd.n_leaves;
-  const bool rows_plan = q.kind == FGPU_PLAN_FILTER;
-  fgpu_stats& st = res->stats;
-  st.rows_scanned = c.total_rows;
-  st.rows_touched = c.touched_rows == ~uint64_t(0) ? c.total_rows : c.touched_rows;
-  st.row_groups = uint32_t(n_rg);
-  st.row_groups_pruned = c.pruned_row_groups;
+  std::shared_ptr<void> fresh(new Compiled(), [](void* p) { delete static_cast<Compiled*>(p); });
+  int32_t rc = compile(ctx, q, tx, w, static_cast<Compiled*>(fresh.get()));
+  q.plan_cache.reset();
+  if (rc) return rc;
+  q.plan_cache = std::move(fresh);
+  q.cache_epoch = plan_table.epoch;
+  q.cache_tx = tx;
+  q.cache_env = w.key;
+  return FGPU_OK;
+}
 
-  // ---- where every row group goes ----
-  GeneralTables G(n_rg, n_slots, n_leaves, int(c.key_leaves.size()));
+// Row groups of the plan -> the general tables, or the sorted-run, prefix-sum or tile-aggregate plan that takes them.
+int32_t route_row_groups(fgpu_ctx* ctx, const QueryPlan& q, Compiled& c, const QueryDesc& qd, const Switches& w, bool rows_plan, GeneralTables& G,
+                         RunsPlan& R, PrefixPlan& P, TilePlan& T, fgpu_stats& st) {
+  const int n_slots = qd.n_slots, n_leaves = qd.n_leaves;
   const uint32_t tile_len = rows_plan ? uint32_t(kTileRows) : uint32_t(qd.vl);  // rows plan: CTA tiles; scan: warp vectors
-  RunsPlan R;
-  PrefixPlan P;
-  TilePlan T;
   const bool runs_q = !rows_plan && runs_query(c, qd, w, &R);
   const bool prefix_q = runs_q && prefix_query(c, R, w);
   const bool tile_q = !rows_plan && tile_query(c, qd, w, &T);
-  for (int g0 = 0; g0 < n_rg; g0++) {
+  for (int g0 = 0; g0 < qd.n_rg; g0++) {
     const size_t lut_mark = G.lut_fix.size();
     if (int32_t rc = describe_row_group(ctx, q, c, g0, G, st)) return rc;
     const VisibleRG& v = c.rgs[size_t(g0)];
@@ -2416,6 +2552,38 @@ int32_t run_scan(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, fgpu_result* re
     G.n++;
   }
   G.first_tile[size_t(G.n)] = G.tiles;
+  return FGPU_OK;
+}
+
+// Plans and launches one Execute.  On success the result owns the device table (or, for a cached plan, the plan does).
+// collective: 0 no exchange; 1 / 2: the first run of a plan pushes its partial table and leaves the result pending
+// (the merge half is collective_end); a cached plan does what run_cached does for the mode.
+int32_t run_scan(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, fgpu_result* res, bool count_groups = false, bool cacheable = false,
+                 int collective = 0) {
+  PhaseClock pc;
+  const Switches w = switches();
+  if (int32_t rc = compiled_plan(ctx, q, tx, w)) return rc;
+  Compiled& c = *static_cast<Compiled*>(q.plan_cache.get());
+  if (cacheable && c.exec && c.exec->ready && !w.no_exec_cache) return run_cached(ctx, *c.exec, res, collective);
+  c.exec.reset();
+  for (LeafHost& lh : c.leaves) lh.lut_off = size_t(-1);  // per-Execute state of the plan
+  for (LeafHost& lh : c.key_leaves) lh.lut_off = size_t(-1);
+  pc.mark("compile");
+  QueryDesc qd = c.qd;  // a copy: the plan in `c` may be reused by the next Execute
+  const int n_rg = qd.n_rg;
+  const bool rows_plan = q.kind == FGPU_PLAN_FILTER;
+  fgpu_stats& st = res->stats;
+  st.rows_scanned = c.total_rows;
+  st.rows_touched = c.touched_rows == ~uint64_t(0) ? c.total_rows : c.touched_rows;
+  st.row_groups = uint32_t(n_rg);
+  st.row_groups_pruned = c.pruned_row_groups;
+
+  // ---- where every row group goes ----
+  GeneralTables G(n_rg, qd.n_slots, qd.n_leaves, int(c.key_leaves.size()));
+  RunsPlan R;
+  PrefixPlan P;
+  TilePlan T;
+  if (int32_t rc = route_row_groups(ctx, q, c, qd, w, rows_plan, G, R, P, T, st)) return rc;
   qd.n_rg = G.n;
   qd.n_tiles = G.tiles;
   if (int32_t rc = runs_layout(ctx, c, w, R, P, st)) return rc;
@@ -2444,153 +2612,63 @@ int32_t run_scan(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, fgpu_result* re
     return rc;
   }
 
-  // device block: [tables | counters 64 B | group counter 16 B | QueryDesc]
+  // device block: [plans' tables | counters 64 B | group counter 16 B | QueryDesc]
   HostImage img;
-  const size_t o_chunks = img.add(G.chunks), o_lrt = img.add(G.lrt), o_first = img.add(G.first_tile), o_rows = img.add(G.rg_rows);
-  const size_t o_lut = img.add(G.lutbytes);
-  BoolKeys bk = c.bool_keys;
-  const size_t o_klrt = img.add(G.key_lrt), o_bk = c.has_bool_keys() ? img.add(&bk, sizeof bk) : 0;
-  const size_t o_runs = img.add(R.rgs), o_runs_span = img.add(R.first_span);
-  const size_t o_prefix = img.add(P.rgs), o_win = img.add(P.wins);
-  const size_t o_tile = img.add(T.rgs), o_tile_first = img.add(T.first_tile);
-  size_t o_take = 0, o_take_span = 0, o_take_count = 0;
-  if (take_q) {
-    o_take = img.add(K.rgs);
-    o_take_span = img.add(K.first_span);
-    o_take_count = img.add(nullptr, (size_t(K.td.n_spans) + 1) * 8);
-  }
+  G.place(img, c);
+  R.place(img);
+  P.place(img);
+  T.place(img);
+  if (take_q) K.place(img);
   const size_t o_cnt = img.add(nullptr, 64 + 16);
   const size_t o_qd = img.add(&qd, sizeof(QueryDesc));
   const size_t aux_bytes = img.end;
   const size_t o_ret = HostImage::align16(aux_bytes);  // scratch only: counters + group count read back
   CUDA_TRY(abuf.alloc(aux_bytes, ctx->stream));
   uint8_t* aux = static_cast<uint8_t*>(abuf.p);
-  const uint8_t* lut = aux + o_lut;
-  for (auto& fx : G.lut_fix) G.lrt[fx.first].lut = lut + fx.second;
-  for (auto& fx : G.key_lut_fix) G.key_lrt[fx.first].lut = lut + fx.second;
-  if (c.has_bool_keys()) {
-    bk.leaf_rt = reinterpret_cast<const LeafRt*>(aux + o_klrt);
-    qd.bool_keys = reinterpret_cast<const BoolKeys*>(aux + o_bk);
-  }
-  for (RunsRg& r : R.rgs)
-    for (const uint8_t*& p : r.pred_lut) lut_rebase(p, lut);
-  for (TileAggRg& r : T.rgs)
-    for (const uint8_t*& p : r.pred_lut) lut_rebase(p, lut);
-  for (TakeRg& r : K.rgs)
-    for (const uint8_t*& p : r.pred_lut) lut_rebase(p, lut);
-  qd.chunks = reinterpret_cast<const ChunkDesc*>(aux + o_chunks);
-  qd.leaf_rt = reinterpret_cast<const LeafRt*>(aux + o_lrt);
-  qd.rg_first_tile = reinterpret_cast<const uint32_t*>(aux + o_first);
-  qd.rg_rows = reinterpret_cast<const uint32_t*>(aux + o_rows);
   qd.counters = cache_mode ? reinterpret_cast<unsigned long long*>(static_cast<uint8_t*>(tbuf.p) + tbytes)  // behind the table: one copy brings both back
-                           : reinterpret_cast<unsigned long long*>(aux + o_cnt);
-  const QueryDesc* qdesc_dev = reinterpret_cast<const QueryDesc*>(aux + o_qd);
+                           : dev_at<unsigned long long>(aux, o_cnt);
+  ScanLaunch L;
+  const uint8_t* lut = G.bind(aux, qd);
+  R.bind(aux, lut, qd, L);
+  P.bind(aux, L);
+  T.bind(aux, lut, qd, L);
+  if (take_q) K.bind(aux, lut, qd);
+  const QueryDesc* qdesc_dev = dev_at<const QueryDesc>(aux, o_qd);
   CUDA_TRY(ctx->ensure_scratch(o_ret + 128));
   std::memset(ctx->scratch, 0, o_ret + 128);
   img.copy_to(ctx->scratch);
 
   FinalizeDesc& fd = res->fd;
-  fd = FinalizeDesc{};
-  fd.table_mode = qd.table_mode;
-  fd.key_words = qd.key_words;
-  fd.n_keys = qd.n_keys;
-  fd.n_aggs = qd.n_aggs;
-  fd.table_slots = qd.table_slots;
-  for (int k = 0; k < qd.n_keys; k++) {
-    fd.keys[k] = qd.keys[k];
-    fd.dense_radix[k] = c.radix(k);
-  }
-  bind_finalize(&fd, qd);
+  fd = finalize_desc(c, qd);
   cudaStream_t s = ctx->stream;
   pc.mark("describe");
   CUDA_TRY(cudaEventRecord(ctx->ev[0], s));
   CUDA_TRY(cudaMemcpyAsync(aux, ctx->scratch, aux_bytes, cudaMemcpyHostToDevice, s));
-  ScanLaunch L;
   PrefixBuilt pb;
   if (rows_plan) {
     CUDA_TRY(cudaMemsetAsync(qd.tile_state, 0, size_t(G.tiles) * 8, s));
     CUDA_TRY(cudaEventRecord(ctx->ev[1], s));
     if (take_q) {
-      TakeDesc& td = K.td;
-      td.rgs = reinterpret_cast<const TakeRg*>(aux + o_take);
-      td.rg_first_span = reinterpret_cast<const uint32_t*>(aux + o_take_span);
-      td.span_count = reinterpret_cast<unsigned long long*>(aux + o_take_count);
-      td.total = qd.counters;
-      for (int o = 0; o < qd.n_out; o++) td.out_data[o] = static_cast<long long*>(qd.out_data[o]);
-      CUDA_TRY(launch_take(td, ctx->sm_count, s));
-      st.kernel_launches += 2;
+      CUDA_TRY(launch_take(K.td, ctx->sm_count, s));
       res->rows_no_nulls = true;
     } else {
       CUDA_TRY(launch_rows(qdesc_dev, qd, ctx->sm_count, s));
     }
     CUDA_TRY(cudaEventRecord(ctx->ev[2], s));
   } else {
-    L.runs = !R.rgs.empty();
-    L.rd = R.rd;
-    L.rd.rgs = reinterpret_cast<const RunsRg*>(aux + o_runs);
-    L.rd.rg_first_span = reinterpret_cast<const uint32_t*>(aux + o_runs_span);
-    L.rd.t_rows = qd.t_rows;
-    for (int a = 0; a < R.na; a++) L.rd.t_agg[a] = qd.t_agg[R.agg_index[a]];
-    L.rd.counters = qd.counters;
-    L.runs_nl = R.nl;
-    L.runs_nk = R.nk;
-    L.runs_na = R.na;
-    L.prefix = !P.rgs.empty();
     if (L.prefix) {
-      // k_runs_prefix stores every cell of the table in place of k_table_init: only right when the table is dense and
-      // every stored aggregate is Sum(int64) (identity 0), which prefix_query and runs_query let through
-      if (qd.table_mode != TM_DENSE) return fail(FGPU_ERR_INVALID, "prefix path planned for a hash-mode table");
-      for (int a = 0; a < qd.n_aggs; a++)
-        if (qd.aggs[a].func != FGPU_AGG_COUNT && (qd.aggs[a].func != FGPU_AGG_SUM || qd.aggs[a].is_float))
-          return fail(FGPU_ERR_INVALID, "prefix path planned for a table with an aggregate other than Sum(int64)");
-      // the plan's segment table: [seg_off | seg | build scratch]
-      const uint32_t n_slots = uint32_t(qd.table_slots);
-      const size_t off_bytes = HostImage::align16(size_t(n_slots + 1) * 4), seg_bytes = HostImage::align16(P.seg_bound * sizeof(PrefixSeg));
-      DevBuf& sbuf = cache_mode ? c.exec->segs : res->segs;
-      CUDA_TRY(sbuf.alloc(off_bytes + seg_bytes + prefix_build_scratch_bytes(n_slots), s));
-      uint8_t* sb = static_cast<uint8_t*>(sbuf.p);
-      const uint32_t* seg_off = reinterpret_cast<const uint32_t*>(sb);
-      PrefixBuildDesc bd = P.bd;
-      bd.rgs = reinterpret_cast<const PrefixRg*>(aux + o_prefix);
-      bd.wins = reinterpret_cast<const PrefixWin*>(aux + o_win);
-      bd.seg = reinterpret_cast<PrefixSeg*>(sb + off_bytes);
-      CUDA_TRY(launch_prefix_build(bd, n_slots, reinterpret_cast<uint32_t*>(sb), sb + off_bytes + seg_bytes, ctx->sm_count, s));
       uint32_t* count = reinterpret_cast<uint32_t*>(ctx->scratch + o_ret + 96);
-      CUDA_TRY(cudaMemcpyAsync(count, seg_off + n_slots, 4, cudaMemcpyDeviceToHost, s));
-      pb.count = count;
-      pb.per_seg = sizeof(PrefixSeg) + 16 * uint64_t(P.n_sums);
-      pb.launches = 3;  // count, scan (as one), scatter
-      st.kernel_launches += pb.launches;
-      st.algorithmic_bytes += uint64_t(n_slots + 1) * 4;  // seg_off
-      PrefixDesc& pd = L.pd;
-      pd.n_slots = n_slots;
-      pd.na = uint32_t(R.na);
-      // lanes per slot: about one segment each up to a warp; a CTA per slot for lists of several hundred
-      const uint64_t per_slot = (P.seg_bound + n_slots - 1) / n_slots;
-      while (pd.group_log2 < 5 && (uint64_t(1) << pd.group_log2) < per_slot) pd.group_log2++;
-      if (per_slot >= 256) pd.group_log2 = 8;
-      pd.all_rows = P.all_rows;
-      pd.rgs = bd.rgs;
-      pd.seg_off = seg_off;
-      pd.seg = bd.seg;
-      pd.t_rows = qd.t_rows;
-      for (int a = 0; a < R.na; a++) pd.t_agg[a] = qd.t_agg[R.agg_index[a]];
-      pd.counters = qd.counters;
+      if (int32_t rc = prefix_build(ctx, P, R, qd, cache_mode ? c.exec->segs : res->segs, count, &L.pd, &pb, st)) return rc;
     }
-    L.tile = !T.rgs.empty();
-    L.td = T.td;
-    L.td.rgs = reinterpret_cast<const TileAggRg*>(aux + o_tile);
-    L.td.rg_first_tile = reinterpret_cast<const uint32_t*>(aux + o_tile_first);
-    L.td.t_rows = qd.t_rows;
-    for (uint32_t a = 0; a < T.td.na; a++) L.td.t_agg[a] = qd.t_agg[T.agg_index[a]];
-    L.td.counters = qd.counters;
     if (int32_t rc = launch_aggregate_scan(ctx, qd, qdesc_dev, L)) return rc;
-    st.kernel_launches += uint32_t(L.runs) + uint32_t(L.prefix) + uint32_t(L.tile);
     st.row_groups_runs += uint32_t(R.rgs.size() + P.rgs.size());
     st.row_groups_prefix += uint32_t(P.rgs.size());
     st.row_groups_tiles += uint32_t(T.rgs.size());
   }
-  st.kernel_launches += (rows_plan || L.prefix ? 0 : 1) + (G.tiles ? 1 : 0);  // k_table_init, k_scan
+  // k_table_init unless k_runs_prefix stores the table; k_finalize_dense of a kept plan, or the group count behind the scan
+  count_groups = count_groups && !rows_plan && !cache_mode && !collective;  // (a collective Execute's table is not final yet)
+  st.kernel_launches += (rows_plan || L.prefix ? 0 : 1) + (take_q ? K.launches() : G.launches()) + R.launches() + P.launches() + pb.launches +
+                        T.launches() + (cache_mode ? 1 : 0) + (count_groups ? 1 : 0);
   st.h2d_bytes += aux_bytes + sizeof(QueryDesc);
   unsigned long long* counters = reinterpret_cast<unsigned long long*>(ctx->scratch + o_ret);
   res->cnt_ptr = reinterpret_cast<unsigned int*>(qd.counters + 8);  // 16 bytes behind the counters, zeroed by the upload / the table init
@@ -2599,7 +2677,6 @@ int32_t run_scan(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, fgpu_result* re
     if (int32_t rc = comm_push(ctx, tbuf.p, tbytes, &res->pending_seq, &res->pending_bytes)) return rc;
     res->pending = true;
     res->plan_keep = q.plan_cache;
-    count_groups = false;  // the table is not final yet
   }
   if (cache_mode) {
     ExecCache& x = *c.exec;
@@ -2608,9 +2685,8 @@ int32_t run_scan(fgpu_ctx* ctx, const QueryPlan& q, uint64_t tx, fgpu_result* re
     x.launch = L;
     return keep_exec_cache(ctx, q, c, qd, res, pc, pb);
   }
-  if (count_groups && !rows_plan) {  // count the result rows behind the scan: one host round trip less
+  if (count_groups) {  // count the result rows behind the scan: one host round trip less
     CUDA_TRY(launch_count_groups(fd, res->cnt_ptr, s));
-    st.kernel_launches++;
     res->groups_known = true;
   }
   CUDA_TRY(cudaMemcpyAsync(counters, qd.counters, 64 + 16, cudaMemcpyDeviceToHost, s));

@@ -27,12 +27,16 @@
 // per-warp vectors; see DESIGN.md.)
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <climits>
 #include <cstdint>
+#include <map>
+#include <mutex>
 
 #include "device_types.h"
 #include "kernels.h"
 #include "agg_ops.cuh"
+#include "ptx.cuh"
 
 namespace fgpu {
 
@@ -47,8 +51,6 @@ static_assert(STEPS == 4, "unrolled for 4 steps");
 
 constexpr uint32_t kNoSlot = 0xffffffffu;
 constexpr uint32_t FULL = 0xffffffffu;
-
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
 
 // ---- hybrid stream cursor ------------------------------------------------------------------------------
 struct HybCur {
@@ -1152,12 +1154,6 @@ struct FastPlan {
   FastAgg agg[kFastAggs];
 };
 
-__device__ __forceinline__ long long lds64(uint32_t a) {
-  long long v;
-  asm volatile("ld.shared.b64 %0, [%1];" : "=l"(v) : "r"(a));
-  return v;
-}
-
 // lane 0 builds the plan of the warp's current row group from the cached descriptors
 __device__ __noinline__ void build_fast_plan(const QueryDesc& q, const ChunkDesc* chunks, const LeafRt* lrt, FastPlan* fp) {
   fp->ok = 0;
@@ -1385,7 +1381,7 @@ __device__ __noinline__ uint32_t fast_pass(const QueryDesc& q, uint8_t* wb, cons
       act = idx < n_in;
 #pragma unroll
       for (int l = 0; l < NL; l++) {
-        const long long x = lds64(lcol[l] + uint32_t(s) * 256u);
+        const long long x = (long long)lds64(lcol[l] + uint32_t(s) * 256u);
         bool in;
         if (lflags[l] & 1u) {
           const double d = (lflags[l] & 2u) ? __longlong_as_double(x) : double(x);
@@ -1407,7 +1403,7 @@ __device__ __noinline__ uint32_t fast_pass(const QueryDesc& q, uint8_t* wb, cons
       cnt += act ? 1u : 0u;
 #pragma unroll
       for (int a = 0; a < NA; a++) {
-        const long long val = lds64(acol[a] + uint32_t(s) * 256u);
+        const long long val = (long long)lds64(acol[a] + uint32_t(s) * 256u);
         if (sum64[a]) part[a] = (long long)((unsigned long long)part[a] + (act ? (unsigned long long)val : 0ull));
         else if (act) part[a] = agg_combine(uint8_t(fp.agg[a].func & 0xff), (fp.agg[a].func >> 8) != 0, part[a], val);
       }
@@ -1416,7 +1412,7 @@ __device__ __noinline__ uint32_t fast_pass(const QueryDesc& q, uint8_t* wb, cons
     // ---- cold: step s leaves the running group ----
     long long val[NA > 0 ? NA : 1];
 #pragma unroll
-    for (int a = 0; a < NA; a++) val[a] = lds64(acol[a] + uint32_t(s) * 256u);
+    for (int a = 0; a < NA; a++) val[a] = (long long)lds64(acol[a] + uint32_t(s) * 256u);
     fast_cold_step<NA>(q, fp, slot, act, val, lane, cs, cnt, part);
     s++;
   }
@@ -1506,7 +1502,7 @@ __device__ __noinline__ uint32_t fast_pass_tight(const QueryDesc& q, uint8_t* wb
     bool act = true;
 #pragma unroll
     for (int l = 0; l < NL; l++) {
-      const long long x = lds64(lcol[l] + uint32_t(s) * 256u);
+      const long long x = (long long)lds64(lcol[l] + uint32_t(s) * 256u);
       act = act && x >= lo[l] && x <= hi[l];
     }
     return act;
@@ -1534,7 +1530,7 @@ __device__ __noinline__ uint32_t fast_pass_tight(const QueryDesc& q, uint8_t* wb
     long long val[NA > 0 ? NA : 1], p2[NA > 0 ? NA : 1];
 #pragma unroll
     for (int a = 0; a < NA; a++) {
-      val[a] = lds64(acol[a] + uint32_t(s) * 256u);
+      val[a] = (long long)lds64(acol[a] + uint32_t(s) * 256u);
       p2[a] = (long long)part[a];
     }
     fast_cold_step<NA>(q, fp, slot, act, val, lane, cs, cnt, p2);
@@ -1572,7 +1568,7 @@ __device__ __noinline__ uint32_t fast_pass_tight(const QueryDesc& q, uint8_t* wb
       cnt += act ? 1u : 0u;
       sel += act ? 1u : 0u;
 #pragma unroll
-      for (int a = 0; a < NA; a++) part[a] += act ? (unsigned long long)lds64(acol[a] + uint32_t(s) * 256u) : 0ull;
+      for (int a = 0; a < NA; a++) part[a] += act ? lds64(acol[a] + uint32_t(s) * 256u) : 0ull;
     }
     if (s >= steps) break;
     // ---- the step that holds row `safe`: lanes below it still belong to the running group ----
@@ -1583,7 +1579,7 @@ __device__ __noinline__ uint32_t fast_pass_tight(const QueryDesc& q, uint8_t* wb
     sel += act ? 1u : 0u;
     cnt += old ? 1u : 0u;
 #pragma unroll
-    for (int a = 0; a < NA; a++) part[a] += old ? (unsigned long long)lds64(acol[a] + uint32_t(s) * 256u) : 0ull;
+    for (int a = 0; a < NA; a++) part[a] += old ? lds64(acol[a] + uint32_t(s) * 256u) : 0ull;
     if (safe < rend) {
       advance(safe);
       uint32_t safe2 = rend, us2 = 0;
@@ -1600,7 +1596,7 @@ __device__ __noinline__ uint32_t fast_pass_tight(const QueryDesc& q, uint8_t* wb
         }
         cnt += fresh ? 1u : 0u;
 #pragma unroll
-        for (int a = 0; a < NA; a++) part[a] += fresh ? (unsigned long long)lds64(acol[a] + uint32_t(s) * 256u) : 0ull;
+        for (int a = 0; a < NA; a++) part[a] += fresh ? lds64(acol[a] + uint32_t(s) * 256u) : 0ull;
       } else {
         general_step(s, r, fresh);
       }
@@ -2011,12 +2007,52 @@ __global__ void __launch_bounds__(NT) k_decode(ChunkDesc c, uint32_t n_chunks, i
 // host launchers
 // ======================================================================================================
 namespace {
+struct KernelConfig {
+  size_t smem_limit = 0;                       // dynamic shared memory limit raised so far (0: the default)
+  std::map<std::pair<int, size_t>, int> ctas;  // (threads, dynamic shared memory) -> resident CTAs per SM
+};
+std::mutex config_mu;
+std::map<std::pair<int, const void*>, KernelConfig> configs;  // (device, kernel), guarded by config_mu
+
+cudaError_t kernel_config(const void* kern, KernelConfig** out) {  // (config_mu held)
+  int dev = 0;
+  const cudaError_t e = cudaGetDevice(&dev);
+  if (e == cudaSuccess) *out = &configs[{dev, kern}];
+  return e;
+}
+
 int grid_for(size_t n) {
   int blocks = int((n + 255) / 256);
   if (blocks > 132 * 8) blocks = 132 * 8;  // 8 CTAs per SM of an H100 SXM (132 SMs), grid-stride beyond
   return blocks < 1 ? 1 : blocks;
 }
 }  // namespace
+
+cudaError_t kernel_smem_at_least(const void* kern, size_t smem) {
+  std::lock_guard<std::mutex> lock(config_mu);
+  KernelConfig* k = nullptr;
+  cudaError_t e = kernel_config(kern, &k);
+  if (e != cudaSuccess || smem <= k->smem_limit) return e;
+  e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
+  if (e == cudaSuccess) k->smem_limit = smem;
+  return e;
+}
+
+cudaError_t kernel_ctas_per_sm(const void* kern, int threads, size_t smem, int* per_sm) {
+  std::lock_guard<std::mutex> lock(config_mu);
+  KernelConfig* k = nullptr;
+  cudaError_t e = kernel_config(kern, &k);
+  if (e != cudaSuccess) return e;
+  auto it = k->ctas.find({threads, smem});
+  if (it == k->ctas.end()) {
+    int n = 0;
+    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kern, threads, smem);
+    if (e != cudaSuccess) return e;
+    it = k->ctas.emplace(std::make_pair(threads, smem), std::max(n, 1)).first;
+  }
+  *per_sm = it->second;
+  return cudaSuccess;
+}
 
 cudaError_t launch_table_init(const QueryDesc& q, cudaStream_t st, bool zero_counters) {
   k_table_init<<<grid_for(q.table_slots), 256, 0, st>>>(q, zero_counters);
@@ -2027,20 +2063,11 @@ cudaError_t launch_scan(const QueryDesc* d_q, const QueryDesc& q, int sm_count, 
   if (q.n_tiles == 0) return cudaSuccess;
   const int warps = kVecThreads / 32;
   const size_t smem = size_t(q.wr_bytes) * warps + (q.n_rg <= 2048 ? (size_t(q.n_rg) + 1) * 4 + 16 : 0);
-  static size_t configured = 0;
-  if (smem > configured) {
-    cudaError_t e = cudaFuncSetAttribute(k_scan, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
-    if (e != cudaSuccess) return e;
-    configured = smem;
-  }
-  static size_t occ_smem = ~size_t(0);
-  static int per_sm = 0;
-  if (occ_smem != smem) {
-    cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_scan, kVecThreads, smem);
-    if (e != cudaSuccess) return e;
-    if (per_sm < 1) per_sm = 1;
-    occ_smem = smem;
-  }
+  const void* kern = reinterpret_cast<const void*>(k_scan);
+  int per_sm = 0;
+  cudaError_t e = kernel_smem_at_least(kern, smem);
+  if (e == cudaSuccess) e = kernel_ctas_per_sm(kern, kVecThreads, smem, &per_sm);
+  if (e != cudaSuccess) return e;
   uint32_t grid = uint32_t(sm_count) * uint32_t(per_sm);
   const uint32_t need = (q.n_tiles + warps - 1) / warps;
   if (grid > need) grid = need;
@@ -2051,9 +2078,8 @@ cudaError_t launch_scan(const QueryDesc* d_q, const QueryDesc& q, int sm_count, 
 cudaError_t launch_rows(const QueryDesc* d_q, const QueryDesc& q, int sm_count, cudaStream_t st) {
   if (q.n_tiles == 0) return cudaSuccess;
   int per_sm = 0;
-  cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_rows, NT, 0);
+  cudaError_t e = kernel_ctas_per_sm(reinterpret_cast<const void*>(k_rows), NT, 0, &per_sm);
   if (e != cudaSuccess) return e;
-  if (per_sm < 1) per_sm = 1;
   uint32_t grid = uint32_t(sm_count) * uint32_t(per_sm);
   if (grid > q.n_tiles) grid = q.n_tiles;
   k_rows<<<grid, NT, 0, st>>>(d_q);

@@ -16,6 +16,11 @@ constexpr int kVecThreads = 128;  // scan kernel: 4 independent warps per CTA
 constexpr int kMaxVecRows = 1024;  // rows per warp vector (multiple of kIndexRows)
 constexpr int kIndexRows = 128;  // chunk index granularity (one warp): fixed when run directories are built
 
+// Launch configuration of a kernel on the current device, cached per (device, kernel) behind one mutex: raise its
+// dynamic shared memory limit to at least `smem` bytes, and its resident CTAs per SM at (threads, smem), at least 1.
+cudaError_t kernel_smem_at_least(const void* kern, size_t smem);
+cudaError_t kernel_ctas_per_sm(const void* kern, int threads, size_t smem, int* per_sm);
+
 cudaError_t launch_table_init(const QueryDesc& q, cudaStream_t st, bool zero_counters = true);
 cudaError_t launch_scan(const QueryDesc* d_q, const QueryDesc& q, int sm_count, cudaStream_t st);
 // sorted-run scan, CTA-cooperative with TMA-staged column tiles (runs_tma.cu): nl range leaves, nk run-length keys,

@@ -25,17 +25,13 @@
 
 #include "device_types.h"
 #include "kernels.h"
+#include "ptx.cuh"
 
 namespace fgpu {
 namespace {
 
 constexpr unsigned FULL = 0xffffffffu;
 constexpr int kPfWarps = 8;  // warps per CTA (independent)
-
-template <typename T>
-__device__ __forceinline__ T ldg_ptr(T const* p) {
-  return reinterpret_cast<T>(__ldg(reinterpret_cast<const unsigned long long*>(p)));
-}
 
 // Warp-cooperative: index of the run that holds `row` (the last entry whose start <= row), from the row's 128-row seed.
 __device__ __forceinline__ uint32_t run_of_row(const Run* runs, const Seed* seeds, uint32_t n_runs, uint32_t row, uint32_t lane) {

@@ -33,11 +33,11 @@
 #include <cstdio>
 
 #include <algorithm>
-#include <unordered_map>
 
 #include "agg_ops.cuh"
 #include "device_types.h"
 #include "kernels.h"
+#include "ptx.cuh"
 
 namespace fgpu {
 namespace {
@@ -46,57 +46,9 @@ constexpr unsigned FULL = 0xffffffffu;
 constexpr uint32_t kNoSlot = 0xffffffffu;
 constexpr int kNQ = kRunsKeys + kRunsPreds;  // most cursor columns of one launch
 
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return uint32_t(__cvta_generic_to_shared(p)); }
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "WAIT_%=:\n"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-      "@p bra DONE_%=;\n"
-      "bra WAIT_%=;\n"
-      "DONE_%=:\n"
-      "}\n" ::"r"(bar),
-      "r"(parity)
-      : "memory");
-}
-__device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst), "l"(src), "r"(bytes),
-               "r"(bar)
-               : "memory");
-}
-__device__ __forceinline__ unsigned long long lds64(uint32_t a) {
-  unsigned long long v;
-  asm volatile("ld.shared.b64 %0, [%1];" : "=l"(v) : "r"(a));
-  return v;
-}
 __device__ __forceinline__ uint2 lds_v2(uint32_t a) {
   uint2 v;
   asm volatile("ld.shared.v2.b32 {%0, %1}, [%2];" : "=r"(v.x), "=r"(v.y) : "r"(a));
-  return v;
-}
-__device__ __forceinline__ uint32_t lds32(uint32_t a) {
-  uint32_t v;
-  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(a));
-  return v;
-}
-__device__ __forceinline__ uint32_t lds16(uint32_t a) {
-  uint32_t v;
-  asm volatile("ld.shared.u16 %0, [%1];" : "=r"(v) : "r"(a));
-  return v;
-}
-__device__ __forceinline__ uint32_t lds8(uint32_t a) {
-  uint32_t v;
-  asm volatile("ld.shared.u8 %0, [%1];" : "=r"(v) : "r"(a));
   return v;
 }
 // one staged value of 1 << LG bytes, zero-extended
@@ -121,11 +73,6 @@ __device__ __forceinline__ void sts_v2(uint32_t a, uint32_t x, uint32_t y) {
   asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(a), "r"(x), "r"(y) : "memory");
 }
 __device__ __forceinline__ void sts32(uint32_t a, uint32_t x) { asm volatile("st.shared.b32 [%0], %1;" ::"r"(a), "r"(x) : "memory"); }
-
-template <typename T>
-__device__ __forceinline__ T ldg_ptr(T const* p) {
-  return reinterpret_cast<T>(__ldg(reinterpret_cast<const unsigned long long*>(p)));
-}
 
 // Cursor column q of a row group: keys first, then the dictionary leaves.
 struct CursorCol {
@@ -722,13 +669,8 @@ cudaError_t launch_runs_tma(const RunsDesc& d, int nl, int nk, int na, int sm_co
   if (d.n_spans == 0) return cudaSuccess;
   const size_t smem = runs_tma_smem_bytes(d);
   RtKern kern = pick(d, nl, nk, na);
-  static std::unordered_map<const void*, size_t> configured;  // (guarded by the engine's mutex)
-  size_t& cfg = configured[reinterpret_cast<const void*>(kern)];
-  if (smem > cfg) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
-    if (e != cudaSuccess) return e;
-    cfg = smem;
-  }
+  const cudaError_t e = kernel_smem_at_least(reinterpret_cast<const void*>(kern), smem);
+  if (e != cudaSuccess) return e;
   uint32_t grid = uint32_t(sm_count) * uint32_t(runs_tma_ctas_per_sm(d));
   const uint32_t chunks = (d.n_spans + d.span_blocks - 1) / d.span_blocks;
   if (grid > chunks) grid = chunks;

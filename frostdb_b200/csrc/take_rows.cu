@@ -21,8 +21,6 @@
 // selected row 8 read + 8 written per projected column.
 #include <cuda_runtime.h>
 
-#include <unordered_map>
-
 #include "device_types.h"
 #include "kernels.h"
 
@@ -229,13 +227,9 @@ __global__ void __launch_bounds__(kTakeThreads) k_take_write(const __grid_consta
 
 template <typename K>
 cudaError_t run(K kern, const TakeDesc& d, int sm_count, cudaStream_t st) {
-  static std::unordered_map<const void*, int> occ;  // (instances share one function type: key by address)
-  int& per_sm = occ[reinterpret_cast<const void*>(kern)];
-  if (per_sm == 0) {
-    cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kTakeThreads, 0);
-    if (e != cudaSuccess) return e;
-    if (per_sm < 1) per_sm = 1;
-  }
+  int per_sm = 0;
+  const cudaError_t e = kernel_ctas_per_sm(reinterpret_cast<const void*>(kern), kTakeThreads, 0, &per_sm);
+  if (e != cudaSuccess) return e;
   uint32_t grid = uint32_t(sm_count) * uint32_t(per_sm);
   const uint32_t need = (d.n_spans + kTakeWarps - 1) / kTakeWarps;
   if (grid > need) grid = need;

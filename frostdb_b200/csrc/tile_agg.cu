@@ -29,11 +29,10 @@
 // Algorithmic bytes per row: 8 per staged PLAIN column + w / 8 per staged code column.
 #include <cuda_runtime.h>
 
-#include <unordered_map>
-
 #include "agg_ops.cuh"
 #include "device_types.h"
 #include "kernels.h"
+#include "ptx.cuh"
 
 namespace fgpu {
 namespace {
@@ -42,56 +41,6 @@ constexpr unsigned FULL = 0xffffffffu;
 constexpr int NC = kTaConsumerWarps * 32;  // consumer threads
 constexpr uint32_t kHdrBytes = 256;        // per-stage tile header: TileAggRg + row range
 static_assert(sizeof(TileAggRg) + 16 <= kHdrBytes, "tile header fits its slot");
-
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return uint32_t(__cvta_generic_to_shared(p)); }
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "WAIT_%=:\n"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-      "@p bra DONE_%=;\n"
-      "bra WAIT_%=;\n"
-      "DONE_%=:\n"
-      "}\n" ::"r"(bar),
-      "r"(parity)
-      : "memory");
-}
-// global -> shared bulk copy through the TMA unit (non-tensor form): bytes % 16 == 0, both addresses 16-byte aligned
-__device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst), "l"(src), "r"(bytes),
-               "r"(bar)
-               : "memory");
-}
-__device__ __forceinline__ unsigned long long lds64(uint32_t a) {
-  unsigned long long v;
-  asm volatile("ld.shared.b64 %0, [%1];" : "=l"(v) : "r"(a));
-  return v;
-}
-__device__ __forceinline__ uint32_t lds32(uint32_t a) {
-  uint32_t v;
-  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(a));
-  return v;
-}
-__device__ __forceinline__ uint32_t lds_u8(uint32_t a) {
-  uint32_t v;
-  asm volatile("ld.shared.u8 %0, [%1];" : "=r"(v) : "r"(a));
-  return v;
-}
-__device__ __forceinline__ uint32_t lds_u16(uint32_t a) {
-  uint32_t v;
-  asm volatile("ld.shared.u16 %0, [%1];" : "=r"(v) : "r"(a));
-  return v;
-}
 
 // Predicated shared-memory atomics (PTX-level predicates keep the row loop free of divergence regions).
 __device__ __forceinline__ void red_add_shared_if(uint32_t addr, uint32_t v, bool p) {
@@ -382,7 +331,7 @@ __global__ void __launch_bounds__(kTaThreads, 1) k_tile_agg(const __grid_constan
                 const uint32_t cb = slot_s + poff[p];
 #pragma unroll
                 for (int j = 0; j < RB; j++) {
-                  const uint32_t code = psh[p] == 0 ? lds_u8(cb + r[j]) : (psh[p] == 1 ? lds_u16(cb + r[j] * 2u) : lds32(cb + r[j] * 4u));
+                  const uint32_t code = psh[p] == 0 ? lds8(cb + r[j]) : (psh[p] == 1 ? lds16(cb + r[j] * 2u) : lds32(cb + r[j] * 4u));
                   const bool isnull = pbias[p] == 0u && code == 0u;
                   const uint32_t id = isnull ? 0u : code + pbias[p] - 1u;
                   const bool pass = isnull ? (d.pred_null[p] != 0) : (__ldg(plut[p] + id) != 0);
@@ -404,10 +353,10 @@ __global__ void __launch_bounds__(kTaThreads, 1) k_tile_agg(const __grid_constan
               const uint32_t cb = slot_s + koff[k];
               if (K8 || ksh[k] == 0) {
 #pragma unroll
-                for (int j = 0; j < RB; j++) slot[j] += (lds_u8(cb + r[j]) + kbias[k]) * kstride[k];
+                for (int j = 0; j < RB; j++) slot[j] += (lds8(cb + r[j]) + kbias[k]) * kstride[k];
               } else if (ksh[k] == 1) {
 #pragma unroll
-                for (int j = 0; j < RB; j++) slot[j] += (lds_u16(cb + r[j] * 2u) + kbias[k]) * kstride[k];
+                for (int j = 0; j < RB; j++) slot[j] += (lds16(cb + r[j] * 2u) + kbias[k]) * kstride[k];
               } else {
 #pragma unroll
                 for (int j = 0; j < RB; j++) slot[j] += (lds32(cb + r[j] * 4u) + kbias[k]) * kstride[k];
@@ -559,13 +508,8 @@ cudaError_t launch_tile_agg(const TileAggDesc& d, int sm_count, cudaStream_t st)
     if (d.smem_table) kern = simple ? k_tile_agg<true, true, -1, -1, false, false> : k_tile_agg<true, false, -1, -1, false, false>;
     else kern = simple ? k_tile_agg<false, true, -1, -1, false, false> : k_tile_agg<false, false, -1, -1, false, false>;
   }
-  static std::unordered_map<const void*, size_t> configured;  // (guarded by the engine's mutex)
-  size_t& cfg = configured[reinterpret_cast<const void*>(kern)];
-  if (smem > cfg) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
-    if (e != cudaSuccess) return e;
-    cfg = smem;
-  }
+  const cudaError_t e = kernel_smem_at_least(reinterpret_cast<const void*>(kern), smem);
+  if (e != cudaSuccess) return e;
   uint32_t grid = uint32_t(sm_count);
   const uint32_t need = (d.n_tiles + d.chunk_tiles - 1) / d.chunk_tiles;
   if (grid > need) grid = need;
