@@ -127,12 +127,18 @@ struct ProgOp {
   int64_t imm;  // PO_CONST: int64 or the bits of a double
 };
 
+// Unique(int64) is two stored cells, a Min then a Max of the same column, in which a NULL row counts as INT64_MIN and as
+// INT64_MAX: the group's value is the one both cells hold, NULL when they differ (aggregate.go:677-730).  Every reducer,
+// merge and exchange treats them as the Min and Max they are; only the scan's input and the finalize read `unique`.
+enum UniqueCell : uint8_t { UC_NONE = 0, UC_LO = 1, UC_HI = 2 };
+
 struct AggDesc {
-  uint8_t func;      // logicalplan.AggFunc value
+  uint8_t func;      // logicalplan.AggFunc value (a Unique cell: Min or Max)
   uint8_t is_float;  // expression evaluates in float64
   uint8_t prog_off;
   uint8_t prog_len;
-  uint32_t _pad;
+  uint8_t unique;    // UniqueCell; the UC_HI cell directly follows its UC_LO cell
+  uint8_t _pad[3];
 };
 
 enum TableMode : int32_t { TM_DENSE = 0, TM_HASH = 1 };
@@ -531,6 +537,7 @@ struct DenseOut {
   unsigned long long seq, bytes, timeout_ns;
   unsigned long long* err;              // the query's counters[3]: 1 timeout, 2 table shapes differ
   uint8_t agg_func[kMaxAggs], agg_is_float[kMaxAggs];
+  uint8_t agg_unique[kMaxAggs];         // UniqueCell: a UC_HI cell's column holds the validity bytes of its UC_LO cell's
   int8_t agg_pos[kMaxAggs];             // index among the stored aggregates, -1: Count (= rows)
   uint32_t* hdr;  // 256 bytes of device memory, zero between launches (see k_finalize_dense)
   uint8_t* out;   // device or page-locked host memory: [header 256 B: count u32 @0, counters u64 x4 @32, any_null u32 per key @64][n_keys x max_out u32 (8-byte aligned)][n_aggs x max_out i64]
@@ -572,6 +579,7 @@ struct FinalizeDesc {
   long long* out_aggs;  // [n_aggs][max_out]
   unsigned long long* out_rows;  // [max_out]
   unsigned int* out_count;
+  uint8_t agg_unique[kMaxAggs];  // as DenseOut::agg_unique
 };
 
 }  // namespace fgpu

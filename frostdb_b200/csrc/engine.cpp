@@ -76,6 +76,7 @@ const char* agg_string(int f) {  // logicalplan.AggFunc.String(), expr.go:731-75
     case FGPU_AGG_MAX: return "max";
     case FGPU_AGG_COUNT: return "count";
     case FGPU_AGG_AVG: return "avg";
+    case FGPU_AGG_UNIQUE: return "unique";
     default: return "?";
   }
 }
@@ -424,6 +425,11 @@ struct Compiled {
   uint64_t touched_rows = ~uint64_t(0);  // rows of the row groups that survive pruning (~0: nothing was pruned)
   uint32_t radix(int k) const { return dense_radix[size_t(k)] ? dense_radix[size_t(k)] : 1; }  // (int64 keys have none)
   bool has_bool_keys() const { return !key_leaves.empty(); }  // (every boolean key has a leaf)
+  bool has_unique() const {  // a Unique aggregate: only k_scan's general path feeds its cells the NULL rows
+    for (int a = 0; a < qd.n_aggs; a++)
+      if (qd.aggs[a].unique) return true;
+    return false;
+  }
 };
 
 // A boolean expression -> postfix program over its leaves, appended to *leaves and *prog.  `other`: leaves of the plan
@@ -1061,17 +1067,26 @@ bool in_every_row_group(const QueryPlan& q, int node, const std::vector<VisibleR
 int32_t compile_aggregates(const QueryPlan& q, const std::map<std::string, int>& slot_of, Compiled* c, std::vector<ProgOp>* prog) {
   QueryDesc& qd = c->qd;
   if (q.aggs.size() > size_t(kMaxAggs)) return fail(FGPU_ERR_UNSUPPORTED, "too many aggregates");
-  qd.n_aggs = int32_t(q.aggs.size());
-  for (size_t a = 0; a < q.aggs.size(); a++) {
-    AggDesc& ad = qd.aggs[a];
+  size_t cells = 0;  // stored cells and Counts: a Unique takes two (see UniqueCell)
+  for (const fgpu_agg& g : q.aggs) cells += g.func == FGPU_AGG_UNIQUE ? 2 : 1;
+  if (cells > size_t(kMaxAggs)) return fail(FGPU_ERR_UNSUPPORTED, "too many aggregates");
+  qd.n_aggs = int32_t(cells);
+  for (size_t a = 0, cell = 0; a < q.aggs.size(); a++) {
+    AggDesc& ad = qd.aggs[cell];
     int f = q.aggs[a].func;
-    if (f != FGPU_AGG_SUM && f != FGPU_AGG_MIN && f != FGPU_AGG_MAX && f != FGPU_AGG_COUNT)
+    if (f != FGPU_AGG_SUM && f != FGPU_AGG_MIN && f != FGPU_AGG_MAX && f != FGPU_AGG_COUNT && f != FGPU_AGG_UNIQUE)
       return fail(FGPU_ERR_UNSUPPORTED, std::string("aggregate function not supported on the GPU path: ") + agg_string(f));
-    ad.func = uint8_t(f);
+    const bool unique = f == FGPU_AGG_UNIQUE;
+    // a NULL row decides a Unique, and expressions do not track NULLs
+    if (unique && q.exprs[size_t(q.aggs[a].expr)].kind != FGPU_EXPR_COLUMN)
+      return fail(FGPU_ERR_UNSUPPORTED, "unique over an expression is not supported on the GPU path");
+    ad.func = uint8_t(unique ? FGPU_AGG_MIN : f);
     bool any_float = false, any_int_col = false;
     size_t off = prog->size();
     int32_t rc = compile_agg_expr(q, q.aggs[a].expr, slot_of, *c, prog, &any_float, &any_int_col);
     if (rc) return rc;
+    // the reference refuses Unique over float64 when it executes: the caller keeps the plan on its own operators
+    if (unique && any_float) return fail(FGPU_ERR_UNSUPPORTED, "unique is defined for int64 columns only");
     if (any_float && any_int_col) return fail(FGPU_ERR_UNSUPPORTED, "arithmetic mixes int64 and float64 columns");
     if (any_float) {  // integer literals take part as doubles
       for (size_t p = off; p < prog->size(); p++)
@@ -1087,11 +1102,18 @@ int32_t compile_aggregates(const QueryPlan& q, const std::map<std::string, int>&
     std::string missing;
     if (!in_every_row_group(q, q.aggs[a].expr, c->rgs, &missing))
       return fail(FGPU_ERR_NOT_FOUND, "aggregate field(s) not found [\"" + missing + "\"], aggregations are not possible without it");
+    if (unique) {  // the Min cell, then the Max cell over the same program
+      ad.unique = UC_LO;
+      qd.aggs[cell + 1] = ad;
+      qd.aggs[cell + 1].func = FGPU_AGG_MAX;
+      qd.aggs[cell + 1].unique = UC_HI;
+    }
+    cell += unique ? 2 : 1;
   }
   // every aggregate's columns are looked up before any program is sized or its depth checked
   if (prog->size() > size_t(kMaxProg)) return fail(FGPU_ERR_UNSUPPORTED, "aggregate expressions too large");
   for (size_t p = 0; p < prog->size(); p++) qd.prog[p] = (*prog)[p];
-  for (size_t a = 0; a < q.aggs.size(); a++)
+  for (int a = 0; a < qd.n_aggs; a++)
     if (prog_depth(*prog, qd.aggs[a].prog_off, qd.aggs[a].prog_len) > 3)
       return fail(FGPU_ERR_UNSUPPORTED, "aggregate expression nests too deeply for the GPU path");
   return FGPU_OK;
@@ -1219,7 +1241,7 @@ bool plain_load(const QueryDesc& qd, int a) { return qd.aggs[a].prog_len == 1 &&
 // fused fast path of k_scan: conjunction of numeric leaves, dense dictionary keys, simple aggregates
 bool fast_path_ok(const Compiled& c, const Switches& w) {
   const QueryDesc& qd = c.qd;
-  if (w.no_fast || c.has_bool_keys() || qd.table_mode != TM_DENSE || (qd.n_filter_prog != 0 && qd.filter_kind != FK_AND) ||
+  if (w.no_fast || c.has_bool_keys() || c.has_unique() || qd.table_mode != TM_DENSE || (qd.n_filter_prog != 0 && qd.filter_kind != FK_AND) ||
       qd.n_leaves > 2 || qd.n_keys > 3)
     return false;
   for (int l = 0; l < qd.n_leaves; l++) {
@@ -1748,7 +1770,7 @@ struct RunsPlan {
 // Dense keys (up to kRunsKeys), a conjunction of int64 range leaves and of dictionary leaves (evaluated once per run),
 // up to kRunsAggs Sum / Min / Max of plain columns.
 bool runs_query(const Compiled& c, const QueryDesc& qd, const Switches& w, RunsPlan* P) {
-  if (w.no_fast || w.no_runs || c.has_bool_keys() || qd.table_mode != TM_DENSE || (qd.n_filter_prog != 0 && qd.filter_kind != FK_AND) ||
+  if (w.no_fast || w.no_runs || c.has_bool_keys() || c.has_unique() || qd.table_mode != TM_DENSE || (qd.n_filter_prog != 0 && qd.filter_kind != FK_AND) ||
       qd.n_keys > kRunsKeys || qd.n_leaves > kRunsLeaves + kRunsPreds)
     return false;
   RunsDesc& rd = P->rd;
@@ -1881,7 +1903,7 @@ struct PrefixBuilt {
 };
 
 bool prefix_query(const Compiled& c, const RunsPlan& R, const Switches& w) {
-  if (w.no_prefix || c.has_bool_keys()) return false;
+  if (w.no_prefix || c.has_bool_keys() || c.has_unique()) return false;
   for (int a = 0; a < R.na; a++)
     if (R.rd.agg_func[a] != uint32_t(FGPU_AGG_SUM)) return false;  // Min / Max / float64 Sum stay with k_runs_tma
   return true;
@@ -2079,7 +2101,7 @@ struct TilePlan {
 };
 
 bool tile_query(const Compiled& c, const QueryDesc& qd, const Switches& w, TilePlan* T) {
-  if (w.no_tile || c.has_bool_keys() || qd.table_mode != TM_DENSE || (qd.n_filter_prog != 0 && qd.filter_kind != FK_AND) || qd.n_keys > kTaKeys)
+  if (w.no_tile || c.has_bool_keys() || c.has_unique() || qd.table_mode != TM_DENSE || (qd.n_filter_prog != 0 && qd.filter_kind != FK_AND) || qd.n_keys > kTaKeys)
     return false;
   TileAggDesc& td = T->td;
   auto plain_of = [&](int slot) { return find_or_add(T->plain_slot, &td.n_plain, kTaPlain, slot); };
@@ -2384,10 +2406,11 @@ ResultShape result_shape(const QueryPlan& q, const Compiled& c) {
       k.dict = nullptr;
     }
   }
-  for (size_t a = 0; a < q.aggs.size(); a++) {
+  for (size_t a = 0, cell = 0; a < q.aggs.size(); a++) {
     r.agg_names.push_back(std::string(agg_string(q.aggs[a].func)) + "(" + q.expr_name(q.aggs[a].expr) + ")");
-    // Count yields int64; Sum/Min/Max keep the input type (aggregate.go:734-950)
-    r.agg_is_float.push_back(c.qd.aggs[a].func != FGPU_AGG_COUNT && c.qd.aggs[a].is_float);
+    // Count yields int64; Sum/Min/Max keep the input type (aggregate.go:734-950); Unique is int64 only
+    r.agg_is_float.push_back(c.qd.aggs[cell].func != FGPU_AGG_COUNT && c.qd.aggs[cell].is_float);
+    cell += c.qd.aggs[cell].unique ? 2 : 1;
   }
   return r;
 }
@@ -2416,6 +2439,7 @@ int32_t keep_exec_cache(fgpu_ctx* ctx, const QueryPlan& q, Compiled& c, const Qu
     for (int a = 0; a < qd.n_aggs; a++) {
       f.agg_func[a] = qd.aggs[a].func;
       f.agg_is_float[a] = qd.aggs[a].is_float;
+      f.agg_unique[a] = qd.aggs[a].unique;
       f.agg_pos[a] = qd.aggs[a].func == FGPU_AGG_COUNT ? int8_t(-1) : int8_t(pos++);
     }
   }
@@ -2469,6 +2493,7 @@ FinalizeDesc finalize_desc(const Compiled& c, const QueryDesc& qd) {
     fd.keys[k] = qd.keys[k];
     fd.dense_radix[k] = c.radix(k);
   }
+  for (int a = 0; a < qd.n_aggs; a++) fd.agg_unique[a] = qd.aggs[a].unique;
   bind_finalize(&fd, qd);
   return fd;
 }
@@ -2746,15 +2771,17 @@ int32_t finalize_dense_host(fgpu_result* res, ExecCache& x) {
     cols.push_back(std::move(col));
   }
   const uint8_t* aggs = img + 256 + size_t(nk) * key_bytes;
-  for (int a = 0; a < na; a++) {
+  for (int a = 0, o = 0; a < na; a++) {
+    if (qd.aggs[a].unique == UC_HI) continue;  // the validity of the Unique before it
     OwnedColumn col;
-    col.name = x.shape.agg_names[size_t(a)];
-    col.format = x.shape.agg_is_float[size_t(a)] ? "g" : "l";
+    col.name = x.shape.agg_names[size_t(o)];
+    col.format = x.shape.agg_is_float[size_t(o++)] ? "g" : "l";
     col.length = int64_t(G);
     if (G > 0) {
       col.ext = aggs + size_t(a) * x.dout.max_out * 8;
       col.ext_keep = keep;
     }
+    if (qd.aggs[a].unique == UC_LO) validity_from_bytes(col, aggs + size_t(a + 1) * x.dout.max_out * 8, G);
     cols.push_back(std::move(col));
   }
   res->stats.algorithmic_bytes += (size_t(nk) + size_t(na)) * G * 8;
@@ -2873,10 +2900,12 @@ int32_t finalize_result(fgpu_ctx* ctx, fgpu_result* res) {
 
   // ---- build Arrow columns (aggregate.go:551-625: group columns first, then aggregates) --------
   std::vector<OwnedColumn> cols;
-  for (int c = 0; c < nk + na; c++) {
+  for (int c = 0, o = 0; c < nk + na; c++) {
     const bool key = c < nk;
+    const uint8_t unique = key ? UC_NONE : res->qd.aggs[c - nk].unique;
+    if (unique == UC_HI) continue;  // the validity of the Unique before it
     OwnedColumn col;
-    col.name = key ? res->shape.keys[size_t(c)].name : res->shape.agg_names[size_t(c - nk)];
+    col.name = key ? res->shape.keys[size_t(c)].name : res->shape.agg_names[size_t(o)];
     col.length = int64_t(G);
     if (key && res->shape.keys[size_t(c)].is_bool) {  // codes (1 false, 2 true) packed into bits in place
       bool_key_column(col, reinterpret_cast<long long*>(blocks[size_t(c)].get()), G);
@@ -2888,12 +2917,14 @@ int32_t finalize_result(fgpu_ctx* ctx, fgpu_result* res) {
       dict_key_column(col, reinterpret_cast<const long long*>(blocks[size_t(c)].get()), G, nullptr, res->shape.keys[size_t(c)].dict_snapshot,
                       KeyDict::kUsed);
     } else {
-      col.format = !key && res->shape.agg_is_float[size_t(c - nk)] ? "g" : "l";
+      col.format = !key && res->shape.agg_is_float[size_t(o)] ? "g" : "l";
+      if (unique == UC_LO) validity_from_bytes(col, blocks[size_t(c + 1)].get(), G);
       if (G) {
         col.ext = blocks[size_t(c)].get();
         col.ext_keep = std::move(blocks[size_t(c)]).keep();
       }
     }
+    o += key ? 0 : 1;
     cols.push_back(std::move(col));
   }
   res->stats.algorithmic_bytes += (size_t(nk) + size_t(na)) * G * 8;

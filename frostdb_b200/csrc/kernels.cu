@@ -1076,6 +1076,7 @@ __device__ __noinline__ void vec_aggregate(const VecCtx& v, uint8_t* wb, int a, 
     if (simple) {
       bool null;
       val = rd.next(v.r0 + uint32_t(s) * 32 + lane, v.n_rows, null);  // every step: the cursor must see all rows
+      if (null && ad.unique) val = ad.unique == UC_LO ? (long long)0x8000000000000000ull : 0x7fffffffffffffffll;  // (other aggregates read 0)
     } else {
       val = m.tmp1[s * 32 + lane];
     }
@@ -1926,8 +1927,16 @@ __global__ void k_finalize(FinalizeDesc f) {
       }
       f.out_keys[size_t(k) * f.max_out + o] = code;
     }
-    for (int a = 0; a < f.n_aggs; a++)
-      f.out_aggs[size_t(a) * f.max_out + o] = f.t_agg[a] ? f.t_agg[a][s] : (long long)rows;
+    for (int a = 0; a < f.n_aggs; a++) {
+      const long long v = f.t_agg[a] ? f.t_agg[a][s] : (long long)rows;
+      if (f.agg_unique[a] == UC_HI) {  // Unique: the value where both cells meet, else NULL (0); this column: validity bytes
+        const long long lo = f.t_agg[a - 1][s];
+        f.out_aggs[size_t(a - 1) * f.max_out + o] = lo == v ? lo : 0;
+        reinterpret_cast<uint8_t*>(f.out_aggs + size_t(a) * f.max_out)[o] = lo == v;
+      } else {
+        f.out_aggs[size_t(a) * f.max_out + o] = v;
+      }
+    }
   }
 }
 
@@ -2157,6 +2166,7 @@ __global__ void __launch_bounds__(256) k_finalize_dense(DenseOut f) {
       if (!code) hdr[16 + k] = 1u;
     }
     long long* aggs = reinterpret_cast<long long*>(f.out + 256 + size_t(f.n_keys) * key_bytes);
+    long long lo = 0;  // a Unique's UC_LO cell, written with its UC_HI cell (f.out may be page-locked: never read back)
     for (uint32_t a = 0; a < f.n_aggs; a++) {
       long long v;
       if (f.n_src > 0) {
@@ -2172,7 +2182,14 @@ __global__ void __launch_bounds__(256) k_finalize_dense(DenseOut f) {
       } else {
         v = f.t_agg[a] ? f.t_agg[a][s] : (long long)rows;
       }
-      aggs[size_t(a) * f.max_out + o] = v;
+      if (f.agg_unique[a] == UC_LO) {
+        lo = v;
+      } else if (f.agg_unique[a] == UC_HI) {  // as k_finalize: the value, or NULL (0) with a 0 validity byte in this column
+        aggs[size_t(a - 1) * f.max_out + o] = lo == v ? lo : 0;
+        reinterpret_cast<uint8_t*>(aggs + size_t(a) * f.max_out)[o] = lo == v;
+      } else {
+        aggs[size_t(a) * f.max_out + o] = v;
+      }
     }
   }
   __shared__ bool last;

@@ -24,7 +24,9 @@ _OP_STR = {OpEq: "==", OpNotEq: "!=", OpLt: "<", OpLtEq: "<=", OpGt: ">", OpGtEq
            OpContains: "contains", OpNotContains: "not contains"}
 
 AggFuncSum, AggFuncMin, AggFuncMax, AggFuncCount, AggFuncAvg = _lib.AGG_SUM, _lib.AGG_MIN, _lib.AGG_MAX, _lib.AGG_COUNT, _lib.AGG_AVG
-_AGG_STR = {AggFuncSum: "sum", AggFuncMin: "min", AggFuncMax: "max", AggFuncCount: "count", AggFuncAvg: "avg"}
+AggFuncUnique = _lib.AGG_UNIQUE
+_AGG_STR = {AggFuncSum: "sum", AggFuncMin: "min", AggFuncMax: "max", AggFuncCount: "count", AggFuncAvg: "avg",
+            AggFuncUnique: "unique"}
 
 
 class Expr:
@@ -167,6 +169,7 @@ def Min(e: Expr): return AggregationFunction(AggFuncMin, e)
 def Max(e: Expr): return AggregationFunction(AggFuncMax, e)
 def Count(e: Expr): return AggregationFunction(AggFuncCount, e)
 def Avg(e: Expr): return AggregationFunction(AggFuncAvg, e)
+def Unique(e: Expr): return AggregationFunction(AggFuncUnique, e)
 
 
 # ---- logical plan nodes (logicalplan.go:17-29) ----------------------------------------------------

@@ -132,7 +132,7 @@ typedef struct fgpu_expr { /* one node of a logicalplan.Expr tree, children by i
 } fgpu_expr;
 
 typedef struct fgpu_agg { /* logicalplan.AggregationFunction{Func, Expr}                         */
-  int32_t func; /* FGPU_AGG_SUM/MIN/MAX/COUNT                                                    */
+  int32_t func; /* FGPU_AGG_SUM/MIN/MAX/COUNT, FGPU_AGG_UNIQUE over a plain int64 column          */
   int32_t expr; /* index of the aggregated expression (COLUMN or arithmetic BINARY)              */
 } fgpu_agg;
 
