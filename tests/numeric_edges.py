@@ -626,7 +626,8 @@ def same_value(got, exp, func: int) -> bool:
 
 
 def assert_same_result(got: dict, exp: dict, aggs: Sequence[lp.AggregationFunction], what: str = "") -> None:
-    assert set(got) == set(exp), f"{what}: groups differ: only engine {sorted(set(got) - set(exp))[:5]}, only reference {sorted(set(exp) - set(got))[:5]}"
+    # (sorted by repr: a NULL key is None, which does not order against strings)
+    assert set(got) == set(exp), f"{what}: groups differ: only engine {sorted(set(got) - set(exp), key=repr)[:5]}, only reference {sorted(set(exp) - set(got), key=repr)[:5]}"
     for k, ev in exp.items():
         gv = got[k]
         for a, g, e in zip(aggs, gv, ev):
