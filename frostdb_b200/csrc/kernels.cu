@@ -17,6 +17,11 @@
 //   k_merge      K6: folds gathered partial tables into the local one (Synchronizer + final
 //                HashAggregate, synchronize.go:16-53, physicalplan.go:438-471).
 //   k_decode     K1 standalone: one column chunk -> dense buffers.
+//   k_flatten    dictionary column chunk -> flat code array for the tile kernel (tile_agg.cu).
+//
+// Every general kernel (k_scan, k_rows, k_decode, k_flatten) reads the hybrid streams of a column chunk through one
+// pair of readers, DictReader and NumReader, 32 rows per step from the per-128-row seeds: k_scan seeds them from its
+// vector's ring slot, the others from the chunk's global seeds.
 //
 // HBM-bound integer / indexing work: no tensor cores.  k_scan is a vectorized engine: every warp owns
 // vectors of 512 rows, prefetches the vector's PLAIN column slices and hybrid-stream seeds into a
@@ -45,8 +50,7 @@ namespace {
 constexpr int NT = kScanThreads;     // threads per CTA
 constexpr int NWARP = NT / 32;       // warps per CTA = chunks per tile
 constexpr int STEPS = kIndexRows / 32;  // 32-row steps per chunk
-constexpr int TILE = kTileRows;
-static_assert(NWARP * kIndexRows == TILE, "tile = one chunk per warp");
+static_assert(NWARP * kIndexRows == kTileRows, "k_rows: tile = one chunk per warp");
 static_assert(STEPS == 4, "unrolled for 4 steps");
 
 constexpr uint32_t kNoSlot = 0xffffffffu;
@@ -104,139 +108,6 @@ __device__ __forceinline__ uint32_t hc_get(HybCur& c, uint32_t ord) {
   return c.lut ? __ldg(c.lut + v) : v;
 }
 
-// Seeds of the chunk's streams: staged copies in shared memory when the producer provided them.
-struct ChunkSeeds {
-  const Seed* val;  // value stream seed of this chunk (shared or global), nullptr when the column has none
-  const Seed* def;  // definition-level stream seed
-};
-__device__ __forceinline__ ChunkSeeds global_seeds(const ChunkDesc& c, uint32_t chunk) {
-  ChunkSeeds s;
-  s.val = (c.kind == CK_DICT_STR || c.kind == CK_DICT64) ? c.seeds + chunk : nullptr;
-  s.def = c.has_nulls ? c.def_seeds + chunk : nullptr;
-  return s;
-}
-
-// Decodes the chunk's STEPS x 32 rows of a dictionary-encoded string column: gid[j] = GLOBAL dictionary
-// id of row (c0 + 32 j + lane), kNullIdx for NULL / out of range / absent column.
-__device__ __forceinline__ void decode_dict_chunk(const ChunkDesc& c, const ChunkSeeds& sd, uint32_t c0, uint32_t n_rows, int lane,
-                                                  uint32_t (&gid)[STEPS]) {
-  if (c.kind == CK_ABSENT) {
-#pragma unroll
-    for (int j = 0; j < STEPS; j++) gid[j] = kNullIdx;
-    return;
-  }
-  const uint32_t lt = (1u << lane) - 1u;
-  HybCur vc, dc;
-  uint32_t vbase = c0;
-  const bool nulls = c.has_nulls;
-  if (nulls) vbase = hc_init(dc, c.def_runs, c.def, nullptr, sd.def);
-  hc_init(vc, c.runs, c.values, c.lut, sd.val);
-#pragma unroll
-  for (int j = 0; j < STEPS; j++) {
-    uint32_t r = c0 + j * 32 + lane;
-    bool valid = r < n_rows;
-    uint32_t ord = r;
-    if (nulls) {
-      if (valid) valid = hc_get(dc, r) != 0;
-      unsigned m = __ballot_sync(FULL, valid);
-      ord = vbase + __popc(m & lt);
-      vbase += __popc(m);
-    }
-    gid[j] = valid ? hc_get(vc, ord) : kNullIdx;
-  }
-}
-
-// Decodes the chunk's rows of a numeric column: bits[j] raw 8 bytes (0 for NULL, as
-// builder.AppendValue leaves NULL slots: pqarrow/builder/utils.go:54-58, optbuilders.go:337-340),
-// nullmask bit j set when the row is NULL / absent / out of range.  `staged` is the tile's slice of a
-// PLAIN column in shared memory (indexed by row - tile_r0) or nullptr.
-__device__ __forceinline__ void decode_num_chunk(const ChunkDesc& c, const ChunkSeeds& sd, const long long* staged, uint32_t tile_r0,
-                                                 uint32_t c0, uint32_t n_rows, int lane, long long (&bits)[STEPS], uint32_t& nullmask) {
-  nullmask = 0;
-  if (c.kind == CK_ABSENT) {
-#pragma unroll
-    for (int j = 0; j < STEPS; j++) bits[j] = 0;
-    nullmask = (1u << STEPS) - 1u;
-    return;
-  }
-  const long long* vals = reinterpret_cast<const long long*>(c.values);
-  if (c.kind == CK_PLAIN64 && !c.has_nulls) {
-#pragma unroll
-    for (int j = 0; j < STEPS; j++) {
-      uint32_t r = c0 + j * 32 + lane;
-      bool inb = r < n_rows;
-      long long v = 0;
-      if (inb) v = staged ? staged[r - tile_r0] : __ldg(vals + r);
-      bits[j] = v;
-      if (!inb) nullmask |= 1u << j;
-    }
-    return;
-  }
-  const uint32_t lt = (1u << lane) - 1u;
-  HybCur vc, dc;
-  uint32_t vbase = c0;
-  const bool nulls = c.has_nulls;
-  if (nulls) vbase = hc_init(dc, c.def_runs, c.def, nullptr, sd.def);
-  const bool dict = c.kind == CK_DICT64;
-  if (dict) hc_init(vc, c.runs, c.values, nullptr, sd.val);
-#pragma unroll
-  for (int j = 0; j < STEPS; j++) {
-    uint32_t r = c0 + j * 32 + lane;
-    bool valid = r < n_rows;
-    uint32_t ord = r;
-    if (nulls) {
-      if (valid) valid = hc_get(dc, r) != 0;
-      unsigned m = __ballot_sync(FULL, valid);
-      ord = vbase + __popc(m & lt);
-      vbase += __popc(m);
-    }
-    long long v = 0;
-    if (valid) v = dict ? __ldg(&c.dict64[hc_get(vc, ord)]) : __ldg(vals + ord);
-    bits[j] = v;
-    if (!valid) nullmask |= 1u << j;
-  }
-}
-
-// What the consumer knows about the tile it is working on.
-struct TileCtx {
-  const QueryDesc* q;
-  const ChunkDesc* chunks;  // [n_slots] of the row group
-  const LeafRt* lrt;        // [n_leaves] of the row group
-  const uint8_t* stage;     // shared-memory stage of this tile (nullptr: nothing staged, read HBM)
-  uint32_t tile_r0;         // first row of the tile inside the row group
-  uint32_t chunk;           // this warp's chunk index inside the row group
-  uint32_t chunk_in_tile;
-  uint32_t c0;              // first row of the chunk
-  uint32_t n_rows;          // rows of the row group
-};
-__device__ __forceinline__ size_t stage_plain_bytes() { return size_t(TILE) * 8; }
-__device__ __forceinline__ size_t stage_seed_bytes() { return size_t(NWARP) * sizeof(Seed); }
-__device__ __forceinline__ const long long* staged_plain(const TileCtx& t, int slot) {
-  if (!t.stage) return nullptr;
-  int p = t.q->slot_plain_stage[slot];
-  if (p < 0) return nullptr;
-  const ChunkDesc& c = t.chunks[slot];
-  if (c.kind != CK_PLAIN64 || c.has_nulls) return nullptr;
-  return reinterpret_cast<const long long*>(t.stage + size_t(p) * stage_plain_bytes());
-}
-__device__ __forceinline__ ChunkSeeds seeds_for(const TileCtx& t, int slot) {
-  const ChunkDesc& c = t.chunks[slot];
-  ChunkSeeds s = global_seeds(c, t.chunk);
-  if (t.stage) {
-    const uint8_t* base = t.stage + size_t(t.q->n_stage_plain) * stage_plain_bytes();
-    int sv = t.q->slot_seed_stage[slot][0], sdf = t.q->slot_seed_stage[slot][1];
-    if (s.val && sv >= 0) s.val = reinterpret_cast<const Seed*>(base + size_t(sv) * stage_seed_bytes()) + t.chunk_in_tile;
-    if (s.def && sdf >= 0) s.def = reinterpret_cast<const Seed*>(base + size_t(sdf) * stage_seed_bytes()) + t.chunk_in_tile;
-  }
-  return s;
-}
-__device__ __forceinline__ void tile_dict(const TileCtx& t, int slot, int lane, uint32_t (&gid)[STEPS]) {
-  decode_dict_chunk(t.chunks[slot], seeds_for(t, slot), t.c0, t.n_rows, lane, gid);
-}
-__device__ __forceinline__ void tile_num(const TileCtx& t, int slot, int lane, long long (&bits)[STEPS], uint32_t& nullmask) {
-  decode_num_chunk(t.chunks[slot], seeds_for(t, slot), staged_plain(t, slot), t.tile_r0, t.c0, t.n_rows, lane, bits, nullmask);
-}
-
 // ---- predicate --------------------------------------------------------------------------------------------
 // Canonical numeric leaf: value inside [lo, hi] (inclusive), optionally negated.  NaN is never inside.
 __device__ __forceinline__ bool leaf_range(const LeafDesc& ld, long long bits, bool f64col) {
@@ -250,7 +121,7 @@ __device__ __forceinline__ bool leaf_range(const LeafDesc& ld, long long bits, b
   return in != (ld.neg != 0);
 }
 
-// A boolean key's postfix program over its leaf bits (0..31 push leaf; 0x80 AND; 0x81 OR), as eval_filter runs the filter's.
+// A postfix program over leaf bits (0..31 push leaf; 0x80 AND; 0x81 OR): the filter's and each boolean key's.
 __device__ __forceinline__ bool eval_postfix(const uint8_t* prog, int n, uint32_t bits) {
   uint32_t stack = 0;  // stack kept in a 32-bit word
   int sp = 0;
@@ -273,87 +144,7 @@ __device__ __forceinline__ bool eval_postfix(const uint8_t* prog, int n, uint32_
 __device__ __forceinline__ bool eval_filter(const QueryDesc& q, uint32_t bits) {
   if (q.filter_kind == FK_AND) return (bits & q.filter_mask) == q.filter_mask;
   if (q.filter_kind == FK_OR) return (bits & q.filter_mask) != 0;
-  uint32_t stack = 0;  // postfix program over leaf bits; stack kept in a 32-bit word
-  int sp = 0;
-  for (int i = 0; i < q.n_filter_prog; i++) {
-    uint8_t op = q.filter_prog[i];
-    if (op < 0x80) {
-      stack = (stack & ~(1u << sp)) | (((bits >> op) & 1u) << sp);
-      sp++;
-    } else {
-      uint32_t b = (stack >> (sp - 1)) & 1u, a = (stack >> (sp - 2)) & 1u;
-      uint32_t r = (op == 0x80) ? (a & b) : (a | b);
-      sp -= 2;
-      stack = (stack & ~(1u << sp)) | (r << sp);
-      sp++;
-    }
-  }
-  return stack & 1u;
-}
-
-// Evaluates every predicate leaf of the chunk: leafbits[j] bit l = leaf l selects row j.
-// NULL semantics: binaryscalarexpr.go:143-150 (numeric NULL never selected), :165-172,:205-212
-// (dictionary == NULL / != NULL), missing columns :47-73 (LM_ALL / LM_NONE precomputed on the host).
-__device__ __forceinline__ void eval_leaves(const TileCtx& t, int lane, uint32_t (&leafbits)[STEPS]) {
-  const QueryDesc& q = *t.q;
-  const LeafRt* __restrict__ lrt = t.lrt;
-  uint32_t cbits = 0;
-  for (int l = 0; l < q.n_leaves; l++)
-    if (lrt[l].mode == LM_ALL) cbits |= 1u << l;
-#pragma unroll
-  for (int j = 0; j < STEPS; j++) leafbits[j] = cbits;
-  for (int slot = 0; slot < q.n_slots; slot++) {
-    if (!q.slot_used_by_leaf[slot]) continue;
-    if (q.slot_type[slot] == ST_DICT) {
-      uint32_t gid[STEPS];
-      tile_dict(t, slot, lane, gid);
-      for (int l = 0; l < q.n_leaves; l++) {
-        if (q.leaves[l].slot != slot || lrt[l].mode != LM_EVAL) continue;
-        const uint8_t* lut = lrt[l].lut;
-        const uint32_t nullres = lrt[l].null_result;
-#pragma unroll
-        for (int j = 0; j < STEPS; j++) {
-          uint32_t r = (gid[j] == kNullIdx) ? nullres : uint32_t(__ldg(lut + gid[j]));
-          leafbits[j] |= (r & 1u) << l;
-        }
-      }
-    } else {
-      long long bits[STEPS];
-      uint32_t nullmask;
-      tile_num(t, slot, lane, bits, nullmask);
-      const bool f64col = q.slot_type[slot] == ST_F64;
-      for (int l = 0; l < q.n_leaves; l++) {
-        const LeafDesc& ld = q.leaves[l];
-        if (ld.slot != slot || lrt[l].mode != LM_EVAL) continue;
-#pragma unroll
-        for (int j = 0; j < STEPS; j++) {
-          bool r = false;
-          if (!((nullmask >> j) & 1u)) {
-            r = leaf_range(ld, bits[j], f64col);
-          }
-          leafbits[j] |= uint32_t(r) << l;
-        }
-      }
-    }
-  }
-}
-
-// Selected rows of the chunk: bit j = this lane's row of step j passes the predicate.
-__device__ __forceinline__ uint32_t chunk_selection(const TileCtx& t, int lane) {
-  const QueryDesc& q = *t.q;
-  uint32_t actbits = 0;
-  if (q.n_filter_prog > 0) {
-    uint32_t leafbits[STEPS];
-    eval_leaves(t, lane, leafbits);
-#pragma unroll
-    for (int j = 0; j < STEPS; j++)
-      if (t.c0 + j * 32 + lane < t.n_rows && eval_filter(q, leafbits[j])) actbits |= 1u << j;
-  } else {
-#pragma unroll
-    for (int j = 0; j < STEPS; j++)
-      if (t.c0 + j * 32 + lane < t.n_rows) actbits |= 1u << j;
-  }
-  return actbits;
+  return eval_postfix(q.filter_prog, q.n_filter_prog, bits);
 }
 
 // ---- aggregate expressions ----------------------------------------------------------------------------------
@@ -552,6 +343,20 @@ struct DictReader {
     if (nulls) vbase = hc_init(dc, c.def_runs, c.def, nullptr, sd >= 0 ? reinterpret_cast<const Seed*>(seeds) + sd : c.def_seeds + v.chunk);
     hc_init(vc, c.runs, c.values, c.lut, sv >= 0 ? reinterpret_cast<const Seed*>(seeds) + sv : c.seeds + v.chunk);
   }
+  // Streams 128-row chunk `chunk` of c from its global seeds.  A second initialiser rather than a core shared with the
+  // one above: routing k_scan's through a shared core moves spills across k_scan's call graph.  It starts from a zeroed
+  // reader: a cursor the chunk's kind leaves unset would be read undefined across the unrolled steps of the kernels
+  // that use it, which keeps its registers live through the whole kernel (k_rows: 151 registers instead of 72).
+  __device__ __forceinline__ void init(const ChunkDesc& c, uint32_t chunk, int lane) {
+    *this = DictReader{};
+    absent = c.kind == CK_ABSENT;
+    nulls = !absent && c.has_nulls;
+    lt = (1u << lane) - 1u;
+    vbase = chunk * kIndexRows;
+    if (absent) return;
+    if (nulls) vbase = hc_init(dc, c.def_runs, c.def, nullptr, c.def_seeds + chunk);
+    hc_init(vc, c.runs, c.values, c.lut, c.seeds + chunk);
+  }
   // global dictionary id of row r (this lane's row of the current step), kNullIdx for NULL / out of range
   __device__ __forceinline__ uint32_t next(uint32_t r, uint32_t n_rows) {
     if (absent) return kNullIdx;
@@ -598,6 +403,22 @@ struct NumReader {
     const int sv = v.q->slot_seed_stage[slot][0], sd = v.q->slot_seed_stage[slot][1];
     if (nulls) vbase = hc_init(dc, c.def_runs, c.def, nullptr, sd >= 0 ? reinterpret_cast<const Seed*>(seeds) + sd : c.def_seeds + v.chunk);
     if (dict) hc_init(vc, c.runs, c.values, nullptr, sv >= 0 ? reinterpret_cast<const Seed*>(seeds) + sv : c.seeds + v.chunk);
+  }
+  // Streams 128-row chunk `chunk` of c from its global seeds, from a zeroed reader (see DictReader).
+  __device__ __forceinline__ void init(const ChunkDesc& c, uint32_t chunk, int lane) {
+    *this = NumReader{};
+    r0 = chunk * kIndexRows;
+    lt = (1u << lane) - 1u;
+    if (c.kind == CK_ABSENT) { mode = 0; return; }
+    vals = reinterpret_cast<const long long*>(c.values);
+    if (c.kind == CK_PLAIN64 && !c.has_nulls) { mode = 1; return; }
+    mode = 2;
+    nulls = c.has_nulls;
+    dict = c.kind == CK_DICT64;
+    dict64 = reinterpret_cast<const long long*>(c.dict64);
+    vbase = r0;
+    if (nulls) vbase = hc_init(dc, c.def_runs, c.def, nullptr, c.def_seeds + chunk);
+    if (dict) hc_init(vc, c.runs, c.values, nullptr, c.seeds + chunk);
   }
   __device__ __forceinline__ long long next(uint32_t r, uint32_t n_rows, bool& null) {
     if (mode == 1) {
@@ -1778,7 +1599,68 @@ __global__ void __launch_bounds__(kVecThreads, 4) k_scan(const QueryDesc* __rest
 // ======================================================================================================
 // k_rows: predicate + order-preserving compaction of the projected columns
 // ======================================================================================================
-__global__ void __launch_bounds__(NT) k_rows(const QueryDesc* __restrict__ qp) {
+// Selected rows of the warp's 128-row chunk: bit j = this lane's row of step j passes the predicate.  Every slot a
+// leaf reads is decoded once for all of its leaves into leafbits[j] (bit l = leaf l selects row j).
+// NULL semantics: binaryscalarexpr.go:143-150 (numeric NULL never selected), :165-172,:205-212
+// (dictionary == NULL / != NULL), missing columns :47-73 (LM_ALL / LM_NONE precomputed on the host).
+__device__ __forceinline__ uint32_t chunk_selection(const QueryDesc& q, const ChunkDesc* chunks, const LeafRt* __restrict__ lrt,
+                                                    uint32_t chunk, uint32_t n_rows, int lane) {
+  const uint32_t c0 = chunk * kIndexRows;
+  uint32_t actbits = 0;
+  if (q.n_filter_prog == 0) {
+#pragma unroll
+    for (int j = 0; j < STEPS; j++)
+      if (c0 + j * 32 + lane < n_rows) actbits |= 1u << j;
+    return actbits;
+  }
+  uint32_t cbits = 0;
+  for (int l = 0; l < q.n_leaves; l++)
+    if (lrt[l].mode == LM_ALL) cbits |= 1u << l;
+  uint32_t leafbits[STEPS];
+#pragma unroll
+  for (int j = 0; j < STEPS; j++) leafbits[j] = cbits;
+  for (int slot = 0; slot < q.n_slots; slot++) {
+    if (!q.slot_used_by_leaf[slot]) continue;
+    if (q.slot_type[slot] == ST_DICT) {
+      DictReader rd;
+      rd.init(chunks[slot], chunk, lane);
+      uint32_t gid[STEPS];
+#pragma unroll
+      for (int j = 0; j < STEPS; j++) gid[j] = rd.next(c0 + j * 32 + lane, n_rows);
+      for (int l = 0; l < q.n_leaves; l++) {
+        if (q.leaves[l].slot != slot || lrt[l].mode != LM_EVAL) continue;
+        const uint8_t* lut = lrt[l].lut;
+        const uint32_t nullres = lrt[l].null_result;
+#pragma unroll
+        for (int j = 0; j < STEPS; j++) {
+          uint32_t r = (gid[j] == kNullIdx) ? nullres : uint32_t(__ldg(lut + gid[j]));
+          leafbits[j] |= (r & 1u) << l;
+        }
+      }
+    } else {
+      NumReader rd;
+      rd.init(chunks[slot], chunk, lane);
+      long long bits[STEPS];
+      bool null[STEPS];
+#pragma unroll
+      for (int j = 0; j < STEPS; j++) bits[j] = rd.next(c0 + j * 32 + lane, n_rows, null[j]);
+      const bool f64col = q.slot_type[slot] == ST_F64;
+      for (int l = 0; l < q.n_leaves; l++) {
+        const LeafDesc& ld = q.leaves[l];
+        if (ld.slot != slot || lrt[l].mode != LM_EVAL) continue;
+#pragma unroll
+        for (int j = 0; j < STEPS; j++) leafbits[j] |= uint32_t(!null[j] && leaf_range(ld, bits[j], f64col)) << l;
+      }
+    }
+  }
+#pragma unroll
+  for (int j = 0; j < STEPS; j++)
+    if (c0 + j * 32 + lane < n_rows && eval_filter(q, leafbits[j])) actbits |= 1u << j;
+  return actbits;
+}
+
+// At least two CTAs per SM: without a minimum, ptxas spills registers to fit four.
+__global__ void __launch_bounds__(NT, 2) k_rows(const QueryDesc* __restrict__ qp) {
   __shared__ QueryDesc sq;
   __shared__ uint32_t warp_cnt[NWARP];
   __shared__ unsigned long long tile_base_s;
@@ -1802,19 +1684,12 @@ __global__ void __launch_bounds__(NT) k_rows(const QueryDesc* __restrict__ qp) {
     if (tile >= q.n_tiles) break;
     const int rg = find_rg(q.rg_first_tile, q.n_rg, tile);
     const uint32_t tile_in_rg = tile - __ldg(&q.rg_first_tile[rg]);
-    TileCtx t;
-    t.q = &q;
-    t.n_rows = __ldg(&q.rg_rows[rg]);
-    t.tile_r0 = tile_in_rg * TILE;
-    t.chunk_in_tile = uint32_t(warp);
-    t.chunk = tile_in_rg * NWARP + warp;
-    t.c0 = t.chunk * kIndexRows;
-    t.chunks = q.chunks + size_t(rg) * q.n_slots;
-    t.lrt = q.leaf_rt + size_t(rg) * q.n_leaves;
-    t.stage = nullptr;
+    const uint32_t n_rows = __ldg(&q.rg_rows[rg]);
+    const uint32_t chunk = tile_in_rg * NWARP + warp, c0 = chunk * kIndexRows;
+    const ChunkDesc* chunks = q.chunks + size_t(rg) * q.n_slots;
 
     uint32_t actbits = 0;
-    if (t.c0 < t.n_rows) actbits = chunk_selection(t, lane);
+    if (c0 < n_rows) actbits = chunk_selection(q, chunks, q.leaf_rt + size_t(rg) * q.n_leaves, chunk, n_rows, lane);
     // rank of every selected row inside the warp's chunk, in row order
     uint32_t rank[STEPS];
     uint32_t wtotal = 0;
@@ -1858,28 +1733,32 @@ __global__ void __launch_bounds__(NT) k_rows(const QueryDesc* __restrict__ qp) {
     __syncthreads();
     const unsigned long long base = tile_base_s + wbase;
     // ---- write the projected columns of the selected rows ---------------------------------------
-    if (t.c0 < t.n_rows && wtotal > 0) {
+    if (c0 < n_rows && wtotal > 0) {
       for (int o = 0; o < q.n_out; o++) {
         const int slot = q.out_slot[o];
         if (q.slot_type[slot] == ST_DICT) {
-          uint32_t gid[STEPS];
-          tile_dict(t, slot, lane, gid);
+          DictReader rd;
+          rd.init(chunks[slot], chunk, lane);
           int32_t* out = reinterpret_cast<int32_t*>(q.out_data[o]);
 #pragma unroll
-          for (int j = 0; j < STEPS; j++)
-            if ((actbits >> j) & 1u) out[base + rank[j]] = (gid[j] == kNullIdx) ? -1 : int32_t(gid[j]);
+          for (int j = 0; j < STEPS; j++) {
+            const uint32_t gid = rd.next(c0 + j * 32 + lane, n_rows);
+            if ((actbits >> j) & 1u) out[base + rank[j]] = (gid == kNullIdx) ? -1 : int32_t(gid);
+          }
         } else {
-          long long v[STEPS];
-          uint32_t nm;
-          tile_num(t, slot, lane, v, nm);
+          NumReader rd;
+          rd.init(chunks[slot], chunk, lane);
           long long* out = reinterpret_cast<long long*>(q.out_data[o]);
           uint8_t* valid = q.out_valid[o];
 #pragma unroll
-          for (int j = 0; j < STEPS; j++)
+          for (int j = 0; j < STEPS; j++) {
+            bool null;
+            const long long v = rd.next(c0 + j * 32 + lane, n_rows, null);
             if ((actbits >> j) & 1u) {
-              out[base + rank[j]] = v[j];
-              valid[base + rank[j]] = ((nm >> j) & 1u) ? 0 : 1;
+              out[base + rank[j]] = v;
+              valid[base + rank[j]] = null ? 0 : 1;
             }
+          }
         }
       }
     }
@@ -1987,25 +1866,30 @@ __global__ void __launch_bounds__(NT) k_decode(ChunkDesc c, uint32_t n_chunks, i
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   for (uint32_t chunk = blockIdx.x * NWARP + warp; chunk < n_chunks; chunk += gridDim.x * NWARP) {
     const uint32_t c0 = chunk * kIndexRows;
-    const ChunkSeeds sd = global_seeds(c, chunk);
     if (c.kind == CK_DICT_STR) {
+      DictReader rd;
+      rd.init(c, chunk, lane);
       uint32_t gid[STEPS];
-      decode_dict_chunk(c, sd, c0, c.n_rows, lane, gid);
+#pragma unroll
+      for (int j = 0; j < STEPS; j++) gid[j] = rd.next(c0 + j * 32 + lane, c.n_rows);
 #pragma unroll
       for (int j = 0; j < STEPS; j++) {
-        uint32_t r = c0 + j * 32 + lane;
+        const uint32_t r = c0 + j * 32 + lane;
         if (r < c.n_rows) out_i32[r] = (gid[j] == kNullIdx) ? -1 : int32_t(gid[j]);
       }
     } else {
+      NumReader rd;
+      rd.init(c, chunk, lane);
       long long v[STEPS];
-      uint32_t nm;
-      decode_num_chunk(c, sd, nullptr, 0, c0, c.n_rows, lane, v, nm);
+      bool null[STEPS];
+#pragma unroll
+      for (int j = 0; j < STEPS; j++) v[j] = rd.next(c0 + j * 32 + lane, c.n_rows, null[j]);
 #pragma unroll
       for (int j = 0; j < STEPS; j++) {
-        uint32_t r = c0 + j * 32 + lane;
+        const uint32_t r = c0 + j * 32 + lane;
         if (r < c.n_rows) {
           out_i64[r] = v[j];
-          out_valid[r] = ((nm >> j) & 1u) ? 0 : 1;
+          out_valid[r] = null[j] ? 0 : 1;
         }
       }
     }
@@ -2281,6 +2165,17 @@ cudaError_t launch_make_seeds(void* image, uint64_t jobs_off, uint32_t n_jobs, u
   return cudaGetLastError();
 }
 
+// Index of the last job whose first_block <= blk (jobs ascending by first_block).
+template <typename Job>
+__device__ __forceinline__ uint32_t job_of_block(const Job* jobs, uint32_t n_jobs, uint32_t blk) {
+  uint32_t lo = 0, hi = n_jobs;
+  while (hi - lo > 1) {
+    const uint32_t mid = (lo + hi) >> 1;
+    if (__ldg(&jobs[mid].first_block) <= blk) lo = mid; else hi = mid;
+  }
+  return lo;
+}
+
 // ======================================================================================================
 // k_flatten: dictionary column chunk -> flat code array (one warp per 128-row block).
 //   code = global dictionary id (+ 1 when the chunk has NULLs, 0 = NULL), w = 8, 16 or 32 bits per row.
@@ -2290,15 +2185,13 @@ cudaError_t launch_make_seeds(void* image, uint64_t jobs_off, uint32_t n_jobs, u
 __global__ void __launch_bounds__(NT) k_flatten(const FlatJob* __restrict__ jobs, uint32_t n_jobs, uint32_t total_blocks) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   for (uint32_t blk = blockIdx.x * NWARP + warp; blk < total_blocks; blk += gridDim.x * NWARP) {
-    uint32_t lo = 0, hi = n_jobs;  // last job with first_block <= blk
-    while (hi - lo > 1) {
-      const uint32_t mid = (lo + hi) >> 1;
-      if (__ldg(&jobs[mid].first_block) <= blk) lo = mid; else hi = mid;
-    }
-    const FlatJob& J = jobs[lo];
+    const FlatJob& J = jobs[job_of_block(jobs, n_jobs, blk)];
     const uint32_t chunk = blk - J.first_block, c0 = chunk * kIndexRows, w = J.w;
+    DictReader rd;
+    rd.init(J.chunk, chunk, lane);
     uint32_t gid[STEPS];
-    decode_dict_chunk(J.chunk, global_seeds(J.chunk, chunk), c0, J.chunk.n_rows, lane, gid);
+#pragma unroll
+    for (int j = 0; j < STEPS; j++) gid[j] = rd.next(c0 + j * 32 + lane, J.chunk.n_rows);
 #pragma unroll
     for (int j = 0; j < STEPS; j++) {
       const uint32_t code = (gid[j] == kNullIdx) ? 0u : gid[j] + 1u - J.bias;  // rows past the end: 0 (padding)
@@ -2328,20 +2221,11 @@ cudaError_t launch_flatten(const FlatJob* d_jobs, uint32_t n_jobs, uint32_t tota
 //                   block sums before it).
 // One CTA per kNarrowRows-row block of one job.
 // ======================================================================================================
-__device__ __forceinline__ uint32_t narrow_job(const NarrowJob* jobs, uint32_t n_jobs, uint32_t blk) {
-  uint32_t lo = 0, hi = n_jobs;  // last job with first_block <= blk
-  while (hi - lo > 1) {
-    const uint32_t mid = (lo + hi) >> 1;
-    if (__ldg(&jobs[mid].first_block) <= blk) lo = mid; else hi = mid;
-  }
-  return lo;
-}
-
 __global__ void __launch_bounds__(NT) k_chunk_minmax(const NarrowJob* __restrict__ jobs, uint32_t n_jobs, long long* mm,
                                                      unsigned long long* bsum) {
   __shared__ long long s_lo[NWARP], s_hi[NWARP];
   __shared__ unsigned long long s_sum[NWARP];
-  const uint32_t j = narrow_job(jobs, n_jobs, blockIdx.x);
+  const uint32_t j = job_of_block(jobs, n_jobs, blockIdx.x);
   const NarrowJob& J = jobs[j];
   const uint32_t r0 = (blockIdx.x - J.first_block) * kNarrowRows, r1 = min(J.n_rows, r0 + kNarrowRows);
   long long lo = LLONG_MAX, hi = LLONG_MIN;
@@ -2399,7 +2283,7 @@ __device__ __forceinline__ unsigned long long cta_exclusive_sum(unsigned long lo
 
 __global__ void __launch_bounds__(NT) k_narrow(const NarrowJob* __restrict__ jobs, uint32_t n_jobs, const unsigned long long* __restrict__ bsum) {
   __shared__ unsigned long long s_warp[NWARP];
-  const NarrowJob& J = jobs[narrow_job(jobs, n_jobs, blockIdx.x)];
+  const NarrowJob& J = jobs[job_of_block(jobs, n_jobs, blockIdx.x)];
   const uint32_t blk = blockIdx.x - J.first_block;
   const uint32_t r0 = blk * kNarrowRows, r1 = min(J.n_rows, r0 + kNarrowRows), w = J.w;
   const unsigned long long base = (unsigned long long)J.base;

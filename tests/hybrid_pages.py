@@ -454,6 +454,8 @@ class Reference:
             return np.ones(self.n, bool)
         if filt.Op == lp.OpAnd:
             return self.mask(filt.Left) & self.mask(filt.Right)
+        if filt.Op == lp.OpOr:
+            return self.mask(filt.Left) | self.mask(filt.Right)
         name, op, lit = filt.Left.Name(), filt.Op, filt.Right.Value
         if name in self.str_cols:
             codes, d = self.str_cols[name]

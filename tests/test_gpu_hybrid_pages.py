@@ -223,10 +223,14 @@ def test_filter_only_rows_on_the_take_kernels_and_k_rows(store, zoo, refs, name)
 
 @pytest.mark.parametrize("name", [l.name for l in hp.LAYOUTS if not l.error])
 def test_filter_only_rows_with_dictionary_outputs(zoo, refs, name):
-    """Projecting labels.z and the nullable dictvalue: k_rows decodes both through HybCur."""
+    """Projecting labels.z and the nullable dictvalue: k_rows decodes both through HybCur.  Besides the aggregate plans'
+    filters, a general filter program with two leaves on dictvalue."""
     layout = hp.LAYOUT_BY_NAME[name]
     db, made = zoo
     ref = reference(refs, name)
     filters = {f.Name(): f for f, _, _ in hp.plans(layout) if f is not None}
+    dv, z = lp.Col("dictvalue"), lp.Col("labels.z")
+    program = lp.And(lp.Or(dv.Lt(lp.Literal(2)), dv.Gt(lp.Literal(5))), z.NotEq(lp.Literal(hp.zoo_literal(layout))))
+    filters[program.Name()] = program
     for filt in filters.values():
         check_rows(db, made[(name, "eager")], ref, filt, ["labels.z", "value", "dictvalue"], f"{name} {filt.Name()}")
